@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- contract benchmark of the FO1 hot path on N B200s (one rank per GPU).
+"""bench.py -- benchmark of the FO1 hot path on N H100s (one rank per GPU).
 
 Workload (BASELINE.json configs[2], the configuration the headline metric is quoted on): per GPU a batch of 32
 synthetic 896x896 images, 64 boxes each, random-init 3B FO1 weights: dual vision towers (ViT + DaViT) -> SimpleFPN ->
@@ -10,11 +10,11 @@ fixed), one NCCL all-gather of the decoded ids per step.  A "step" is one pass o
   e2e   : the same through the public pipeline API from pinned HOST buffers: H2D of the raw uint8 images and the boxes,
           device-side pre-processing (bicubic smart-resize, normalise, patchify for both towers) and D2H of the token ids,
           all inside the timed region.
-  roofline     : the dominant kernel (tcgen05 GEMM) -- algorithmic FLOPs / CUDA-event launch time (one extra
-                 instrumented step after the timed region) vs the measured cuBLAS bf16 sustained peak.
-  roofline_hfre: HFRE gather -- SURVEY 8d algorithmic bytes / launch time vs the measured HBM copy bandwidth.
+  roofline     : the dominant kernel (wgmma GEMM) -- algorithmic FLOPs / CUDA-event launch time (one extra
+                 instrumented step after the timed region) vs the bf16 tensor peak (MEASURED_PEAKS.json if present, else the H100 SXM data sheet).
+  roofline_hfre: HFRE gather -- SURVEY 8d algorithmic bytes / launch time vs the HBM bandwidth (same source).
   roofline_decode: one decode step -- bytes it must stream (bf16 weights + the live K/V) / its device time vs HBM.
-  cpu_baseline : the reference's OWN modules (oracle/reference_path.py over the copy in baseline/_ref/, ``kind: "reference"``)
+  cpu_baseline : the reference's OWN modules (oracle/reference_path.py over the copy in oracle/_ref/, ``kind: "reference"``)
                  timed on the host cores on ONE full-depth image with a shortened decode (stated in ``sample``); the oracle
                  port (``kind: "port"``) only if that copy is absent.
 ``--impl reference`` times that CPU arm alone: one full-depth image per step, all decode tokens, every host thread.
@@ -22,7 +22,11 @@ fixed), one NCCL all-gather of the decoded ids per step.  A "step" is one pass o
 Workloads (``--workload``): c3 (default, the headline configuration), c4 (COCO shape: 640 px -> 46x46 grid, 100 boxes,
 16 images / GPU), c5 (counting: 1344 px, 300 boxes, 128 tokens, 8 images / GPU), c2 (HFRE-only: towers + region tokens of
 8 x 896 px x 100 boxes; value = GB/s of the HFRE operator).  ``--global-batch G`` fixes the TOTAL batch and splits it over
-the ranks (strong scaling) instead of the per-GPU batch (weak scaling)."""
+the ranks (strong scaling) instead of the per-GPU batch (weak scaling).
+
+``--dump-outputs DIR`` writes what the last timed step returned to its caller (the decoded token ids and their lengths; the region
+tokens for c2) as float32 ``DIR/<name>.npy``.  Inputs and weights are seeded, so two builds run with the same arguments can be
+compared output for output."""
 import argparse
 import json
 import os
@@ -53,11 +57,11 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], tflops=d.get("bf16_tflops_sustained", d["bf16_tflops"]), source="measured")
-    return dict(hbm_gbs=6650.0, tflops=1400.0, source="fallback")
+    return dict(hbm_gbs=3350.0, tflops=989.0, source="H100 SXM data sheet")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region."""
 
     def __init__(self, index: int):
         self.proc = None
@@ -107,7 +111,7 @@ class ClockSampler:
 
 def reference_arm(args, cfg, steps, decode_tokens, warm=0):
     """The CPU arm: ONE image per step through the reference's own modules (oracle/reference_path.py; the oracle port if
-    baseline/_ref is absent), fp32, FULL depth, on the host cores this process owns (affinity + cgroup quota: with every logical CPU of
+    oracle/_ref is absent), fp32, FULL depth, on the host cores this process owns (affinity + cgroup quota: with every logical CPU of
     the box the OpenMP pool of a quota-limited container thrashes -- 455 s per image instead of ~45 s).  ``decode_tokens`` < args.tokens
     shortens the greedy loop; the remaining steps are then added at the measured per-token cost (the note says so).  --cpu-sample swaps the
     full depth for a bounded depth sample (8 of 32 ViT blocks, 4 of 36 decoder layers, DaViT stage 3 at 3 of 9) scaled to full depth.
@@ -142,7 +146,7 @@ def reference_arm(args, cfg, steps, decode_tokens, warm=0):
             total = t["total_s"] + (T - dt) * per_tok
             t["llm_decode_s_per_token"] = per_tok
             times.append(total); detail = t
-        what = ("the reference's own modules (baseline/_ref copy of vlm_fo1: Qwen2_5_VisionTransformerPretrainedModel + custom_forward + "
+        what = ("the reference's own modules (oracle/_ref copy of vlm_fo1: Qwen2_5_VisionTransformerPretrainedModel + custom_forward + "
                 f"GATHER, DaViT, HFREModule incl. SimpleFP, mm_projector_aux, Qwen2_5_VLDecoderLayer; "
                 f"attention '{rp.attn}'), model loop / splice / greedy loop restated")
     else:
@@ -159,7 +163,7 @@ def reference_arm(args, cfg, steps, decode_tokens, warm=0):
             per_tok = t.get("llm_decode_s_per_token", 0.0)
             total = t["vit_s"] + t["davit_s"] + t["fpn_s"] + t["hfre_s"] + t["proj_s"] + t["llm_prefill_s"] + (T - 1) * per_tok
             times.append(total); detail = t
-        what = "oracle/pipeline.py (the CPU restatement of the reference; baseline/_ref is absent on this machine)"
+        what = "oracle/pipeline.py (the CPU restatement of the reference; oracle/_ref is absent on this machine)"
     note = (f"1 image per step, {args.size}x{args.size}, {args.boxes} boxes, {depth_note} (ViT {cfg.vit['depth']} blocks, DaViT "
             f"{cfg.davit['depths']}, LLM {cfg.llm['num_hidden_layers']} layers), fp32, {cores} host threads, through {what}; "
             + (f"all {T} decode tokens executed" if dt >= T else
@@ -185,16 +189,6 @@ def hfre_algorithmic_bytes(HF, cfg, host, size):
     return tot
 
 
-def load_traffic(workload: str, per_gpu_batch: int):
-    """DRAM bytes per launch of the roofline kernels from the committed ncu capture of this round (profiles/): the bench
-    cannot run under ncu, so `traffic` is read from the capture of the same command -- one C3 step at 32 images per GPU
-    (profiles/r02_ncu_dram_step.csv).  Any other workload / batch launches other shapes: no figure (null) rather than a wrong one."""
-    p = os.path.join(REPO, "profiles", "r02_traffic.json")
-    if workload != "c3" or per_gpu_batch != 32 or not os.path.exists(p):
-        return {}
-    return json.load(open(p))
-
-
 def main():
     out = _claim_stdout()
     ap = argparse.ArgumentParser()
@@ -212,6 +206,7 @@ def main():
     ap.add_argument("--cpu-sample", action="store_true", help="CPU legs run a bounded depth sample scaled to full depth instead of every block (~45 s per image)")
     ap.add_argument("--cpu-tokens", type=int, default=64, help="decode steps the in-run cpu_baseline executes (rest at the measured per-token time)")
     ap.add_argument("--profile-run", action="store_true", help="warm-up exactly as given, one timed pass, nothing else (for ncu)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the outputs of the last timed step as DIR/<name>.npy (float32)")
     ap.add_argument("--small", action="store_true", help="tiny architecture (plumbing check only; NOT a valid bench number)")
     args = ap.parse_args()
     wl = WORKLOADS[args.workload]
@@ -241,7 +236,7 @@ def main():
                           f"{args.boxes} boxes/img, {T}-token greedy decode, random-init 3B FO1 (variant B: SimpleFPN, D=5888, mlp2x_gelu projector)",
               "workload_id": args.workload, "global_batch": G, "per_gpu_batch": per_rank_max, "image_size": args.size,
               "boxes_per_image": args.boxes, "decode_tokens": T, "parallelism": f"dp{world}",
-              "l2_policy": "working set (8.3 GB weights + GBs of activations per step) >> 126 MB L2; no flush needed",
+              "l2_policy": "working set (8.3 GB weights + GBs of activations per step) >> 50 MB L2; no flush needed",
               "small_arch": bool(args.small)}
     metric, unit = (METRIC, UNIT) if not hfre_only else ("HFRE GB/s (SURVEY 8d unique bytes / fo1_hfre_forward time), dual-ViT forward + region tokens", "GB/s")
 
@@ -249,9 +244,8 @@ def main():
     if args.impl == "reference":
         if rank != 0:
             return
-        # bounded: a step is ONE full-depth image (~45 s on the 16 cores a box grants); one untimed warm-up step (if any was asked for)
-        # and at most two timed ones, so that any --steps K --warmup W ends within a few minutes of host time
-        steps = max(1, min(args.steps, 2))
+        # a step is ONE full-depth image (tens of seconds on 16 host cores); one untimed warm-up step (if any was asked for)
+        steps = max(1, args.steps)
         ips, kind, cores, note, detail = reference_arm(args, cfg, steps, min(args.cpu_tokens, max(T, 1)), warm=min(args.warmup, 1))
         value = ips
         if hfre_only:                                # the HFRE stage alone, same unit as the GPU arm
@@ -339,8 +333,18 @@ def main():
         step(resident)
     torch.cuda.synchronize()
     L.fo1_launch_count_reset()
+    last = {}
+
+    def timed_step():
+        last["res"] = step(resident)
+
     with ClockSampler(local) as cs:
-        ms = timed(lambda: step(resident), args.steps)
+        ms = timed(timed_step, args.steps)
+    if args.dump_outputs and rank == 0:
+        # what the caller of the step receives: the region tokens (c2) or every rank's decoded ids and lengths, gathered
+        res = last["res"]
+        dump_outputs(args.dump_outputs, {"region_tokens": res["region_tokens"]} if hfre_only else
+                     {"tokens": res["all_tokens"], "lens": res["all_lens"]})
     launches = int(L.fo1_launch_count())
     clocks = cs.summary()
     ips = G * args.steps / (ms / 1000.0)
@@ -359,7 +363,7 @@ def main():
     if rank == 0:
         # ---- extra instrumented steps (rank 0 only, no collective: the other ranks are already at the final barrier) ----
         peaks = load_peaks()
-        traffic = load_traffic(args.workload, B)
+        traffic = {}      # DRAM bytes per launch need a hardware-counter capture; none is kept for this GPU
         if hfre_only:
             local_step = lambda: pipe.encode(resident)
         else:
@@ -393,16 +397,16 @@ def main():
         roof_gemm = None
         if g and g["ms"] > 0:
             ach = g["flops"] / g["ms"] / 1e9
-            roof_gemm = {"kernel": "gemm_bf16_tcgen05_pair_kernel (CTA pairs, tcgen05.mma.cta_group::2; the few sub-wave problems: gemm_bf16_tcgen05_kernel), M > 128 launches of one step", "bound": "tensor", "achieved": ach,
+            roof_gemm = {"kernel": "gemm_bf16_wgmma_kernel, M > 128 launches of one step", "bound": "tensor", "achieved": ach,
                          "peak": peaks["tflops"], "unit": "TFLOP/s", "frac": ach / peaks["tflops"], "traffic": traffic.get("gemm_bytes_per_launch"),
-                         "peak_source": f"MEASURED_PEAKS.json bf16_tflops_sustained ({peaks['source']})",
+                         "peak_source": f"bf16 tensor peak ({peaks['source']})",
                          "launches": g["launches"], "ms_per_launch": g["ms"] / g["launches"], "share_of_step": g["ms"] / step_ms,
                          "algorithmic_bytes_per_launch": g["bytes"] / g["launches"]}
         for tag in ("attn", "attn_causal"):
             a = prof.get(tag)
             if a and a["ms"] > 0 and a["flops"] > 0:
                 ach = a["flops"] / a["ms"] / 1e9
-                line["roofline_" + tag] = {"kernel": "attn_tc_kernel (tcgen05 flash attention" + (", causal GQA prefill)" if tag == "attn_causal" else ", ViT / DaViT)"),
+                line["roofline_" + tag] = {"kernel": "attn_tc_kernel (wgmma flash attention" + (", causal GQA prefill)" if tag == "attn_causal" else ", ViT / DaViT)"),
                                            "bound": "tensor", "achieved": ach, "peak": peaks["tflops"], "unit": "TFLOP/s", "frac": ach / peaks["tflops"],
                                            "traffic": traffic.get(tag + "_bytes_per_launch"), "launches": a["launches"], "share_of_step": a["ms"] / step_ms}
         h = prof.get("hfre_sweep_mma") or prof.get("hfre_sweep") or prof.get("hfre_gather")
@@ -417,7 +421,7 @@ def main():
                          "algorithmic_bytes_per_launch": tot / h["launches"], "ms": h["ms"],
                          "operator_ms": stage, "operator_GBs": (tot / stage / 1e6) if stage else None,
                          "operator_frac": (tot / stage / 1e6 / peaks["hbm_gbs"]) if stage else None,
-                         "peak_source": f"MEASURED_PEAKS.json hbm_gbs ({peaks['source']})"}
+                         "peak_source": f"HBM bandwidth ({peaks['source']})"}
             line["roofline_hfre"] = roof_hfre
         if hfre_only and roof_hfre:
             # C2's metric IS the HFRE rate: value = whole operator (all its kernels), roofline = its sweep kernel
@@ -464,6 +468,20 @@ def main():
     if dist is not None:
         dist.barrier()
         dist.destroy_process_group()
+
+
+def dump_outputs(path, res, limit_bytes=64 << 20):
+    """``res[name]`` -> ``path/<name>.npy`` as float32.  An array that would push the total past ``limit_bytes`` is cut to a fixed,
+    seeded sample of its flattened elements."""
+    os.makedirs(path, exist_ok=True)
+    budget = limit_bytes
+    names = list(res)
+    for name in names:
+        a = res[name].detach().float().cpu().numpy()
+        if a.nbytes > budget // len(names):
+            idx = np.sort(np.random.default_rng(0).choice(a.size, size=budget // len(names) // 4, replace=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(path, name + ".npy"), np.ascontiguousarray(a, dtype=np.float32))
 
 
 def _claim_stdout():

@@ -1,5 +1,5 @@
 /*
- * fo1.h -- C ABI of libfo1.so, the B200 (sm_100a) engine for the VLM-FO1 inference hot path.
+ * fo1.h -- C ABI of libfo1.so, the H100 (sm_90a) engine for the VLM-FO1 inference hot path.
  *
  * Plain C types only: device pointers, sizes, a cudaStream_t passed as void*.  Every entry point
  * returns 0 on success or a negative fo1_status; fo1_last_error() returns a message for the calling
@@ -97,8 +97,8 @@ int fo1_hfre_forward(const fo1_hfre_image* images, int32_t n_images, const fo1_h
                      void* workspace, size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * Dense contraction: D[M,N] = epilogue(A[M,K] . W[N,K]^T) -- bf16 operands, fp32 accumulate in TMEM
- * (tcgen05.mma, operands staged by TMA).  Replaces every nn.Linear / 1x1 conv / patch-embed on the
+ * Dense contraction: D[M,N] = epilogue(A[M,K] . W[N,K]^T) -- bf16 operands, fp32 accumulate in registers
+ * (wgmma, operands staged by TMA).  Replaces every nn.Linear / 1x1 conv / patch-embed on the
  * path (modeling_qwen2_5_vl.py:88-111, 176-177, 151-155, 731-734, 633-635; modeling_davit.py:62-66,
  * 157-158, 235-236; simple_fpn.py:143-175; multimodal_projector/builder.py:100-106).
  * ---------------------------------------------------------------------------------------------- */
@@ -131,7 +131,7 @@ int fo1_gemm_bf16(const fo1_gemm_desc* d, void* stream);
 /* ------------------------------------------------------------------------------------------------
  * Variable-length softmax attention over packed token rows (replaces flash_attn_varlen_func at
  * modeling_qwen2_5_vl.py:205 and _flash_attention_forward at :895, and DaViT's window attention
- * modeling_davit.py:261-268) on tcgen05 / TMEM with TMA-fed K/V rings.  q/k/v/o: bf16 rows with the given
+ * modeling_davit.py:261-268) on wgmma with TMA-fed K/V rings.  q/k/v/o: bf16 rows with the given
  * pitches (elements, multiples of 8; 16-byte aligned bases); head h of a row starts at h*head_dim.
  * cu_seqlens: device int32 [n_seqs+1]; total_rows = cu_seqlens[n_seqs] (the host passes it: it sizes the grid).
  * head_dim in {32, 64, 80, 128}.
@@ -151,7 +151,7 @@ int fo1_attention_varlen(const fo1_attn_desc* d, void* stream);
 /* DaViT channel-group attention (ChannelAttention.forward, modeling_davit.py:151-172) for n_images maps of n_tokens tokens:
  * qkv bf16 [n_images][n_tokens][3*channels] (q | k | v as the fused Linear emits them), groups * 32 == channels;
  * out bf16 [n_images][n_tokens][channels] = (softmax_c2((q N^-0.5)^T k) v^T)^T per group of 32 channels.  Both contractions
- * run on tcgen05 (the Gram over the token axis with MN-major operands straight from the TMA tiles); partial Grams of the
+ * run on wgmma (the Gram over the token axis with MN-major operands straight from the TMA tiles); partial Grams of the
  * token chunks live in `workspace` and are summed in a fixed order (bit-reproducible, no atomics). */
 size_t fo1_channel_attention_workspace_bytes(int32_t n_images, int32_t n_tokens, int32_t channels);
 int fo1_channel_attention(const void* qkv, int32_t n_images, int32_t n_tokens, int32_t channels, int32_t groups, void* out,

@@ -1,8 +1,8 @@
 """The FO1 hot path assembled from the REFERENCE'S OWN modules, on the CPU -- TEST / BASELINE INFRASTRUCTURE ONLY.
 
 ``bench.py --impl reference`` and the ``cpu_baseline`` leg time this (``kind: "reference"``).  The reference is a Python
-tree without packaging metadata, so ``__graft_entry__.build()`` copies its ``vlm_fo1`` package (Python files only) into the
-git-ignored ``baseline/_ref/`` where ``/root/reference`` exists; that directory travels to the GPU box with the snapshot.
+tree without packaging metadata, so ``stage_copy()`` (called by ``__graft_entry__.build()``) copies its ``vlm_fo1`` package
+(Python files only) into the git-ignored ``oracle/_ref/`` where a checkout of the reference is at hand (``FO1_REFERENCE_ROOT``).
 The modules are imported from there with the three shims of ``oracle/ref_shim.py`` (SURVEY.md section 8c):
 
   ViT + taps      Qwen2_5_VisionTransformerPretrainedModel + replace_qwen_vit_forward + GATHER   (qwen2_5_vl_encoder.py:86-158, 37-80)
@@ -27,11 +27,32 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 REPO = os.path.dirname(HERE)
-REF_COPY = os.path.join(REPO, "baseline", "_ref")
+REF_COPY = os.path.join(HERE, "_ref")
 
 
 def available() -> bool:
     return os.path.isdir(os.path.join(REF_COPY, "vlm_fo1", "model"))
+
+
+def stage_copy() -> bool:
+    """Copy the Python files of the reference's ``vlm_fo1`` package, and its demo caller ``inference.py`` (which
+    tests/test_gpu_boundary.py executes unmodified against this repo's ``vlm_fo1`` mirror), from the reference checkout
+    (``oracle/ref_shim.py``: REFERENCE_ROOT) into ``oracle/_ref/``.  Nothing from this copy is product code or tracked by git.
+    Returns whether a copy is in place afterwards."""
+    import shutil
+    try:
+        from . import ref_shim
+    except ImportError:
+        import ref_shim  # type: ignore
+    src = os.path.join(ref_shim.REFERENCE_ROOT, "vlm_fo1")
+    dst = os.path.join(REF_COPY, "vlm_fo1")
+    if not os.path.isdir(src) or os.path.abspath(src) == os.path.abspath(dst):
+        return available()
+    if os.path.isdir(dst):
+        shutil.rmtree(dst)
+    shutil.copytree(src, dst, ignore=lambda d, names: [n for n in names if not (n.endswith(".py") or os.path.isdir(os.path.join(d, n)))])
+    shutil.copy(os.path.join(os.path.dirname(src), "inference.py"), os.path.join(REF_COPY, "inference.py"))
+    return True
 
 
 def _fill_(mod: torch.nn.Module) -> None:

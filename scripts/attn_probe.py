@@ -9,7 +9,7 @@ from importlib import import_module
 import fo1_b200  # noqa
 ops = import_module("vlm-fo1_b200.ops")
 NCU = len(sys.argv) > 1 and sys.argv[1] == "ncu"
-PEAK = json.load(open(os.path.join(REPO, "MEASURED_PEAKS.json")))["bf16_tflops"] if os.path.exists(os.path.join(REPO, "MEASURED_PEAKS.json")) else 1590.0
+PEAK = json.load(open(os.path.join(REPO, "MEASURED_PEAKS.json")))["bf16_tflops"] if os.path.exists(os.path.join(REPO, "MEASURED_PEAKS.json")) else 989.0   # H100 SXM data sheet, dense bf16
 flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
 
 

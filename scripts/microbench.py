@@ -1,5 +1,5 @@
-"""Kernel micro-benchmarks on one B200 (CUDA-event timing, L2 flushed between iterations).
-Writes gpurun_out/microbench_<tag>.json.  Not the contract bench (bench.py)."""
+"""Kernel micro-benchmarks on one H100 (CUDA-event timing, L2 flushed between iterations).
+Writes bench_out/microbench_<tag>.json.  Not the headline benchmark (bench.py)."""
 import json
 import os
 import sys
@@ -17,7 +17,7 @@ import fo1_b200  # noqa: E402
 ops = import_module("vlm-fo1_b200.ops")
 H = import_module("vlm-fo1_b200.hfre")
 
-PEAKS = json.load(open(os.path.join(REPO, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(REPO, "MEASURED_PEAKS.json")) else {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}
+PEAKS = json.load(open(os.path.join(REPO, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(REPO, "MEASURED_PEAKS.json")) else {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}   # H100 SXM data sheet
 _flush = None
 
 
@@ -142,5 +142,5 @@ if __name__ == "__main__":
         bench_gemm(res)
     if "decode" in which:
         bench_decode_gemms(res)
-    os.makedirs(os.path.join(REPO, "gpurun_out"), exist_ok=True)
-    json.dump(res, open(os.path.join(REPO, "gpurun_out", f"microbench_{tag}.json"), "w"), indent=1)
+    os.makedirs(os.path.join(REPO, "bench_out"), exist_ok=True)
+    json.dump(res, open(os.path.join(REPO, "bench_out", f"microbench_{tag}.json"), "w"), indent=1)

@@ -4,7 +4,7 @@
 //   mode 1: mode 0 + two __syncthreads per 4 stages (the cross-warp reduction cadence)
 //   mode 2: per-warp rings fed by ONE cp.async.bulk per stage from a tile-contiguous copy (stage bytes = SB)
 //   mode 3: mode 2 + the two __syncthreads per tile
-// build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o scripts/probes/stream_probe scripts/probes/stream_probe.cu
+// build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o scripts/probes/stream_probe scripts/probes/stream_probe.cu
 #include <cstdio>
 #include <cstdint>
 #include <cstdlib>

@@ -1,7 +1,7 @@
-"""Tile-width / split-K sweep of the decode (M = batch) GEMMs on one B200.  Each configuration streams a ROTATION of
+"""Tile-width / split-K sweep of the decode (M = batch) GEMMs on one H100.  Each configuration streams a ROTATION of
 distinct weight matrices (> L2 in total, like the 36 layers of a decode step) captured in one CUDA graph, so the
 number is the steady-state back-to-back time per launch, not a cold single launch.
-Writes gpurun_out/sweep_skinny_<tag>.json."""
+Writes bench_out/sweep_skinny_<tag>.json."""
 import json
 import os
 import sys
@@ -77,5 +77,5 @@ if __name__ == "__main__":
     allr = []
     for n in names:
         allr += run(n, M)
-    os.makedirs(os.path.join(REPO, "gpurun_out"), exist_ok=True)
-    json.dump(allr, open(os.path.join(REPO, "gpurun_out", f"sweep_skinny_{tag}.json"), "w"), indent=1)
+    os.makedirs(os.path.join(REPO, "bench_out"), exist_ok=True)
+    json.dump(allr, open(os.path.join(REPO, "bench_out", f"sweep_skinny_{tag}.json"), "w"), indent=1)

@@ -1,4 +1,5 @@
-"""Load tests/golden/*.npz fixtures (weights are stored as bf16 bit patterns under 'w::<name>')."""
+"""Load tests/golden/*.npz fixtures (weights are stored as bf16 bit patterns under 'w::<name>').  A fixture too large for one file
+continues in <name>.part1.npz, <name>.part2.npz, ... (oracle/gen_golden.py: save)."""
 import json
 import os
 
@@ -9,9 +10,13 @@ GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
 def load(name):
-    z = np.load(os.path.join(GOLDEN, name + ".npz"))
+    z = dict(np.load(os.path.join(GOLDEN, name + ".npz")))
+    i = 1
+    while os.path.exists(os.path.join(GOLDEN, f"{name}.part{i}.npz")):
+        z.update(np.load(os.path.join(GOLDEN, f"{name}.part{i}.npz")))
+        i += 1
     sd, rest = {}, {}
-    for k in z.files:
+    for k in z:
         if k.startswith("w::"):
             sd[k[3:]] = torch.from_numpy(z[k].copy()).view(torch.bfloat16).float()
         elif k == "cfg_json":

@@ -60,7 +60,7 @@ def test_attention_varlen(hd, qh, kvh, causal, lens):
 
 
 def test_attention_large_logits_rescale():
-    """Rows whose running maximum keeps growing (keys sorted by increasing score) force the lazy O rescale in TMEM on every
+    """Rows whose running maximum keeps growing (keys sorted by increasing score) force the lazy O rescale (in registers) on every
     key tile; a peaked softmax (logit range ~ 60) must still match fp32."""
     from importlib import import_module
     import fo1_b200  # noqa: F401

@@ -57,16 +57,16 @@ def test_inference_py_call_sequence(tmp_path):
 
 
 def test_reference_inference_py_runs_unmodified(tmp_path, monkeypatch):
-    """The reference's own ``inference.py`` FILE (staged byte-for-byte into baseline/_ref/ by __graft_entry__.build()), executed
+    """The reference's own ``inference.py`` FILE (staged byte-for-byte into oracle/_ref/ by __graft_entry__.build()), executed
     with runpy from a working directory laid out like the reference's (./resources/<checkpoint>, ./demo/demo_image.jpg) with
     this repo first on sys.path, so that its imports resolve to the repo's ``vlm_fo1`` / ``detect_tools`` mirror.  No statement
     of the script is re-typed here; max_tokens stays at the script's 4096 (a random-init model never emits <|im_end|>)."""
     import runpy
     import sys
     REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    script = os.path.join(REPO, "baseline", "_ref", "inference.py")
+    script = os.path.join(REPO, "oracle", "_ref", "inference.py")
     if not os.path.exists(script):
-        pytest.skip("baseline/_ref/inference.py not staged (build() copies it where /root/reference exists)")
+        pytest.skip("oracle/_ref/inference.py not staged (build() copies it where a reference checkout exists)")
     from importlib import import_module
     import fo1_b200  # noqa: F401
     E = import_module("vlm-fo1_b200.engine"); FB = import_module("vlm-fo1_b200.fabricate")

@@ -1,4 +1,4 @@
-"""-m gpu: DaViT channel-group attention (tcgen05 Gram over the token axis + tcgen05 mixing of v) vs a plain torch fp32 statement of
+"""-m gpu: DaViT channel-group attention (wgmma Gram over the token axis + wgmma mixing of v) vs a plain torch fp32 statement of
 ChannelAttention.forward (modeling_davit.py:151-172), at the DaViT-large stage shapes, ragged token counts, channel counts that
 are not a multiple of the 128-channel CTA tile, several token chunks (partial Grams summed in fixed order) and batch slots."""
 import pytest

@@ -1,7 +1,7 @@
 """-m gpu: the persistent decode kernel (csrc/decode_mega.cu: the whole greedy loop as one cooperative launch) against the
 per-kernel decode path it replaces (FO1_NO_MEGA=1: CUDA graph of the per-layer kernels) and against itself:
-  * same tokens as the per-kernel path wherever that path's own top-1 / top-2 margin is not a near-tie (two different
-    summation orders of the same bf16 data), at the 3B widths, ragged prompt lengths, several batch sizes (1 / 2 / 4 / 8 key
+  * same tokens as the per-kernel path wherever the top-1 / top-2 margin is not a near-tie (two different summation orders of
+    the same bf16 data): at the first step where a sequence differs the two candidates' logits are measured, at the 3B widths, ragged prompt lengths, several batch sizes (1 / 2 / 4 / 8 key
     splits per (sequence, kv head));
   * bit-reproducible run to run and independent of the batch slot; stop ids / padding / lens handled like the reference loop."""
 import os
@@ -19,6 +19,9 @@ def _mega_up_to_32(monkeypatch):
     monkeypatch.setenv("FO1_MEGA_MAX_B", "32")
 
 
+NEAR_TIE = 1.0 / 32     # of the standard deviation of a row of logits
+
+
 def _engine(layers=2, vocab=32000):
     from importlib import import_module
     import fo1_b200  # noqa: F401
@@ -31,7 +34,7 @@ def _engine(layers=2, vocab=32000):
     eng = E.Engine(cfg)
     eng.set_weights(W.prepare_llm(sd, cfg.llm, eng.device))
     eng.finalize()
-    return eng
+    return eng, sd
 
 
 def _batch(lens, seed=0):
@@ -41,9 +44,32 @@ def _batch(lens, seed=0):
     return torch.cat(embs).cuda(), torch.cat(pos, dim=1).contiguous(), [0] * len(lens)
 
 
+def _divergences(eng, sd, emb, lens, a, b):
+    """For every sequence whose two token rows differ: (sequence, first differing step t, gap, lead, std).  The prefix up to t is
+    common to both paths, so it is scored once more, teacher-forced, as a prompt (the prefill's fp32 logits at its last position):
+    ``gap`` = |logit of one candidate - logit of the other|, ``lead`` = how far the better of the two candidates lies below the best
+    logit of the whole vocabulary, ``std`` = the spread of that row of logits."""
+    table = sd["embed_tokens.weight"]
+    starts = [0]
+    for L in lens:
+        starts.append(starts[-1] + L)
+    found = []
+    for i in range(len(lens)):
+        if torch.equal(a[i], b[i]):
+            continue
+        t = int((a[i] != b[i]).nonzero()[0])
+        prefix = torch.cat([emb[starts[i]:starts[i + 1]], table[a[i, :t].long().cuda()].to(torch.bfloat16)])
+        n = prefix.shape[0]
+        pos = torch.arange(n, dtype=torch.int32).view(1, -1).expand(3, -1).contiguous()
+        lg = eng.generate(prefix, pos, [n], [0], 1, stop_ids=[], pad_id=0, want_prefill_logits=True, early_exit_interval=0)["prefill_logits"][0].float().cpu()
+        la, lb = float(lg[int(a[i, t])]), float(lg[int(b[i, t])])
+        found.append((i, t, abs(la - lb), float(lg.max()) - max(la, lb), float(lg.std())))
+    return found
+
+
 @pytest.mark.parametrize("lens", [[300, 517, 64, 1, 129], [700] * 2 + [33] * 14, [257] * 32, [1195]])
 def test_mega_matches_per_kernel_path(lens):
-    eng = _engine()
+    eng, sd = _engine()
     emb, pos, deltas = _batch(lens)
     T = 10
     out = eng.generate(emb, pos, lens, deltas, T, stop_ids=[], pad_id=0, early_exit_interval=0)
@@ -61,13 +87,19 @@ def test_mega_matches_per_kernel_path(lens):
     # a sequence may part ways at a near-tie of its logits (then the prefixes differ and later tokens are not comparable):
     # count sequences that agree on every token; with random-init weights most do
     same = sum(int(torch.equal(a[i], b[i])) for i in range(len(lens)))
-    first_diff = [int((a[i] != b[i]).nonzero()[0]) if not torch.equal(a[i], b[i]) else T for i in range(len(lens))]
-    assert same >= int(0.6 * len(lens)) and min(first_diff) >= 3, (same, first_diff)
+    assert same >= int(0.6 * len(lens)), same
+    # ... and where one parts ways, it must BE a near-tie: the two candidates, scored once more on the common prefix, are the top
+    # of the vocabulary and closer to each other than NEAR_TIE of the logits' spread.  Summing the same bf16 data in another order
+    # moves a logit by about a hundredth of that spread (hidden states re-round at 2^-9 relative per storage point; on H100 the
+    # gaps found at such positions were 0.2 .. 2.4 % of it), while the best two of 32000 unrelated logits lie about a fifth of
+    # it apart: a GEMM that computes something else picks tokens that fail this.
+    for i, t, gap, lead, std in _divergences(eng, sd, emb, lens, a, b):
+        assert gap <= NEAR_TIE * std and lead <= NEAR_TIE * std, (i, t, gap, lead, std)
     assert out["lens"].cpu().tolist() == [T] * len(lens)
 
 
 def test_mega_batch_slot_independence_and_stop_ids():
-    eng = _engine()
+    eng, _ = _engine()
     lens = [200, 333, 200]
     emb, pos, deltas = _batch(lens, seed=3)
     emb[533:733] = emb[0:200]                                          # sequence 2 == sequence 0

@@ -1,4 +1,4 @@
-"""-m gpu (needs 2 GPUs: run with ``gpurun --gpus 2``): the same sample list decoded by 1 rank and by 2 ranks (torchrun, NCCL,
+"""-m gpu (needs 2 GPUs): the same sample list decoded by 1 rank and by 2 ranks (torchrun, NCCL,
 dp.shard_range + dp.gather_ids -- the code bench.py runs) returns IDENTICAL token ids in the same order.  This holds bit for
 bit because no kernel's result depends on where a sample sits in the batch: attention tiles restart at every image / prompt,
 the channel-attention Gram and the HFRE sums are reduced in an order-independent way, GEMM rows are independent."""

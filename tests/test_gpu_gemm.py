@@ -1,4 +1,4 @@
-"""-m gpu: the tcgen05 GEMM (through the C ABI) vs a plain torch fp32 reference of the same op.
+"""-m gpu: the wgmma GEMM (through the C ABI) vs a plain torch fp32 reference of the same op.
 Inputs are bf16-rounded; accumulation is fp32 in both; tolerance 1e-3 relative on the fp32 result,
 plus bf16 output rounding (2^-8) when the output is bf16."""
 import pytest
@@ -47,6 +47,45 @@ def test_gemm_plain(M, N, K):
     out16 = ops.gemm(a, w)
     torch.cuda.synchronize()
     _check(out16, _ref(a, w), True)
+
+
+def _check_rows(got, a, w, rows, bias=None, act=None, residual=None):
+    """sampled rows of a problem too large for a full fp32 reference"""
+    ref = _ref(a[rows], w, bias, act, None if residual is None else residual[rows])
+    _check(got[rows], ref, got.dtype == torch.bfloat16)
+
+
+@pytest.mark.parametrize("M,N,K", [(32768, 3840, 1280), (19000, 1280, 3456), (37888 + 77, 520, 1280)])
+def test_gemm_large_plain(M, N, K):
+    """the tower / prefill shapes of a 32-image batch: many waves of 256-wide tiles per persistent CTA, ragged last tiles"""
+    ops = _ops()
+    g = torch.Generator(device="cuda").manual_seed(M + N)
+    a = (torch.randn(M, K, device="cuda", generator=g) * 0.5).bfloat16()
+    w = (torch.randn(N, K, device="cuda", generator=g) * 0.05).bfloat16()
+    out = ops.gemm(a, w)
+    torch.cuda.synchronize()
+    assert torch.isfinite(out.float()).all()
+    rows = torch.cat([torch.randint(0, M, (256,), device="cuda"), torch.arange(M - 130, M, device="cuda")])
+    _check_rows(out, a, w, rows)
+
+
+def test_gemm_large_epilogues():
+    ops = _ops()
+    g = torch.Generator(device="cuda").manual_seed(7)
+    M, N, K = 38400, 2560, 1280
+    a = (torch.randn(M, K, device="cuda", generator=g) * 0.5).bfloat16()
+    w = (torch.randn(N, K, device="cuda", generator=g) * 0.05).bfloat16()
+    bias = (torch.randn(N, device="cuda", generator=g) * 0.1).bfloat16()
+    res = torch.randn(M, N, device="cuda", generator=g).bfloat16()
+    rows = torch.randint(0, M, (256,), device="cuda")
+    out = ops.gemm(a, w, bias=bias, act="gelu", residual=res)
+    _check_rows(out, a, w, rows, bias, "gelu", res)
+    out = ops.gemm(a, w, out_dtype=torch.float32)
+    _check_rows(out, a, w, rows)
+    out = ops.gemm(a, w, bias=bias, act="silu", gated=True)        # W rows interleave [32 gate | 32 up] blocks
+    y = (a[rows].float() @ w.float().t() + bias.float()).view(len(rows), N // 64, 2, 32)
+    ref = (torch.nn.functional.silu(y[:, :, 0]) * y[:, :, 1]).reshape(len(rows), N // 2)
+    _check(out[rows], ref, True)
 
 
 @pytest.mark.parametrize("act", [None, "gelu", "silu"])

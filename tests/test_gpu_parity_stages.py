@@ -11,8 +11,8 @@ walk: sqrt(10) x that for one transformer block).  Three checks per stage:
   (B) max-norm  max|engine - bf16 oracle| / max|oracle| <= 1e-3 + k * 2^-8, k = single-ulp flips tolerated at the largest
       element (stated per test);
   (C) relative RMS  ||engine - bf16 oracle|| / ||oracle|| <= 1.5e-3 x sqrt(storage points of the stage).
-fp32 outputs (HFRE): 1e-3 max-norm, as north_star states.  Measured values of every run are written to gpurun_out/ and the
-round's are committed under profiles/.
+fp32 outputs (HFRE): 1e-3 max-norm, as north_star states.  Measured values of every run are written as
+parity_<name>.json (``_record`` below).
 
 Geometries: C4 -- 640 -> 644 px, grid 46x46 (ragged ViT windows {64, 48, 36}, SURVEY.md appendix A2; images straddle the
 128-row attention tiles), DaViT 160/80/40/20 maps (window padding +8/+4/+8/+4), prompt of 244 + 529 tokens; C5 -- 1344 px,
@@ -316,7 +316,7 @@ def _mem_available_gb():
 FULL_DEPTH_CASES = [pytest.param(448, 16, 32, id="full_depth_448px"),
                     pytest.param(896, 64, 24, id="full_depth_c3_896px",
                                  marks=pytest.mark.skipif(not os.environ.get("FO1_PARITY_C3"),
-                                                          reason="~15 min of fp32 CPU oracle: run with FO1_PARITY_C3=1 (result committed in profiles/)"))]
+                                                          reason="~15 min of fp32 CPU oracle: run with FO1_PARITY_C3=1"))]
 
 
 @pytest.mark.parametrize("S,n_boxes,T", FULL_DEPTH_CASES)

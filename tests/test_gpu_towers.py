@@ -116,7 +116,7 @@ def test_region_projector_matches_oracle():
 
 @pytest.mark.parametrize("grid", [(32, 32), (16, 16), (64, 64)])
 def test_fpn_implicit_conv_equals_im2col_path(grid, monkeypatch):
-    """SimpleFPN's 3x3 convs run as an implicit GEMM (4-D TMA patches, zero padding by the out-of-range fill, gemm_tcgen05.cu
+    """SimpleFPN's 3x3 convs run as an implicit GEMM (4-D TMA patches, zero padding by the out-of-range fill, gemm_wgmma.cu
     conv3x3_gemm); FO1_FPN_IM2COL forces the explicit column matrix + linear.  Same products in the same k order: bit-identical."""
     E, W = _mods()
     CK = __import__("importlib").import_module("vlm-fo1_b200.checkpoint")
@@ -136,7 +136,7 @@ def test_fpn_implicit_conv_equals_im2col_path(grid, monkeypatch):
         assert torch.isfinite(a[i].float()).all()
         rows = a[i].shape[0] * a[i].shape[1] * a[i].shape[2]
         diff = (a[i].float() - b[i].float()).abs()
-        if rows >= 148 * 128:      # both paths run the same unsplit 256-wide tiles: same products, same order
+        if rows >= 132 * 128:      # both paths run the same unsplit 256-wide tiles: same products, same order
             assert torch.equal(a[i], b[i]), (i, float(diff.max()))
         else:                      # the explicit path's small GEMM is split over K (other summation order): bf16-ulp flips before the LayerNorm
             assert float(diff.max()) <= 0.0625 and float(diff.mean()) < 2e-3 and float((diff == 0).float().mean()) > 0.8, \

@@ -1,4 +1,4 @@
-"""vlm-fo1_b200 -- host-side mirror of the VLM-FO1 hot path over libfo1.so (sm_100a CUDA).
+"""vlm-fo1_b200 -- host-side mirror of the VLM-FO1 hot path over libfo1.so (sm_90a CUDA).
 
 The directory name follows the repo convention (``vlm-fo1_b200``); import it as
 ``importlib.import_module("vlm-fo1_b200")`` or through the ``fo1_b200`` alias module at the repo root.

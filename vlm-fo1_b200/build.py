@@ -1,4 +1,4 @@
-"""Build libfo1.so (sm_100a) in-tree with nvcc.  No torch extension machinery: the product is a
+"""Build libfo1.so (sm_90a) in-tree with nvcc.  No torch extension machinery: the product is a
 plain C-ABI shared library loaded through ctypes."""
 from __future__ import annotations
 
@@ -17,7 +17,7 @@ LIB = os.path.join(PKG, "libfo1.so")
 
 NVCC = os.environ.get("NVCC") or shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-Wall", "--expt-relaxed-constexpr",
     "-I", os.path.join(REPO, "include"), "-I", CSRC,
 ]
@@ -68,7 +68,7 @@ def build(verbose: bool = False, force: bool = False) -> str:
         objs = list(ex.map(lambda s: _compile(s, verbose), srcs))
     newest = max(os.path.getmtime(o) for o in objs)
     if force or not os.path.exists(LIB) or os.path.getmtime(LIB) < newest:
-        cmd = [NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"]
+        cmd = [NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-lcudart"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -1,4 +1,4 @@
-// attention_tc.cu -- variable-length softmax attention on the 5th-generation tensor cores (tcgen05 + TMEM + TMA).
+// attention_tc.cu -- variable-length softmax attention on the Hopper tensor cores (wgmma + TMA).
 //
 // One kernel serves the ViT's windowed / full attention (head_dim 80; modeling_qwen2_5_vl.py:172-209, the
 // flash_attn_varlen_func call at :205), DaViT's 12x12 window attention (head_dim 32; modeling_davit.py:225-282) and the
@@ -12,18 +12,18 @@
 // The engines pass a tile table whose tiling restarts at every image / prompt, so a sample's result does not depend on
 // its position in the batch (bit-identical across batch compositions and rank counts).
 //
-// CTA = one (query tile, head), 192 threads, two CTAs per SM:
-//   warp 0   : TMA producer -- Q once, then K and V 64-key tiles through two 2-stage rings (3-D tensor maps over
+// CTA = one (query tile, head), 288 threads:
+//   warp 8   : TMA producer -- Q once, then K and V 64-key tiles through two 2-stage rings (3-D tensor maps over
 //              (head_dim, head, row), 64-wide boxes, 128-byte swizzle; head_dim 80 / 32 are zero-filled to the box by
 //              the TMA out-of-bounds rule, so every operand has 128-byte rows);
-//   warp 1   : tcgen05.mma issuer -- S_j = Q.K_j^T (M 128 x N 64, K-major operands) into one of two TMEM buffers, then
-//              O += P_j.V_j with V taken MN-major straight from its TMA tile (no transposition pass) and P from shared
-//              memory; tcgen05.commit publishes S / frees the ring slots / publishes O;
-//   warps 2-5: softmax -- one thread per query row: tcgen05.ld of its S row, mask, running max / sum in registers,
-//              P = exp2(S*scale - m) written as bf16 in the K-major swizzled layout the next MMA reads.  O stays in
-//              TMEM for the whole key loop; it is rescaled (tcgen05.ld -> mul -> tcgen05.st) only when a row's max has
-//              grown by more than 2^8 since the last rescale (stale maxima are exact: the factor cancels in O / l).
-// Warps whose 32 rows cannot see a key tile at all (the other window of the tile) skip the exponentials.
+//   warps 0-7: two consumer warpgroups, 64 query rows each -- S_j = Q.K_j^T (wgmma m64n64k16, K-major operands) into
+//              registers; softmax on the accumulator fragment (a row lives in the four lanes of a quad): mask, running
+//              max / sum, P = exp2(S*scale - m) packed to bf16 in place as the A fragments of the next wgmma; O += P_j.V_j
+//              with V taken MN-major straight from its TMA tile (no transposition pass).  O stays in registers for the
+//              whole key loop; it is rescaled only when a row's max has grown by more than 2^8 since the last rescale
+//              (stale maxima are exact: the factor cancels in O / l).  While one warpgroup is in its softmax the other
+//              one's wgmma keeps the tensor cores busy.
+// Warps whose 16 rows cannot see a key tile at all (the other window of the tile) skip the exponentials.
 #include <cuda.h>
 
 #include <algorithm>
@@ -40,22 +40,22 @@ int make_tmap_3d_bf16(CUtensorMap* out, const void* ptr, uint64_t d0, uint64_t d
 
 constexpr int kAtM = 128;          // query rows per CTA
 constexpr int kAtN = 64;           // keys per iteration
-constexpr int kAtThreads = 192;
+constexpr int kAtConsumers = 256;  // two warpgroups, 64 query rows each
+constexpr int kAtThreads = kAtConsumers + 32;
 constexpr float kAtRescale = 8.0f; // log2 units a row maximum may lag behind before O is rescaled
 
 template <int HD>
 struct AtCfg {
   static constexpr int HDP = HD <= 64 ? 64 : 128;      // head_dim as staged (zero-filled)
   static constexpr int NDB = HDP / 64;                 // 64-wide boxes per row
+  static constexpr int N0 = NDB == 1 ? HD : 64;        // live dims of the first box
+  static constexpr int N1 = NDB == 2 ? HD - 64 : 16;   // live dims of the second box (16 for head_dim 80; unused with one box)
   static constexpr int kQBytes = NDB * kAtM * 128;
   static constexpr int kKBytes = NDB * kAtN * 128;
   static constexpr int kVBytes = NDB * kAtN * 128;
-  static constexpr int kPBytes = kAtM * 128;
-  static constexpr int kTileBytes = kQBytes + 2 * kKBytes + 2 * kVBytes + kPBytes;
-  // the dynamic window is at least 128-byte aligned: aligning it to 1024 costs at most 896 B; 128 B of barriers
-  // follow the tiles.  head_dim 80 / 128: 115 712 B, exactly what lets two CTAs share an SM (2 x (113 KB + 1 KB)).
+  static constexpr int kTileBytes = kQBytes + 2 * kKBytes + 2 * kVBytes;
+  // the dynamic window is at least 128-byte aligned: aligning it to 1024 costs at most 896 B; 128 B of barriers follow the tiles
   static constexpr int kSmemBytes = kTileBytes + 896 + 128;
-  static constexpr int kTmemCols = 256;                // S0 [0,64) | S1 [64,128) | O [128, 128 + HDP)
   static_assert(HD % 16 == 0 && HD <= 128, "head_dim must be a multiple of 16, at most 128");
 };
 
@@ -91,61 +91,46 @@ __global__ void __launch_bounds__(256) attn_rowseg_kernel(const int* __restrict_
 }
 
 template <int HD, bool CAUSAL>
-__global__ void __launch_bounds__(kAtThreads, 2)
+__global__ void __launch_bounds__(kAtThreads, 1)
 attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                const AttnTcArgs a) {
   using Cfg = AtCfg<HD>;
-  constexpr int NDB = Cfg::NDB;
+  constexpr int NDB = Cfg::NDB, N0 = Cfg::N0, N1 = Cfg::N1;
   extern __shared__ uint8_t at_smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(at_smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* sQ = smem;
   uint8_t* sK = sQ + Cfg::kQBytes;
   uint8_t* sV = sK + 2 * Cfg::kKBytes;
-  uint8_t* sP = sV + 2 * Cfg::kVBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + Cfg::kPBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + 2 * Cfg::kVBytes);
   uint64_t* q_full = bars;            // [1]
   uint64_t* k_full = bars + 1;        // [2]
   uint64_t* k_empty = bars + 3;       // [2]
   uint64_t* v_full = bars + 5;        // [2]
   uint64_t* v_empty = bars + 7;       // [2]
-  uint64_t* s_full = bars + 9;        // [2]
-  uint64_t* s_empty = bars + 11;      // [2]
-  uint64_t* p_full = bars + 13;       // [1]
-  uint64_t* o_done = bars + 14;       // [1]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(sP);   // read once before the first P tile is written (second __syncthreads below)
+  uint64_t* q_empty = bars + 9;       // [1] the consumers are done with the Q tile (their output staging)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  uint64_t* q_empty = bars + 15;      // [1] the softmax warps are done with the Q tile (their output staging) and with O in TMEM
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     ptx::prefetch_tmap(&tmQ);
     ptx::prefetch_tmap(&tmK);
     ptx::prefetch_tmap(&tmV);
     ptx::mbar_init(ptx::smem_u32(q_full), 1);
-    ptx::mbar_init(ptx::smem_u32(q_empty), 128);
+    ptx::mbar_init(ptx::smem_u32(q_empty), kAtConsumers);
     for (int s = 0; s < 2; ++s) {
       ptx::mbar_init(ptx::smem_u32(k_full + s), 1);
-      ptx::mbar_init(ptx::smem_u32(k_empty + s), 1);
+      ptx::mbar_init(ptx::smem_u32(k_empty + s), kAtConsumers / 32);   // one arrive per consumer warp
       ptx::mbar_init(ptx::smem_u32(v_full + s), 1);
-      ptx::mbar_init(ptx::smem_u32(v_empty + s), 1);
-      ptx::mbar_init(ptx::smem_u32(s_full + s), 1);
-      ptx::mbar_init(ptx::smem_u32(s_empty + s), 128);
+      ptx::mbar_init(ptx::smem_u32(v_empty + s), kAtConsumers / 32);
     }
-    ptx::mbar_init(ptx::smem_u32(p_full), 128);
-    ptx::mbar_init(ptx::smem_u32(o_done), 1);
     ptx::mbar_fence_init();
   }
-  if (warp == 1) ptx::tmem_alloc(ptx::smem_u32(tmem_ptr), Cfg::kTmemCols);
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  __syncthreads();                    // everybody holds the TMEM address before the softmax warps reuse its slot for P
 
-  // Persistent CTA: work items (query tile, head), head fastest, static round robin.  Barriers, TMEM and the tensor-map prefetch are
-  // set up once; every role walks the same item list and carries ONE running key-tile counter g across items (ring stage = g & 1,
-  // phase = (g >> 1) & 1), so the K/V ring keeps streaming across item boundaries.  Per item: the Q tile and the O accumulator are
-  // single-buffered -- the producer reloads Q, and the MMA warp restarts O, only after the softmax warps released them (q_empty).
+  // Persistent CTA: work items (query tile, head), head fastest, static round robin.  Barriers and the tensor-map prefetch are set up
+  // once; every role walks the same item list and carries ONE running key-tile counter g across items (ring stage = g & 1, phase =
+  // (g >> 1) & 1), so the K/V ring keeps streaming across item boundaries.  The Q tile is single-buffered: the producer reloads it
+  // only after the consumers released it (q_empty).
   const int n_work = a.n_work;
   auto item_geom = [&](int work, int& head, int& kvh, int& row0, int& rows_valid, int& kv_begin, int& n_kv) {
     head = work % a.q_heads;
@@ -163,7 +148,7 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
     n_kv = (kv_end - kv_begin + kAtN - 1) / kAtN;
   };
 
-  if (warp == 0) {
+  if (warp == kAtConsumers / 32) {
     // ================================================ TMA producer ================================================
     if (ptx::elect_one()) {
       uint32_t g = 0, item = 0;
@@ -190,79 +175,28 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
         }
       }
     }
-  } else if (warp == 1) {
-    // ================================================= MMA issuer =================================================
-    constexpr uint32_t idesc_s = ptx::umma_idesc_bf16(kAtM, kAtN);
+  } else {
+    // ========================================= consumers: S = Q.K^T, softmax, O += P.V =========================================
+    const int wg = warp >> 2;
+    const int fr = lane >> 2, fq2 = (lane & 3) * 2;
+    const int r_lo = warp * 16 + fr;                    // this thread's rows inside the tile: r_lo and r_lo + 8
+    const uint32_t q_addr = ptx::smem_u32(sQ) + wg * (64 * 128);
     uint32_t gbase = 0, item = 0;
     for (int work = blockIdx.x; work < n_work; work += gridDim.x, ++item) {
       int head, kvh, row0, rows_valid, kv_begin, n_kv;
       item_geom(work, head, kvh, row0, rows_valid, kv_begin, n_kv);
-      at_wait(q_full, item & 1);          // (Q is reloaded only after q_empty: O of the previous item has been read out by then)
-      for (int j = 0; j <= n_kv; ++j) {
-        if (j < n_kv) {                                   // S_j = Q . K_j^T
-          const uint32_t g = gbase + j, st = g & 1;
-          at_wait(k_full + st, (g >> 1) & 1);
-          if (g >= 2) at_wait(s_empty + st, ((g >> 1) - 1) & 1);
-          ptx::tc_fence_after();
-          if (ptx::elect_one()) {
-            const uint32_t q_addr = ptx::smem_u32(sQ), k_addr = ptx::smem_u32(sK + st * Cfg::kKBytes);
+      int lo[2], hi[2];
 #pragma unroll
-            for (int kk = 0; kk < HD / 16; ++kk) {
-              const uint64_t da = ptx::umma_desc_k_sw128(q_addr + (kk >> 2) * (kAtM * 128) + (kk & 3) * 32);
-              const uint64_t db = ptx::umma_desc_k_sw128(k_addr + (kk >> 2) * (kAtN * 128) + (kk & 3) * 32);
-              ptx::tc_mma_bf16(tmem_base + st * kAtN, da, db, idesc_s, kk > 0 ? 1u : 0u);
-            }
-            ptx::tc_commit(ptx::smem_u32(s_full + st));
-            ptx::tc_commit(ptx::smem_u32(k_empty + st));
-          }
-          __syncwarp();
-        }
-        if (j >= 1) {                                     // O += P_{j-1} . V_{j-1}
-          const int jj = j - 1;
-          const uint32_t g = gbase + jj, st = g & 1;
-          at_wait(p_full, g & 1);
-          at_wait(v_full + st, (g >> 1) & 1);
-          ptx::tc_fence_after();
-          if (ptx::elect_one()) {
-            const uint32_t p_addr = ptx::smem_u32(sP), v_addr = ptx::smem_u32(sV + st * Cfg::kVBytes);
-#pragma unroll
-            for (int kk = 0; kk < kAtN / 16; ++kk) {
-              const uint64_t da = ptx::umma_desc_k_sw128(p_addr + kk * 32);
-#pragma unroll
-              for (int b = 0; b < NDB; ++b) {
-                constexpr int kLastN = HD - (NDB - 1) * 64;             // live dims of the last box (16 for head_dim 80)
-                const int nb = (b == NDB - 1) ? kLastN : 64;
-                const uint64_t db = ptx::umma_desc_mn_sw128(v_addr + b * (kAtN * 128) + kk * 2048);
-                ptx::tc_mma_bf16(tmem_base + 2 * kAtN + b * 64, da, db, ptx::umma_idesc_bf16(kAtM, nb) | ptx::kUmmaBMajorMN,
-                                 (jj > 0 || kk > 0) ? 1u : 0u);
-              }
-            }
-            ptx::tc_commit(ptx::smem_u32(o_done));
-            ptx::tc_commit(ptx::smem_u32(v_empty + st));
-          }
-          __syncwarp();
+      for (int h = 0; h < 2; ++h) {
+        const int r = r_lo + 8 * h, row = row0 + r;
+        lo[h] = 0; hi[h] = 0;                             // rows beyond the tile: empty key range
+        if (r < rows_valid) {
+          const int2 rs = __ldg(a.rowseg + row);
+          lo[h] = rs.x; hi[h] = rs.y;
+          if (CAUSAL) hi[h] = min(hi[h], row + 1);
         }
       }
-      gbase += (uint32_t)n_kv;
-    }
-  } else {
-    // ================================================== softmax ===================================================
-    const int quarter = warp & 3;                       // TMEM lane quarter this warp may touch (warp id mod 4)
-    const int r = quarter * 32 + lane;                  // row inside the tile == TMEM lane
-    const uint32_t t_lane = tmem_base + ((uint32_t)(quarter * 32) << 16);
-    uint8_t* p_row = sP + r * 128;
-    uint32_t gbase = 0;
-    for (int work = blockIdx.x; work < n_work; work += gridDim.x) {
-      int head, kvh, row0, rows_valid, kv_begin, n_kv;
-      item_geom(work, head, kvh, row0, rows_valid, kv_begin, n_kv);
-      const int row = row0 + r;
-      int lo = 0, hi = 0;                                 // rows beyond T: empty key range
-      if (r < rows_valid) {
-        const int2 rs = __ldg(a.rowseg + row);
-        lo = rs.x; hi = rs.y;
-        if (CAUSAL) hi = min(hi, row + 1);
-      }
-      int wlo_min = lo, wlo_max = lo, whi_min = hi, whi_max = hi;
+      int wlo_min = min(lo[0], lo[1]), wlo_max = max(lo[0], lo[1]), whi_min = min(hi[0], hi[1]), whi_max = max(hi[0], hi[1]);
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) {
         wlo_min = min(wlo_min, __shfl_xor_sync(0xffffffffu, wlo_min, o));
@@ -270,128 +204,159 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
         whi_min = min(whi_min, __shfl_xor_sync(0xffffffffu, whi_min, o));
         whi_max = max(whi_max, __shfl_xor_sync(0xffffffffu, whi_max, o));
       }
-      const uint32_t span = (uint32_t)(hi - lo);
-      float m_run = -INFINITY, l_run = 0.f;               // running max (scaled, log2 units) and sum of this row
+      const uint32_t span[2] = {(uint32_t)(hi[0] - lo[0]), (uint32_t)(hi[1] - lo[1])};
+      float m_run[2] = {-INFINITY, -INFINITY};            // running maxima (scaled, log2 units) of the two rows
+      float l_run[2] = {0.f, 0.f};                        // this thread's share of the two row sums (quad-reduced at the end)
+      float o0[N0 / 2], o1[N1 / 2];
+#pragma unroll
+      for (int i = 0; i < N0 / 2; ++i) o0[i] = 0.f;
+#pragma unroll
+      for (int i = 0; i < N1 / 2; ++i) o1[i] = 0.f;
 
+      at_wait(q_full, item & 1);
       for (int j = 0; j < n_kv; ++j) {
         const uint32_t g = gbase + j, st = g & 1;
         const int k0 = kv_begin + j * kAtN;
         const bool dead = (k0 >= whi_max) || (k0 + kAtN <= wlo_min);          // no row of this warp sees the tile
         const bool interior = (k0 >= wlo_max) && (k0 + kAtN <= whi_min);      // every row sees every key
-        at_wait(s_full + st, (g >> 1) & 1);
-        ptx::tc_fence_after();
-        uint32_t sr[2][32];
-        if (!dead) {
-          ptx::tmem_ld_32x32(t_lane + st * kAtN, sr[0]);
-          ptx::tmem_ld_32x32(t_lane + st * kAtN + 32, sr[1]);
-          ptx::tmem_ld_wait();
-        }
-        ptx::tc_fence_before();
-        ptx::mbar_arrive(ptx::smem_u32(s_empty + st));     // S_j is in registers: the buffer may take S_{j+2}
-        uint32_t pk[32];
+        // ---- S_j = Q . K_j^T (64 x 64 per warpgroup, K-major operands) ----
+        at_wait(k_full + st, (g >> 1) & 1);
+        float s[32];
+#pragma unroll
+        for (int i = 0; i < 32; ++i) s[i] = 0.f;
+        const uint32_t k_addr = ptx::smem_u32(sK + st * Cfg::kKBytes);
+        ptx::wgmma_fence_regs(s);
+        ptx::wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < HD / 16; ++kk)
+          ptx::Wgmma<64>::template ss<0, 0>(s, ptx::wgmma_desc_k_sw128(q_addr + (kk >> 2) * (kAtM * 128) + (kk & 3) * 32),
+                                            ptx::wgmma_desc_k_sw128(k_addr + (kk >> 2) * (kAtN * 128) + (kk & 3) * 32), kk > 0 ? 1u : 0u);
+        ptx::wgmma_commit();
+        ptx::wgmma_wait<0>();
+        ptx::wgmma_fence_regs(s);
+        if (lane == 0) ptx::mbar_arrive(ptx::smem_u32(k_empty + st));
+        // ---- softmax on the fragment: a row lives in the four lanes of a quad, two rows per thread ----
+        uint32_t p[4][4];                                   // P as the A fragments of the four 16-key steps
         if (dead) {
 #pragma unroll
-          for (int c = 0; c < 32; ++c) pk[c] = 0u;
+          for (int kk = 0; kk < 4; ++kk) { p[kk][0] = 0u; p[kk][1] = 0u; p[kk][2] = 0u; p[kk][3] = 0u; }
         } else {
-          float mt = -INFINITY;
-          if (interior) {
 #pragma unroll
-            for (int c = 0; c < 64; ++c) mt = fmaxf(mt, __uint_as_float(sr[c >> 5][c & 31]));
-          } else {
+          for (int h = 0; h < 2; ++h) {
+            float mt = -INFINITY;
 #pragma unroll
-            for (int c = 0; c < 64; ++c) {
-              const bool ok = (uint32_t)(k0 + c - lo) < span;
-              const float x = ok ? __uint_as_float(sr[c >> 5][c & 31]) : -INFINITY;
-              sr[c >> 5][c & 31] = __float_as_uint(x);
-              mt = fmaxf(mt, x);
+            for (int c8 = 0; c8 < 8; ++c8) {
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const int idx = 4 * c8 + 2 * h + e;
+                if (!interior) {
+                  const bool ok = (uint32_t)(k0 + c8 * 8 + fq2 + e - lo[h]) < span[h];
+                  s[idx] = ok ? s[idx] : -INFINITY;
+                }
+                mt = fmaxf(mt, s[idx]);
+              }
             }
-          }
-          const float m_new = fmaxf(m_run, mt * a.sl2);
-          // lazy rescale: keep a stale maximum until it lags by 2^8; a row without any live key so far has O == 0 exactly
-          const bool grow = m_new > m_run + kAtRescale;
-          const bool touch = grow && (m_run != -INFINITY);
-          float alpha = 1.0f;
-          if (grow) {
-            if (touch) { alpha = ex2_approx(m_run - m_new); l_run *= alpha; }
-            m_run = m_new;
-          }
-          if (__any_sync(0xffffffffu, touch)) {            // (touch implies j >= 1: g - 1 is this item's previous tile)
-            at_wait(o_done, (g - 1) & 1);                  // P_{j-1}.V_{j-1} has landed in O
-            ptx::tc_fence_after();
+            mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 1));
+            mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 2));
+            const float m_new = fmaxf(m_run[h], mt * a.sl2);
+            // lazy rescale: keep a stale maximum until it lags by 2^8 (stale maxima are exact: the factor cancels in O / l);
+            // a row without any live key so far has O == 0 exactly
+            if (m_new > m_run[h] + kAtRescale) {
+              if (m_run[h] != -INFINITY) {
+                const float alpha = ex2_approx(m_run[h] - m_new);
+                l_run[h] *= alpha;
 #pragma unroll
-            for (int c = 0; c < (HD + 31) / 32; ++c) {
-              uint32_t orow[32];
-              ptx::tmem_ld_32x32(t_lane + 2 * kAtN + c * 32, orow);
-              ptx::tmem_ld_wait();
+                for (int c8 = 0; c8 < N0 / 8; ++c8) { o0[4 * c8 + 2 * h] *= alpha; o0[4 * c8 + 2 * h + 1] *= alpha; }
+                if constexpr (NDB == 2) {
 #pragma unroll
-              for (int i = 0; i < 32; ++i) orow[i] = __float_as_uint(__uint_as_float(orow[i]) * alpha);
-              ptx::tmem_st_32x32(t_lane + 2 * kAtN + c * 32, orow);
+                  for (int c8 = 0; c8 < N1 / 8; ++c8) { o1[4 * c8 + 2 * h] *= alpha; o1[4 * c8 + 2 * h + 1] *= alpha; }
+                }
+              }
+              m_run[h] = m_new;
             }
-            ptx::tmem_st_wait();
-            ptx::tc_fence_before();
-          }
-          const float m_use = (m_run == -INFINITY) ? 0.f : m_run;
-          float sum = 0.f;
+            const float m_use = (m_run[h] == -INFINITY) ? 0.f : m_run[h];
+            float sum = 0.f;
 #pragma unroll
-          for (int c = 0; c < 64; c += 2) {
-            const float p0 = ex2_approx(fmaf(__uint_as_float(sr[c >> 5][c & 31]), a.sl2, -m_use));
-            const float p1 = ex2_approx(fmaf(__uint_as_float(sr[(c + 1) >> 5][(c + 1) & 31]), a.sl2, -m_use));
-            sum += p0 + p1;
-            pk[c >> 1] = pack_bf16(p0, p1);
+            for (int c8 = 0; c8 < 8; ++c8) {
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const int idx = 4 * c8 + 2 * h + e;
+                s[idx] = ex2_approx(fmaf(s[idx], a.sl2, -m_use));
+                sum += s[idx];
+              }
+            }
+            l_run[h] += sum;
           }
-          l_run += sum;
+#pragma unroll
+          for (int kk = 0; kk < 4; ++kk) {
+            p[kk][0] = pack_bf16(s[8 * kk + 0], s[8 * kk + 1]);
+            p[kk][1] = pack_bf16(s[8 * kk + 2], s[8 * kk + 3]);
+            p[kk][2] = pack_bf16(s[8 * kk + 4], s[8 * kk + 5]);
+            p[kk][3] = pack_bf16(s[8 * kk + 6], s[8 * kk + 7]);
+          }
         }
-        if (g >= 1) at_wait(o_done, (g - 1) & 1);          // the previous P (of this item or the last one) has been consumed: the buffer is free
+        // ---- O += P_j . V_j: P from registers, V MN-major straight from its TMA tile (no transposition pass) ----
+        at_wait(v_full + st, (g >> 1) & 1);
+        const uint32_t v_addr = ptx::smem_u32(sV + st * Cfg::kVBytes);
+        ptx::wgmma_fence_regs(o0);
+        ptx::wgmma_fence_regs(o1);
+        ptx::wgmma_fence();
 #pragma unroll
-        for (int c = 0; c < 8; ++c)
-          *reinterpret_cast<uint4*>(p_row + ((c ^ (r & 7)) << 4)) = make_uint4(pk[4 * c], pk[4 * c + 1], pk[4 * c + 2], pk[4 * c + 3]);
-        ptx::fence_proxy_async_smem();
-        ptx::mbar_arrive(ptx::smem_u32(p_full));
+        for (int kk = 0; kk < kAtN / 16; ++kk) {
+          ptx::Wgmma<N0>::template rs<1>(o0, p[kk], ptx::wgmma_desc_mn_sw128(v_addr + kk * 2048, kAtN * 128), 1u);
+          if constexpr (NDB == 2)
+            ptx::Wgmma<N1>::template rs<1>(o1, p[kk], ptx::wgmma_desc_mn_sw128(v_addr + kAtN * 128 + kk * 2048, kAtN * 128), 1u);
+        }
+        ptx::wgmma_commit();
+        ptx::wgmma_wait<0>();
+        ptx::wgmma_fence_regs(o0);
+        ptx::wgmma_fence_regs(o1);
+        if (lane == 0) ptx::mbar_arrive(ptx::smem_u32(v_empty + st));
       }
       gbase += (uint32_t)n_kv;
 
-      // ---- O / l -> bf16, staged through the (dead) Q tile of this warp, row-contiguous 16-byte stores ----
-      at_wait(o_done, (gbase - 1) & 1);
-      ptx::tc_fence_after();
-      const float inv = l_run > 0.f ? 1.0f / l_run : 0.f;
+      // ---- O / l -> bf16, staged through the (dead) Q tile, row-contiguous 16-byte stores ----
+      float inv[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float l = l_run[h];
+        l += __shfl_xor_sync(0xffffffffu, l, 1);
+        l += __shfl_xor_sync(0xffffffffu, l, 2);
+        inv[h] = l > 0.f ? 1.0f / l : 0.f;
+      }
+      asm volatile("bar.sync 1, 256;" ::: "memory");      // both warpgroups have read Q for the last time
       constexpr int PITCH = Cfg::HDP * 2;
-      uint8_t* stg = sQ + (warp - 2) * 32 * PITCH;
+      uint8_t* stg = sQ + warp * 16 * PITCH;
 #pragma unroll
-      for (int c = 0; c < (HD + 31) / 32; ++c) {
-        uint32_t orow[32];
-        ptx::tmem_ld_32x32(t_lane + 2 * kAtN + c * 32, orow);
-        ptx::tmem_ld_wait();
+      for (int h = 0; h < 2; ++h) {
+        const int rr = fr + 8 * h;
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          if (c * 32 + q * 8 < HD) {
-            const int ch = c * 4 + q;                     // 16-byte chunk of the row
-            *reinterpret_cast<uint4*>(stg + lane * PITCH + (((ch & ~7) | ((ch ^ lane) & 7)) << 4)) =
-                make_uint4(pack_bf16(__uint_as_float(orow[q * 8 + 0]) * inv, __uint_as_float(orow[q * 8 + 1]) * inv),
-                           pack_bf16(__uint_as_float(orow[q * 8 + 2]) * inv, __uint_as_float(orow[q * 8 + 3]) * inv),
-                           pack_bf16(__uint_as_float(orow[q * 8 + 4]) * inv, __uint_as_float(orow[q * 8 + 5]) * inv),
-                           pack_bf16(__uint_as_float(orow[q * 8 + 6]) * inv, __uint_as_float(orow[q * 8 + 7]) * inv));
+        for (int c8 = 0; c8 < N0 / 8; ++c8)
+          *reinterpret_cast<uint32_t*>(stg + rr * PITCH + (((c8 & ~7) | ((c8 ^ rr) & 7)) << 4) + (lane & 3) * 4) =
+              pack_bf16(o0[4 * c8 + 2 * h] * inv[h], o0[4 * c8 + 2 * h + 1] * inv[h]);
+        if constexpr (NDB == 2) {
+#pragma unroll
+          for (int c8 = 0; c8 < N1 / 8; ++c8) {
+            const int ch = 8 + c8;
+            *reinterpret_cast<uint32_t*>(stg + rr * PITCH + (((ch & ~7) | ((ch ^ rr) & 7)) << 4) + (lane & 3) * 4) =
+                pack_bf16(o1[4 * c8 + 2 * h] * inv[h], o1[4 * c8 + 2 * h + 1] * inv[h]);
           }
         }
       }
-      ptx::tc_fence_before();
       __syncwarp();
       constexpr int CH = HD / 8;
-      bf16* op = a.o + (long long)(row0 + quarter * 32) * a.ldo + (long long)head * HD;
-      for (int i = lane; i < 32 * CH; i += 32) {
+      bf16* op = a.o + (long long)(row0 + warp * 16) * a.ldo + (long long)head * HD;
+      for (int i = lane; i < 16 * CH; i += 32) {
         const int rr = i / CH, ch = i - rr * CH;
-        if (quarter * 32 + rr < rows_valid)
+        if (warp * 16 + rr < rows_valid)
           *reinterpret_cast<uint4*>(op + (long long)rr * a.ldo + ch * 8) =
               *reinterpret_cast<const uint4*>(stg + rr * PITCH + (((ch & ~7) | ((ch ^ rr) & 7)) << 4));
       }
       __syncwarp();
       ptx::fence_proxy_async_smem();                       // the next Q tile arrives through the async proxy
-      ptx::mbar_arrive(ptx::smem_u32(q_empty));            // Q tile (staging) and O are free for the next item
+      ptx::mbar_arrive(ptx::smem_u32(q_empty));            // the Q tile (staging) is free for the next item
     }
   }
-
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) ptx::tmem_dealloc(tmem_base, Cfg::kTmemCols);
 }
 
 // ---------------------------------------------------------------------------------------------------------- host
@@ -436,7 +401,6 @@ static int launch_attn_tc(const AttnArgs& a, const int2* rowseg, cudaStream_t s)
   static bool attr_set = false;
   if (!attr_set) {
     FO1_CUDA(cudaFuncSetAttribute(attn_tc_kernel<HD, CAUSAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-    FO1_CUDA(cudaFuncSetAttribute(attn_tc_kernel<HD, CAUSAL>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
     attr_set = true;
   }
   const int T = a.total_rows;
@@ -452,10 +416,10 @@ static int launch_attn_tc(const AttnArgs& a, const int2* rowseg, cudaStream_t s)
   FO1_CHECK_ARG(blocks < (1ll << 31), "attention: grid too large (%lld blocks)", blocks);
   g.n_work = (int)blocks;
   ProfScope prof(CAUSAL ? "attn_causal" : "attn", a.flops, 0.0, s);
-  // persistent for the non-causal shapes (equal-cost items: ViT / DaViT windows 0.40 -> 0.33 ms, 0.78 -> 0.66 ms per layer at 32 images): two
-  // CTAs per SM walk the item list.  Causal prompts have items of very different cost; the static round robin lost 19 % against the
-  // hardware block scheduler there, so they keep one CTA per item (the same kernel with a one-item list).  FO1_ATTN_ONE_ITEM: A/B knob.
-  const long long resident = 2LL * device_sm_count();
+  // persistent for the non-causal shapes (equal-cost items): one CTA per SM walks the item list.  Causal prompts have items of very
+  // different cost, which a static round robin balances badly, so they keep one CTA per item (the same kernel with a one-item
+  // list) and leave the balancing to the hardware block scheduler.  FO1_ATTN_ONE_ITEM: A/B knob.
+  const long long resident = device_sm_count();
   const unsigned grid = (unsigned)((CAUSAL || getenv("FO1_ATTN_ONE_ITEM") != nullptr || blocks < resident) ? blocks : resident);
   attn_tc_kernel<HD, CAUSAL><<<grid, kAtThreads, Cfg::kSmemBytes, s>>>(tmQ, tmK, tmV, g);
   FO1_LAUNCH_CHECK();

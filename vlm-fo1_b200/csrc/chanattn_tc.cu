@@ -1,4 +1,4 @@
-// chanattn_tc.cu -- DaViT channel-group attention (modeling_davit.py:151-172) as two tcgen05 contractions.
+// chanattn_tc.cu -- DaViT channel-group attention (modeling_davit.py:151-172) as two wgmma contractions.
 //
 // Per image and group of 32 channels the reference computes, over the N tokens of the map,
 //     A = softmax_c2( (q * N^-0.5)^T k )   [32 x 32]          out = (A v^T)^T   [N x 32]
@@ -6,18 +6,18 @@
 // arithmetic per byte (the pass over q, k and the pass over v are what cost), so the kernels are built to stream:
 //
 //   chan_gram_tc_kernel  : CTA = (token chunk, 128-channel quad = 4 groups, image).  TMA brings q and k tiles of 128 tokens
-//                          x 128 channels ([token][channel] rows, 128-byte swizzle) through a 3-stage ring; ONE tcgen05.mma
-//                          chain accumulates G[c1][c2] += sum_tok q[tok][c1] k[tok][c2] for the whole 128 x 128 quad in TMEM,
-//                          both operands MN-major straight from the TMA tiles (the token axis is the contraction axis, so no
-//                          transposition is needed).  Only the four 32 x 32 diagonal blocks are kept: each epilogue thread
-//                          owns one row c1 and reads the 32 columns of its own group.  Partial Grams of the token chunks
-//                          are written side by side and summed in a FIXED order by the consumer (no atomics: the result is
-//                          bit-reproducible and independent of the batch slot).
+//                          x 128 channels ([token][channel] rows, 128-byte swizzle) through a 3-stage ring; each of the two
+//                          consumer warpgroups owns one 64-channel half (two groups) and accumulates
+//                          G[c1][c2] += sum_tok q[tok][c1] k[tok][c2] for its 64 x 64 block in registers with ONE wgmma
+//                          chain, both operands MN-major straight from the TMA tiles (the token axis is the contraction
+//                          axis, so no transposition is needed).  Only the two 32 x 32 diagonal blocks are kept.  Partial
+//                          Grams of the token chunks are written side by side and summed in a FIXED order by the consumer
+//                          (no atomics: the result is bit-reproducible and independent of the batch slot).
 //   chan_apply_tc_kernel : same CTA shape.  Prologue: sum the partial Grams, scale, softmax over c2 (fp32), and lay the
 //                          quad's block-diagonal [128 x 128] bf16 matrix out as a K-major swizzled B operand in shared
-//                          memory.  Main loop: v tiles by TMA, out[tok][c1] = sum_c2 v[tok][c2] A[c1][c2] as UMMA 128 x 128 x 16
-//                          steps into a double-buffered TMEM accumulator, epilogue warps convert and write 256-byte rows.
-// The 4x arithmetic waste of multiplying the off-diagonal blocks is free: the tensor pipe is < 20 % busy at HBM speed.
+//                          memory.  Main loop: v tiles by TMA, out[tok][c1] = sum_c2 v[tok][c2] A[c1][c2] as wgmma
+//                          m64n128k16 steps (64 tokens per warpgroup), the warps convert and write 256-byte rows.
+// The arithmetic waste of multiplying the off-diagonal blocks is free: the tensor pipe is far from busy at HBM speed.
 #include <cuda.h>
 
 #include <algorithm>
@@ -32,11 +32,11 @@ int make_tmap_3d_bf16(CUtensorMap* out, const void* ptr, uint64_t d0, uint64_t d
 
 constexpr int kCaTok = 128;               // tokens per tile
 constexpr int kCaQuad = 128;              // channels per CTA (4 groups of 32)
-constexpr int kCaThreads = 192;           // warp 0 TMA, warp 1 MMA, warps 2-5 epilogue
+constexpr int kCaConsumers = 256;         // warps 0-7: two consumer warpgroups
+constexpr int kCaThreads = kCaConsumers + 32;   // warp 8: TMA producer
 constexpr int kCaStages = 3;
 constexpr int kCaBoxBytes = kCaTok * 128; // one [128 tokens][64 channels] box
 constexpr int kCaMaxChunks = 32;
-constexpr uint32_t kUmmaAMajorMN = 1u << 15;
 
 __device__ __forceinline__ void ca_wait(uint64_t* bar, uint32_t parity) {
   const uint32_t b = ptx::smem_u32(bar);
@@ -44,16 +44,6 @@ __device__ __forceinline__ void ca_wait(uint64_t* bar, uint32_t parity) {
   while (!ptx::mbar_try_wait(b, parity)) {
     if (++spins > (1u << 26)) __trap();
   }
-}
-// MN-major operand of 128 MN-elements: two 64-element atoms `lbo` bytes apart, 8-K-index groups 1024 B apart
-__device__ __forceinline__ uint64_t ca_desc_mn(uint32_t smem_addr, uint32_t lbo) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
 }
 
 struct ChanArgs {
@@ -73,27 +63,20 @@ chan_gram_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kCaStages * 4 * kCaBoxBytes);
   uint64_t* full = bars;                 // [stages]
   uint64_t* empty = bars + kCaStages;    // [stages]
-  uint64_t* done = bars + 2 * kCaStages; // [1]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * kCaStages + 1);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int chunk = blockIdx.x, quad = blockIdx.y, b = blockIdx.z;
   const int tile0 = chunk * a.tiles_per_chunk;
   const int n_tiles = max(0, min(a.tiles_per_chunk, (a.N + kCaTok - 1) / kCaTok - tile0));
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     ptx::prefetch_tmap(&tmQ);
     ptx::prefetch_tmap(&tmK);
-    for (int s = 0; s < kCaStages; ++s) { ptx::mbar_init(ptx::smem_u32(full + s), 1); ptx::mbar_init(ptx::smem_u32(empty + s), 1); }
-    ptx::mbar_init(ptx::smem_u32(done), 1);
+    for (int s = 0; s < kCaStages; ++s) { ptx::mbar_init(ptx::smem_u32(full + s), 1); ptx::mbar_init(ptx::smem_u32(empty + s), kCaConsumers / 32); }
     ptx::mbar_fence_init();
   }
-  if (warp == 1) ptx::tmem_alloc(ptx::smem_u32(tmem_ptr), 128);
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
+  if (warp == kCaConsumers / 32) {
     if (ptx::elect_one()) {
       for (int t = 0; t < n_tiles; ++t) {
         const int st = t % kCaStages;
@@ -108,55 +91,49 @@ chan_gram_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
         ptx::tma_load_3d(ptx::smem_u32(base + 3 * kCaBoxBytes), &tmK, fb, quad * kCaQuad + 64, tok, b);
       }
     }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = ptx::umma_idesc_bf16(128, 128) | kUmmaAMajorMN | ptx::kUmmaBMajorMN;
+  } else {
+    const int wg = warp >> 2;               // 64-channel half of the quad: its q box and its k box
+    float acc[32];                          // G[64 x 64] fragment of this warpgroup
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[i] = 0.f;
     for (int t = 0; t < n_tiles; ++t) {
       const int st = t % kCaStages;
       ca_wait(full + st, (t / kCaStages) & 1);
-      ptx::tc_fence_after();
-      if (ptx::elect_one()) {
-        const uint32_t qa = ptx::smem_u32(smem + st * 4 * kCaBoxBytes), ka = qa + 2 * kCaBoxBytes;
+      const uint32_t qa = ptx::smem_u32(smem + st * 4 * kCaBoxBytes) + wg * kCaBoxBytes, ka = qa + 2 * kCaBoxBytes;
+      ptx::wgmma_fence_regs(acc);
+      ptx::wgmma_fence();
 #pragma unroll
-        for (int kk = 0; kk < kCaTok / 16; ++kk)      // 16 tokens per step: 16 rows x 128 B = 2048 B into each box
-          ptx::tc_mma_bf16(tmem_base, ca_desc_mn(qa + kk * 2048, kCaBoxBytes), ca_desc_mn(ka + kk * 2048, kCaBoxBytes), idesc,
-                           (t > 0 || kk > 0) ? 1u : 0u);
-        ptx::tc_commit(ptx::smem_u32(empty + st));
-        if (t == n_tiles - 1) ptx::tc_commit(ptx::smem_u32(done));
+      for (int kk = 0; kk < kCaTok / 16; ++kk)      // 16 tokens per step: 16 rows x 128 B = 2048 B into each box
+        ptx::Wgmma<64>::template ss<1, 1>(acc, ptx::wgmma_desc_mn_sw128(qa + kk * 2048, kCaBoxBytes), ptx::wgmma_desc_mn_sw128(ka + kk * 2048, kCaBoxBytes),
+                                          (t > 0 || kk > 0) ? 1u : 0u);
+      ptx::wgmma_commit();
+      ptx::wgmma_wait<0>();
+      ptx::wgmma_fence_regs(acc);
+      if (lane == 0) ptx::mbar_arrive(ptx::smem_u32(empty + st));
+    }
+    // this warp's 16 rows lie in group (warp / 2) of the quad; of their 64 columns only that group's 32 are kept
+    const int gsel = (warp >> 1) & 1;                 // group inside the warpgroup's half
+    const int g = quad * 4 + (warp >> 1);
+    const int fr = lane >> 2, fq2 = (lane & 3) * 2;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = (warp & 1) * 16 + fr + 8 * h;   // row inside the group
+      if (g * 32 + row >= a.C) continue;
+      float* dst = a.part + ((((long long)chunk * a.B + b) * a.groups + g) * 32 + row) * 32;
+#pragma unroll
+      for (int cc = 0; cc < 4; ++cc) {
+        const float v0 = gsel ? acc[4 * (4 + cc) + 2 * h] : acc[4 * cc + 2 * h];
+        const float v1 = gsel ? acc[4 * (4 + cc) + 2 * h + 1] : acc[4 * cc + 2 * h + 1];
+        *reinterpret_cast<float2*>(dst + cc * 8 + fq2) = make_float2(v0, v1);
       }
-      __syncwarp();
-    }
-  } else {
-    const int quarter = warp & 3;
-    const int c1 = quarter * 32 + lane;                 // row of the quad's Gram == TMEM lane; its group = quarter
-    const int g = quad * 4 + quarter;
-    float* dst = a.part + ((((long long)chunk * a.B + b) * a.groups + g) * 32 + lane) * 32;
-    const bool live = quad * kCaQuad + c1 < a.C;
-    uint32_t r[32];
-    if (n_tiles > 0) {
-      ca_wait(done, 0);
-      ptx::tc_fence_after();
-      ptx::tmem_ld_32x32(tmem_base + ((uint32_t)(quarter * 32) << 16) + quarter * 32, r);   // the 32 columns of this row's own group
-      ptx::tmem_ld_wait();
-    } else {
-#pragma unroll
-      for (int j = 0; j < 32; ++j) r[j] = 0u;
-    }
-    if (live) {
-#pragma unroll
-      for (int q = 0; q < 8; ++q)
-        reinterpret_cast<float4*>(dst)[q] = make_float4(__uint_as_float(r[4 * q]), __uint_as_float(r[4 * q + 1]), __uint_as_float(r[4 * q + 2]),
-                                                        __uint_as_float(r[4 * q + 3]));
     }
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) ptx::tmem_dealloc(tmem_base, 128);
 }
 
 // ----------------------------------------------------------------------------------------------------- apply
 constexpr int kApplyB = 2 * kCaBoxBytes;                       // block-diagonal A as the B operand: two K blocks of [128][64]
 constexpr int kApplyStage = 2 * kCaBoxBytes;                   // v tile: two K blocks of [128 tokens][64 channels]
-constexpr int kApplyStaging = 4 * 32 * 256;                    // per epilogue warp: 32 rows x 256 B
+constexpr int kApplyStaging = (kCaConsumers / 32) * kFragStageBytes;   // per consumer warp: 16 rows x 256 B
 constexpr int kApplySmem = kApplyB + kCaStages * kApplyStage + kApplyStaging + 1024 + 128;
 
 __global__ void __launch_bounds__(kCaThreads, 1)
@@ -169,21 +146,16 @@ chan_apply_tc_kernel(const __grid_constant__ CUtensorMap tmV, const ChanArgs a) 
   uint64_t* bars = reinterpret_cast<uint64_t*>(sStg + kApplyStaging);
   uint64_t* full = bars;                      // [stages]
   uint64_t* empty = bars + kCaStages;         // [stages]
-  uint64_t* acc_full = bars + 2 * kCaStages;  // [2]
-  uint64_t* acc_empty = bars + 2 * kCaStages + 2;   // [2]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * kCaStages + 4);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int chunk = blockIdx.x, quad = blockIdx.y, b = blockIdx.z;
   const int tile0 = chunk * a.tiles_per_chunk;
   const int n_tiles = max(0, min(a.tiles_per_chunk, (a.N + kCaTok - 1) / kCaTok - tile0));
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     ptx::prefetch_tmap(&tmV);
-    for (int s = 0; s < kCaStages; ++s) { ptx::mbar_init(ptx::smem_u32(full + s), 1); ptx::mbar_init(ptx::smem_u32(empty + s), 1); }
-    for (int s = 0; s < 2; ++s) { ptx::mbar_init(ptx::smem_u32(acc_full + s), 1); ptx::mbar_init(ptx::smem_u32(acc_empty + s), 4); }
+    for (int s = 0; s < kCaStages; ++s) { ptx::mbar_init(ptx::smem_u32(full + s), 1); ptx::mbar_init(ptx::smem_u32(empty + s), kCaConsumers / 32); }
     ptx::mbar_fence_init();
   }
-  if (warp == 1) ptx::tmem_alloc(ptx::smem_u32(tmem_ptr), 256);
   // ---- the quad's block-diagonal softmax matrix as a K-major, 128B-swizzled B operand: row c1, 128 columns c2 ----
   if (threadIdx.x < 128) {
     const int c1 = threadIdx.x, grp = c1 >> 5;
@@ -226,12 +198,9 @@ chan_apply_tc_kernel(const __grid_constant__ CUtensorMap tmV, const ChanArgs a) 
     }
     ptx::fence_proxy_async_smem();
   }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
+  if (warp == kCaConsumers / 32) {
     if (ptx::elect_one()) {
       for (int t = 0; t < n_tiles; ++t) {
         const int st = t % kCaStages;
@@ -244,64 +213,48 @@ chan_apply_tc_kernel(const __grid_constant__ CUtensorMap tmV, const ChanArgs a) 
         ptx::tma_load_3d(ptx::smem_u32(base + kCaBoxBytes), &tmV, fb, quad * kCaQuad + 64, tok, b);
       }
     }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = ptx::umma_idesc_bf16(128, 128);
-    for (int t = 0; t < n_tiles; ++t) {
-      const int st = t % kCaStages, acc = t & 1;
-      ca_wait(full + st, (t / kCaStages) & 1);
-      if (t >= 2) ca_wait(acc_empty + acc, ((t >> 1) - 1) & 1);
-      ptx::tc_fence_after();
-      if (ptx::elect_one()) {
-        const uint32_t va = ptx::smem_u32(sV + st * kApplyStage), ba = ptx::smem_u32(sB);
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk)                 // K = 128 channels: two 64-wide K blocks x four 16-wide steps
-          ptx::tc_mma_bf16(tmem_base + acc * 128, ptx::umma_desc_k_sw128(va + (kk >> 2) * kCaBoxBytes + (kk & 3) * 32),
-                           ptx::umma_desc_k_sw128(ba + (kk >> 2) * kCaBoxBytes + (kk & 3) * 32), idesc, kk > 0 ? 1u : 0u);
-        ptx::tc_commit(ptx::smem_u32(empty + st));
-        ptx::tc_commit(ptx::smem_u32(acc_full + acc));
-      }
-      __syncwarp();
-    }
   } else {
-    const int quarter = warp & 3;
-    uint8_t* stg = sStg + (warp - 2) * 32 * 256;
+    const int wg = warp >> 2;                                        // tokens [64 wg, 64 wg + 64) of the tile
+    const int fr = lane >> 2, fq = lane & 3;
+    uint8_t* stg = sStg + warp * kFragStageBytes;
     const int cols_live = min(kCaQuad, a.C - quad * kCaQuad);        // channels of this quad that exist
+    const uint32_t ba = ptx::smem_u32(sB);
     for (int t = 0; t < n_tiles; ++t) {
-      const int acc = t & 1;
-      ca_wait(acc_full + acc, (t >> 1) & 1);
-      ptx::tc_fence_after();
-      const uint32_t taddr = tmem_base + acc * 128 + ((uint32_t)(quarter * 32) << 16);
+      const int st = t % kCaStages;
+      ca_wait(full + st, (t / kCaStages) & 1);
+      const uint32_t va = ptx::smem_u32(sV + st * kApplyStage) + wg * (64 * 128);
+      float acc[64];
 #pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint32_t r[32];
-        ptx::tmem_ld_32x32(taddr + c * 32, r);
-        ptx::tmem_ld_wait();
+      for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+      ptx::wgmma_fence_regs(acc);
+      ptx::wgmma_fence();
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const int ch = c * 4 + q;
-          *reinterpret_cast<uint4*>(stg + lane * 256 + (((ch & ~7) | ((ch ^ lane) & 7)) << 4)) =
-              make_uint4(pack_bf16(__uint_as_float(r[q * 8]), __uint_as_float(r[q * 8 + 1])), pack_bf16(__uint_as_float(r[q * 8 + 2]), __uint_as_float(r[q * 8 + 3])),
-                         pack_bf16(__uint_as_float(r[q * 8 + 4]), __uint_as_float(r[q * 8 + 5])), pack_bf16(__uint_as_float(r[q * 8 + 6]), __uint_as_float(r[q * 8 + 7])));
-        }
+      for (int kk = 0; kk < 8; ++kk)                 // K = 128 channels: two 64-wide K blocks x four 16-wide steps
+        ptx::Wgmma<128>::template ss<0, 0>(acc, ptx::wgmma_desc_k_sw128(va + (kk >> 2) * kCaBoxBytes + (kk & 3) * 32),
+                                           ptx::wgmma_desc_k_sw128(ba + (kk >> 2) * kCaBoxBytes + (kk & 3) * 32), kk > 0 ? 1u : 0u);
+      ptx::wgmma_commit();
+      ptx::wgmma_wait<0>();
+      ptx::wgmma_fence_regs(acc);
+      if (lane == 0) ptx::mbar_arrive(ptx::smem_u32(empty + st));     // the v tile has been read: the producer may refill the slot
+#pragma unroll
+      for (int c8 = 0; c8 < 16; ++c8) {
+        *frag_stage_word(stg, fr, c8 * 4 + fq) = pack_bf16(acc[4 * c8], acc[4 * c8 + 1]);
+        *frag_stage_word(stg, fr + 8, c8 * 4 + fq) = pack_bf16(acc[4 * c8 + 2], acc[4 * c8 + 3]);
       }
-      ptx::tc_fence_before();
       __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(ptx::smem_u32(acc_empty + acc));     // the accumulator is in shared memory: the MMA may reuse it
-      const int tok0 = (tile0 + t) * kCaTok + quarter * 32;
+      const int tok0 = (tile0 + t) * kCaTok + warp * 16;
       const int chunks = cols_live / 8;
       bf16* op = a.out + ((long long)b * a.N + tok0) * a.C + quad * kCaQuad;
-      for (int i = lane; i < 32 * chunks; i += 32) {
-        const int rr = i / chunks, ch = i - rr * chunks;
-        if (tok0 + rr < a.N)
-          *reinterpret_cast<uint4*>(op + (long long)rr * a.C + ch * 8) =
-              *reinterpret_cast<const uint4*>(stg + rr * 256 + (((ch & ~7) | ((ch ^ rr) & 7)) << 4));
+      const int slot = lane & 15;
+#pragma unroll
+      for (int it = 0; it < 8; ++it) {
+        const int rr = 2 * it + (lane >> 4);
+        if (slot < chunks && tok0 + rr < a.N)
+          *reinterpret_cast<uint4*>(op + (long long)rr * a.C + slot * 8) = frag_stage_slot(stg, rr, slot);
       }
       __syncwarp();
     }
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) ptx::tmem_dealloc(tmem_base, 256);
 }
 
 // ------------------------------------------------------------------------------------------------------ host
@@ -309,7 +262,7 @@ chan_apply_tc_kernel(const __grid_constant__ CUtensorMap tmV, const ChanArgs a) 
 // depend on how many neighbours it was batched with (tests/test_gpu_eval_drivers.py: generate_batch == one-by-one generate).
 static void chan_plan(int /*B*/, int N, int C, int* n_chunks, int* tiles_per_chunk) {
   const int quads = ceil_div(C, kCaQuad), tiles = ceil_div(N, kCaTok);
-  int n = ceil_div(2 * 148, std::max(1, quads));     // about two CTAs' worth of work per SM for ONE image; a batch only adds CTAs
+  int n = ceil_div(2 * 132, std::max(1, quads));     // about two CTAs' worth of work per SM for ONE image; a batch only adds CTAs
   n = std::max(1, std::min(n, std::min(tiles, kCaMaxChunks)));
   *tiles_per_chunk = ceil_div(tiles, n);
   *n_chunks = ceil_div(tiles, *tiles_per_chunk);

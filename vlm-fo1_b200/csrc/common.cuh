@@ -1,4 +1,4 @@
-// common.cuh -- shared host/device helpers for libfo1 (sm_100a only).
+// common.cuh -- shared host/device helpers for libfo1 (sm_90a only).
 #pragma once
 
 #include <cuda_bf16.h>
@@ -72,7 +72,7 @@ struct PdlScope {
   explicit PdlScope(bool on) : prev(t_pdl) { t_pdl = on; }
   ~PdlScope() { t_pdl = prev; }
 };
-// Split-K of skinny GEMMs (gemm_tcgen05.cu's automatic choice) is allowed only inside a SplitKScope: the decode steps and the LM head
+// Split-K of skinny GEMMs (gemm_wgmma.cu's automatic choice) is allowed only inside a SplitKScope: the decode steps and the LM head
 // (M = number of sequences: weight streaming, where the choice depends on N and K only) and the public fo1_gemm_bf16.  Every other
 // linear() of the engine keeps ONE accumulation order whatever its M, so a sample's tower / projector / prefill results do not depend
 // on how many neighbours shared its batch (a short prompt alone used to take split-K, the same prompt inside a batch did not).

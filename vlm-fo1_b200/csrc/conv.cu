@@ -1,6 +1,6 @@
 // conv.cu -- spatial kernels of the DaViT tower and SimpleFPN over channels-last bf16 maps [B][H][W][C]:
 // depth-wise 3x3 (+bias +residual), im2col feeders for the dense convolutions (which then run on the
-// tcgen05 GEMM), 2x2 max-pool, and DaViT's channel-group attention.  All memory-bound SIMT kernels.
+// wgmma GEMM), 2x2 max-pool, and DaViT's channel-group attention.  All memory-bound SIMT kernels.
 #include "kernels.cuh"
 
 namespace fo1 {
@@ -226,7 +226,7 @@ __global__ void __launch_bounds__(256) window_reverse_add_kernel(const bf16* __r
 
 static inline int grid_for(long long items) {
   long long b = (items + 255) / 256;
-  const long long cap = 148LL * 32;
+  const long long cap = device_sm_count() * 32LL;
   return (int)(b < 1 ? 1 : (b > cap ? cap : b));
 }
 
@@ -309,7 +309,7 @@ int pixel_shuffle2x(const bf16* src, bf16* dst, int B, int H, int W, int C, cuda
   if ((long long)B * H * W == 0) return FO1_OK;
   long long items = (long long)B * H * W * 4 * (C / 8);
   long long blocks = (items + 255) / 256;
-  if (blocks > 148LL * 32) blocks = 148LL * 32;
+  if (blocks > device_sm_count() * 32LL) blocks = device_sm_count() * 32LL;
   pixel_shuffle2x_kernel<<<(int)blocks, 256, 0, s>>>(src, dst, B, H, W, C);
   FO1_LAUNCH_CHECK();
   return FO1_OK;

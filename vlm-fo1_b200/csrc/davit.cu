@@ -3,7 +3,7 @@
 // DaViT.forward_features (modeling_davit.py:478-506): 4 stages of [ConvEmbed -> depth x (SpatialBlock,
 // ChannelBlock)], each stage's token map returned.  Tokens stay channels-last [B*H*W][C] bf16 throughout
 // (the reference bounces between NCHW and token layouts at every depth-wise conv, :91-99); dense convs are
-// im2col + tcgen05 GEMM; LayerNorm / depth-wise conv / window (un)partition / channel attention are
+// im2col + wgmma GEMM; LayerNorm / depth-wise conv / window (un)partition / channel attention are
 // memory-bound SIMT kernels; biases, GELU and residual adds ride in the GEMM epilogues.
 #include "engine.cuh"
 

@@ -102,8 +102,7 @@ __device__ __forceinline__ unsigned long long mg_now() {
 
 // grid-wide barrier: monotonically increasing arrival counter (zeroed by the host), generation g completes at g * gridDim.x.
 // Thread 0 brackets the arrive / spin with __threadfence() (MEMBAR.SC.GPU), the cooperative-groups pattern.  A variant relying on
-// red.release / ld.acquire alone measured 0.7 us less per crossing and passed the same tests; the conservative form is kept because the
-// round's GPU budget ran out before the lighter one could be soaked.
+// red.release / ld.acquire alone is lighter; the conservative form is kept until the lighter one has been soaked.
 __device__ __forceinline__ void mg_grid_sync(unsigned* bar, unsigned& gen) {
   __syncthreads();
   gen += 1;
@@ -150,8 +149,8 @@ struct MgWork {
   }
 };
 
-// Per-warp cp.async ring.  (A ring of cp.async.bulk copies from a tile-contiguous weight image was measured too: faster in an empty
-// streaming loop -- scripts/probes/stream_probe.cu, 5.4 vs 4.0 TB/s -- but slower here, because expect_tx + the bulk issue + the
+// Per-warp cp.async ring.  (A ring of cp.async.bulk copies from a tile-contiguous weight image was tried too: faster in an empty
+// streaming loop (scripts/probes/stream_probe.cu) but slower here, because expect_tx + the bulk issue + the
 // mbarrier wait cost this latency-bound loop ~500 cycles more per 2-4 KB stage than four cp.async per lane and a wait_group.)
 // Also measured and rejected: the A fragments of the K <= 2048 phases kept in registers to free the 128 KB activation tile for the ring
 // (spills at the 255-register cap, step time doubled).

@@ -1,4 +1,4 @@
-// hfre.cu -- Hybrid Fine-grained Region Encoder on sm_100a: separable-window region pooling.
+// hfre.cu -- Hybrid Fine-grained Region Encoder on sm_90a: separable-window region pooling.
 //
 // What the reference does (hybrid_finegrained_region_encoder.py:319-363, 230-273): up-sample aux
 // levels 1..3 to level 0's grid (F.interpolate bilinear, align_corners=False), concatenate to a
@@ -15,8 +15,8 @@
 // (fo1_hfre_params.algo): the per-box gather (coalesced 16-byte channel vectors, fp32 FMA), the SIMT map sweep (every
 // cell read once, FMA per covering box) and -- the default above a handful of boxes -- the map sweep whose row sums
 // run as mma.sync m16n8k16 tiles (boxes x cells, column weights split hi + lo in bf16): the bytes are still read
-// exactly once with coalesced accesses, the legacy tensor path only replaces the FMA issue slots that capped the SIMT
-// sweep at 10 % of the HBM roofline (DESIGN.md section 4).
+// exactly once with coalesced accesses, the legacy tensor path only replaces the FMA issue slots that cap the SIMT
+// sweep (DESIGN.md section 4).
 #include "common.cuh"
 
 namespace fo1 {
@@ -313,17 +313,17 @@ __global__ void __launch_bounds__(kGatherThreads) hfre_gather_kernel(const Batch
 // channel) at the end.  Per cell and covering box the work is 2 FMA per bf16 pair -- the SIMT FMA
 // rate, not HBM, is then the co-limiter (DESIGN.md section 4).
 // ------------------------------------------------------------------------------------------------
-// packed fp32x2 helpers: one FFMA2 does the two channels a lane owns (sm_100 `fma.rn.f32x2`; a {w, w} pair becomes
-// the instruction's scalar-broadcast operand)
+// fp32 pair helpers: the two channels a lane owns travel as one 64-bit value ({w, w} pairs broadcast a weight); sm_90 has no
+// packed fp32 FMA, so f2_fma is two scalar FMAs
 __device__ __forceinline__ unsigned long long f2_pack(float lo, float hi) {
   unsigned long long r;
   asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
   return r;
 }
+__device__ __forceinline__ float2 f2_unpack(unsigned long long v);
 __device__ __forceinline__ unsigned long long f2_fma(unsigned long long a, unsigned long long b, unsigned long long c) {
-  unsigned long long d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  const float2 x = f2_unpack(a), y = f2_unpack(b), z = f2_unpack(c);
+  return f2_pack(fmaf(x.x, y.x, z.x), fmaf(x.y, y.y, z.y));
 }
 __device__ __forceinline__ float2 f2_unpack(unsigned long long v) {
   float2 r;
@@ -510,8 +510,7 @@ __global__ void __launch_bounds__(kSweepThreads) hfre_sweep_kernel(const BatchDe
 
 // ------------------------------------------------------------------------------------------------
 // Kernel 3'' (algo 3, map sweep on the tensor pipe).  At C2's box density every cell is covered by ~7 boxes, i.e.
-// ~7.5 FLOP per loaded byte: with the bf16 -> fp32 unpacking the SIMT sweep is issue-bound at ~1/8 of the HBM roofline
-// (profiles/: FMA pipe 26 %, 488 M warp instructions for 1.3 GB).  The reduction is a contraction,
+// ~7.5 FLOP per loaded byte: with the bf16 -> fp32 unpacking the SIMT sweep is bound by FMA issue, not by HBM.  The reduction is a contraction,
 //     out[box][c] += sum_y a_y[box] * ( sum_x b_x[box] * L[y][x][c] ),
 // so the inner sum over a region row runs as mma.sync m16n8k16 (A = b_x of 16 boxes, B = 16 cells x 8 channels of
 // the bf16 map, fp32 accumulate) and only the per-row scaling by a_y stays on the FMA pipe (1 FMA per 32 MACs).
@@ -811,7 +810,7 @@ extern "C" int fo1_hfre_forward(const fo1_hfre_image* images, int32_t n_images, 
     int batch_boxes = 0;
     for (int i = 0; i < B.n_images; ++i) batch_boxes += images[base + i].n_boxes > 0 ? images[base + i].n_boxes : 0;
     // algo 0: a sweep wins as soon as boxes overlap (its traffic is the union of the windows, the gather's their sum),
-    // and the tensor-pipe sweep beats the SIMT one at every density measured (profiles/r01_microbench_hfre_*.json)
+    // and the tensor-pipe sweep takes the FMA issue slots out of the SIMT one
     const bool sweep = p->algo == 2 || p->algo == 3 || (p->algo == 0 && batch_boxes >= 8 * B.n_images);
     const bool tensor = p->algo == 3 || (p->algo == 0 && sweep);
     B.rrows = tensor ? kMmaRows : kRegion;

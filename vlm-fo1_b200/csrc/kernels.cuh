@@ -10,7 +10,7 @@ namespace fo1 {
 
 typedef __nv_bfloat16 bf16;
 
-// ---- gemm_tcgen05.cu ----
+// ---- gemm_wgmma.cu ----
 int gemm_bf16(const fo1_gemm_desc* d, cudaStream_t stream);
 int device_sm_count();
 // convenience: D = act(A.W^T + bias) + residual, all row-major contiguous unless ld given
@@ -41,7 +41,7 @@ int rope_kv_append(bf16* qkv, long long ld, const float* cos_sin, int T, int q_h
                    bf16* kc, bf16* vc, int cap, cudaStream_t s);
 
 // ---- attention_tc.cu ----
-// varlen flash attention over packed rows (tcgen05 / TMEM / TMA); q/k/v may live in one packed buffer (pitches in elements)
+// varlen flash attention over packed rows (wgmma / TMA); q/k/v may live in one packed buffer (pitches in elements)
 struct AttnArgs {
   const bf16* q; const bf16* k; const bf16* v; bf16* o;
   long long ldq, ldk, ldv, ldo;     // row pitches (elements)
@@ -78,7 +78,7 @@ int dwconv3x3_residual(const bf16* x, const bf16* w9, const bf16* bias, bf16* y,
 int im2col3x3(const bf16* x, bf16* col, int B, int H, int W, int C, int stride, cudaStream_t s);
 int im2col_stem(const float* img, bf16* col, int H, int W, int kpad, cudaStream_t s);
 int maxpool2x2(const bf16* x, bf16* y, int B, int H, int W, int C, cudaStream_t s);
-// ---- chanattn_tc.cu: DaViT channel-group attention as two tcgen05 contractions; ws = channel_attention_ws_floats() floats
+// ---- chanattn_tc.cu: DaViT channel-group attention as two wgmma contractions; ws = channel_attention_ws_floats() floats
 size_t channel_attention_ws_floats(int B, int N, int C);
 int channel_attention(const bf16* qkv, float* ws, bf16* out, int B, int N, int C, int groups, cudaStream_t s);
 int window_partition(const bf16* x, bf16* dst, int B, int H, int W, int C, int ws, cudaStream_t s);

@@ -1,11 +1,11 @@
-// llm.cu -- Qwen2.5 decoder on sm_100a: embedding splice, M-RoPE bookkeeping, varlen prefill, device-resident
+// llm.cu -- Qwen2.5 decoder on sm_90a: embedding splice, M-RoPE bookkeeping, varlen prefill, device-resident
 // greedy decode with a static K/V cache.
 //
 // Reference: OmChatQwen25VLForCausalLM.forward + prepare_inputs_labels_for_qwen2_5_vl_multimodal
 // (omchat_qwen2_5_vl.py:135-532), Qwen2_5_VLModel / DecoderLayer / Attention / MLP / RMSNorm
 // (modeling_qwen2_5_vl.py:1126-1242, 1014-1095, 738-802, 627-640, 126-140), get_rope_index (:1546-1721),
 // the decode position rule (:1848-1860) and HF's greedy loop with KeywordsStoppingCriteria (mm_utils.py:137-181).
-// B200-first differences: all sequences of the batch run packed (varlen), no padding tokens exist; K/V live
+// Differences from the reference: all sequences of the batch run packed (varlen), no padding tokens exist; K/V live
 // in one static [layer][seq][cap][kv] cache written by the prefill and appended in place by each decode
 // step (the reference torch.cat's a DynamicCache per layer per step); argmax, stop-token test and all loop
 // state stay on the device, the host only enqueues kernels (no per-token sync); lm_head runs on the last
@@ -55,7 +55,7 @@ __global__ void __launch_bounds__(128) kv_store_kernel(const bf16* __restrict__ 
 // (rows G..15 are zero), so K and V are read ONCE per kv head instead of once per query head.  Every warp owns
 // 16-key tiles of the split and streams them through a private cp.async ring (3 tiles = 24 KB, two in flight behind
 // the one being reduced; 16-byte chunks XOR-swizzled by key) -- the load -> use chain of a register-fed version left
-// a warp with one tile in flight and the kernel at 1.3 TB/s.  S = Q.K^T takes its B fragments with ldmatrix, P.V with
+// a warp with one tile in flight.  S = Q.K^T takes its B fragments with ldmatrix, P.V with
 // ldmatrix.trans; the block merges its warps' (m, l, acc) and writes one un-normalised partial per (head, split);
 // decode_attn_combine_kernel merges the splits.
 constexpr int kDecSplits = 8;   // most key splits per (sequence, kv head); the launch uses gridDim.z <= kDecSplits of them
@@ -531,9 +531,8 @@ static int llm_generate_impl(Model* m, fo1_generate_desc* d, cudaStream_t s, boo
   int* d_lens = A.alloc<int>(B);
   int* d_deltas = A.alloc<int>(B);
   // persistent decode kernel (decode_mega.cu): per-CTA slots + the grid barrier
-  // measured with warm clocks, alternating the two paths (scripts/mega_prof.py, profiles/README.md round 2): the persistent kernel
-  // beats the per-kernel graph at every batch it supports (1..32 sequences: -8 % .. -19 % per step).  FO1_MEGA_MAX_B lowers the
-  // threshold, FO1_NO_MEGA disables the kernel.
+  // the persistent kernel serves every batch it supports (1..32 sequences; scripts/mega_prof.py times the two paths alternately).
+  // FO1_MEGA_MAX_B lowers the threshold, FO1_NO_MEGA disables the kernel.
   int mega_max_b = 32;
   if (const char* e = getenv("FO1_MEGA_MAX_B")) mega_max_b = std::max(0, std::min(32, atoi(e)));
   const int mega_grid = (m->llm.mega_ok && B <= mega_max_b && getenv("FO1_NO_MEGA") == nullptr) ? decode_mega_grid() : 0;

@@ -48,7 +48,7 @@ __global__ void gelu_kernel(const bf16* __restrict__ x, bf16* __restrict__ y, lo
 
 static inline int grid1d(long long work_items, int per_block) {
   long long b = (work_items + per_block - 1) / per_block;
-  const long long cap = 148LL * 32;
+  const long long cap = device_sm_count() * 32LL;
   return (int)(b < 1 ? 1 : (b > cap ? cap : b));
 }
 

@@ -1,6 +1,8 @@
-// ptx.cuh -- thin inline-PTX wrappers for the sm_100a async machinery: mbarrier, TMA, tcgen05, TMEM.
+// ptx.cuh -- thin inline-PTX wrappers for the sm_90a async machinery: mbarrier, TMA, wgmma.
 #pragma once
 #include <stdint.h>
+
+#include "wgmma.cuh"
 
 namespace fo1 {
 namespace ptx {
@@ -65,143 +67,57 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const void* tmap, uint
       : "memory");
 }
 
-// ---- tcgen05 / TMEM ----------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], bf16 x bf16 -> fp32, issued by ONE thread
-__device__ __forceinline__ void tc_mma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n.reg .pred P;\nsetp.ne.b32 P, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, P;\n}\n"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns: thread t gets lane (base + t), columns [col, col+32)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 32 consecutive fp32 columns, registers -> TMEM (the mirror of tmem_ld_32x32)
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-        "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]),
-        "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]),
-        "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// generic-proxy shared-memory writes (st.shared) -> visible to the async proxy (tcgen05.mma / TMA reads)
+// ---- wgmma (warpgroup MMA; the instruction wrappers are in wgmma.cuh) ---------------------------
+// generic-proxy shared-memory writes (st.shared) -> visible to the async proxy (wgmma / TMA reads)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
-// MN-major, 128-byte-swizzled operand (e.g. V[key][dim] used as the B operand of P.V: N = dim is the contiguous
-// direction): rows of 128 B = 64 MN-elements of one K index, 8-row (8 K indices) groups SBO = 1024 B apart; a single
-// 64-element atom along MN, so the leading byte offset is not used (cute::UMMA::make_umma_desc<Major::MN>).
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)(8192 >> 4) << 16;                    // LBO: next 64-element atom along MN (unused: N <= 64)
-  d |= (uint64_t)(1024 >> 4) << 32;                    // SBO: next group of 8 K indices
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;                              // SWIZZLE_128B
-  return d;
+// orders the warpgroup's register / shared-memory accesses before the wgmma.mma_async that follow
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses to accumulator registers across an in-flight wgmma
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-constexpr uint32_t kUmmaBMajorMN = 1u << 16;           // instruction-descriptor bit: B operand is MN-major
 
-// K-major, 128-byte-swizzled shared-memory operand descriptor (UMMA SmemDescriptor, sm_100 version 1):
-// rows of 128 B, 8-row swizzle atoms 1024 B apart (SBO), LBO unused for a single K atom.
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t smem_addr) {
+// K-major, 128-byte-swizzled shared-memory operand descriptor: rows of 128 B (64 bf16 of K), 8-row swizzle atoms
+// 1024 B apart (SBO); LBO is not used for a single 64-element K atom.  A 16-element K step inside the atom advances
+// the start address by 32 B.
+__device__ __forceinline__ uint64_t wgmma_desc_k_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);          // start address, 16-byte units
-  d |= (uint64_t)0 << 16;                              // leading byte offset
+  d |= (uint64_t)1 << 16;                              // leading byte offset (ignored)
   d |= (uint64_t)(1024 >> 4) << 32;                    // stride byte offset between 8-row groups
-  d |= (uint64_t)1 << 46;                              // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;                              // SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                              // SWIZZLE_128B
   return d;
 }
-// kind::f16 instruction descriptor: bf16 A/B (K-major), fp32 accumulate, M x N tile
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(uint32_t M, uint32_t N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
+// MN-major, 128-byte-swizzled operand (a [K index][64 MN-elements] TMA tile used with the transpose bit, e.g. V[key][dim]
+// as the B operand of P.V): rows of 128 B = 64 MN-elements of one K index, 8-row (8 K indices) groups SBO = 1024 B
+// apart, 64-element atoms along MN `lbo` bytes apart.  A 16-element K step advances the start address by 2048 B.
+__device__ __forceinline__ uint64_t wgmma_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
+  d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;
+  d |= (uint64_t)(1024 >> 4) << 32;
+  d |= (uint64_t)1 << 62;
+  return d;
 }
 
 }  // namespace ptx
 
-namespace ptx {
-// ---- CTA pair (cta_group::2): two CTAs of a cluster share one 256-row MMA, each holding its 128 rows of A and half of B ---------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
+// ---- accumulator fragments -> row-contiguous global stores -----------------------------------------------------------
+// A warp of a warpgroup owns 16 accumulator rows; lane l holds rows l / 4 and l / 4 + 8, two adjacent columns per
+// 8-column chunk.  Storing from there writes 8 rows x 16 B per instruction, so the warp parks 16 rows x 256 B in shared
+// memory (16-byte slots XOR-swizzled by row: conflict-free both ways) and writes whole 256-byte rows back.
+constexpr int kFragStageBytes = 16 * 256;
+// 4-byte word `w` (0..63) of row `row` (0..15) of a warp's staging block
+__device__ __forceinline__ uint32_t* frag_stage_word(uint8_t* stg, int row, int w) {
+  return reinterpret_cast<uint32_t*>(stg + row * 256 + ((((w >> 2) ^ (row & 7)) << 4) | ((w & 3) << 2)));
 }
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\nbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+__device__ __forceinline__ uint4 frag_stage_slot(const uint8_t* stg, int row, int slot) {
+  return *reinterpret_cast<const uint4*>(stg + row * 256 + ((slot ^ (row & 7)) << 4));
 }
-// shared::cluster address of the same shared-memory offset in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_rank(uint32_t addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void mbar_fence_init_cluster() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t dst_smem, uint32_t ncols) {  // whole warp, in BOTH CTAs of the pair
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// arrive on the mbarrier at this offset in every CTA of `mask` when the pair's previously issued MMAs have completed
-__device__ __forceinline__ void tc_commit_pair(uint32_t bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(mask) : "memory");
-}
-__device__ __forceinline__ void tc_mma_bf16_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n.reg .pred P;\nsetp.ne.b32 P, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, P;\n}\n"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// TMA tile into THIS CTA's shared memory, bytes credited to an mbarrier that may live in the pair's other CTA (cluster address)
-__device__ __forceinline__ void tma_load_2d_pair(uint32_t dst, const void* tmap, uint32_t bar_cluster, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(tmap), "r"(bar_cluster), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_pair(uint32_t dst, const void* tmap, uint32_t bar_cluster, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(dst), "l"(tmap), "r"(bar_cluster), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-
-}  // namespace ptx
 
 }  // namespace fo1

@@ -101,7 +101,7 @@ int rope_kv_append(bf16* qkv, long long ld, const float* cos_sin, int T, int q_h
   FO1_CHECK_ARG(head_dim % 16 == 0 && ld % 8 == 0, "rope_kv_append: head_dim %d must be a multiple of 16 and the pitch of 8", head_dim);
   if (T == 0) return FO1_OK;
   const long long n = (long long)T * (q_heads + kv_heads) * (head_dim / 16) + (long long)T * kv_heads * head_dim / 8;
-  const int blocks = (int)((n + 255) / 256 < 148 * 16 ? (n + 255) / 256 : 148 * 16);
+  const int blocks = (int)((n + 255) / 256 < device_sm_count() * 16 ? (n + 255) / 256 : device_sm_count() * 16);
   launch_k(rope_kv_append_kernel, dim3(blocks), dim3(256), 0, s, qkv, ld, cos_sin, T, q_heads, kv_heads, head_dim, cache_len, kc, vc, cap);
   FO1_LAUNCH_CHECK();
   return FO1_OK;
@@ -120,7 +120,7 @@ int rope_apply(bf16* x, long long ld, const float* cos_sin, int T, int n_heads, 
   FO1_CHECK_ARG(head_dim % 16 == 0 && ld % 8 == 0, "rope_apply: head_dim %d must be a multiple of 16 and the pitch of 8", head_dim);
   if (T == 0) return FO1_OK;
   const long long n = (long long)T * n_heads * (head_dim / 16);
-  const int blocks = (int)((n + 255) / 256 < 148 * 16 ? (n + 255) / 256 : 148 * 16);
+  const int blocks = (int)((n + 255) / 256 < device_sm_count() * 16 ? (n + 255) / 256 : device_sm_count() * 16);
   rope_apply_kernel<<<blocks, 256, 0, s>>>(x, ld, cos_sin, T, n_heads, head_dim);
   FO1_LAUNCH_CHECK();
   return FO1_OK;

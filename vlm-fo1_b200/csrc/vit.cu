@@ -4,7 +4,7 @@
 // order, `depth` blocks of [RMSNorm -> qkv -> 2-D RoPE -> varlen attention (64-token windows, or whole
 // image at the full-attention layers) -> proj + residual -> RMSNorm -> gated-SiLU MLP + residual], hidden
 // state tapped after every full-attention layer, 2x2 merger MLP, inverse permutation.
-// B200-first differences: all images of the batch run as ONE packed token sequence; the window
+// Differences from the reference: all images of the batch run as ONE packed token sequence; the window
 // permutation is folded into the fp32->bf16 cast of the pixel rows; the taps are scattered straight
 // into un-windowed channels-last maps (what the reference builds later with cat/argsort/permute in
 // extract_multi_level_features :37-80); bias / activation / residual live in the GEMM epilogues.

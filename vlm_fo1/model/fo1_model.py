@@ -1,7 +1,7 @@
 """The object ``load_pretrained_model`` returns in place of the reference's ``OmChatQwen25VLForCausalLM``
 (vlm_fo1/model/language_model/omchat_qwen2_5_vl.py:28-41): same ``.config`` attributes the callers read, same
 ``.generate(**kwargs)`` contract (mm_utils.py:640-654 builds the kwargs; returns LongTensor [1, P + T] whose first P
-columns are ``inputs``), everything underneath delegated to the B200 engine."""
+columns are ``inputs``), everything underneath delegated to the H100 engine."""
 from __future__ import annotations
 
 from importlib import import_module
