@@ -77,9 +77,9 @@ def make_hfre_inputs(B, S, N, seed=0):
     return aux_all, pyr_all, ba, bv, grids
 
 
-def bench_hfre(results, B=8, S=896, N=100, algo=0):
+def bench_hfre(results, B=8, S=896, N=100):
     aux_all, pyr_all, ba, bv, grids = make_hfre_inputs(B, S, N)
-    cfg = H.HfreConfig(region_dim=5888, vt_mode="fpn", algo=algo)
+    cfg = H.HfreConfig(region_dim=5888, vt_mode="fpn")
     tot_unique = tot_gather = 0
     for b in range(B):
         shapes = [tuple(a.shape) for a in aux_all[b]] + [tuple(p.shape) for p in pyr_all[b]]
@@ -90,7 +90,7 @@ def bench_hfre(results, B=8, S=896, N=100, algo=0):
         ab = H.algorithmic_bytes(shapes, boxes_l, scales, ups, N, 5888)
         tot_unique += ab["unique_bytes"]; tot_gather += ab["gather_bytes"]
     med, best = timeit(lambda: H.hfre_forward(aux_all, pyr_all, ba, bv, cfg, grids), iters=10)
-    # one profiled pass: CUDA-event time of each tagged kernel (the sweep / gather is the roofline kernel)
+    # one profiled pass: CUDA-event time of each tagged kernel (the sweep is the roofline kernel)
     import ctypes as C
     L = import_module("vlm-fo1_b200._lib").lib()
     L.fo1_profile_enable(1)
@@ -103,8 +103,8 @@ def bench_hfre(results, B=8, S=896, N=100, algo=0):
     L.fo1_profile_enable(0)
     prof = json.loads(buf.value.decode())
     kern = {k: round(v["ms"] / v["launches"], 4) for k, v in prof.items()}
-    main = kern.get("hfre_sweep_mma") or kern.get("hfre_sweep") or kern.get("hfre_gather")
-    r = {"kind": "hfre", "algo": algo, "B": B, "S": S, "N": N, "ms": med, "kernel_ms": kern,
+    main = kern["hfre_sweep_mma"]
+    r = {"kind": "hfre", "B": B, "S": S, "N": N, "ms": med, "kernel_ms": kern,
          "kernel_unique_GBs": tot_unique / main / 1e6, "kernel_frac_of_measured_hbm": tot_unique / main / 1e6 / PEAKS["hbm_gbs"], "ms_best": best, "unique_MB": tot_unique / 1e6, "gather_MB": tot_gather / 1e6,
          "unique_GBs": tot_unique / med / 1e6, "gather_GBs": tot_gather / med / 1e6,
          "frac_of_measured_hbm": tot_unique / med / 1e6 / PEAKS["hbm_gbs"]}
@@ -134,10 +134,9 @@ if __name__ == "__main__":
     res = []
     print("device", torch.cuda.get_device_name(0), "cpus", os.cpu_count(), flush=True)
     if "hfre" in which:
-        for algo in (1, 2, 3):
-            bench_hfre(res, algo=algo)
-        for algo in (1, 2, 3):
-            bench_hfre(res, B=8, S=896, N=32, algo=algo)     # COCO-like box count (mean 31.5)
+        bench_hfre(res)
+        bench_hfre(res, B=8, S=896, N=32)     # COCO-like box count (mean 31.5)
+        bench_hfre(res, B=8, S=896, N=4)      # few boxes per image
     if "gemm" in which:
         bench_gemm(res)
     if "decode" in which:

@@ -66,7 +66,7 @@ def _bf16_round(x):
 
 
 def hfre_level_tensor_sweep(feat_hwc, boxes, scale, P, up_hw, region_rows=8, region_cols=32):
-    """Model of hfre_sweep_mma_kernel (algo 3): per (8 x 32)-cell region and box, the row sums over the region's columns
+    """Model of hfre_sweep_mma_kernel: per (8 x 32)-cell region and box, the row sums over the region's columns
     use the column weights as hi + lo bf16 halves against the bf16 map (products exact, fp32 accumulation), the row
     weight a_y is applied in fp32, regions are added into the output."""
     H, W, C = feat_hwc.shape

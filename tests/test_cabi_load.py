@@ -7,7 +7,7 @@ def test_library_loads_and_exports_header_symbols():
     G.build()
     import fo1_b200
     L = fo1_b200.lib()
-    assert L.fo1_abi_version() == 2
+    assert L.fo1_abi_version() == 3
     syms = fo1_b200._lib.exported_symbols()
     assert "fo1_hfre_forward" in syms and "fo1_gemm_bf16" in syms
     for s in syms:
@@ -23,8 +23,8 @@ def test_hfre_argument_validation_without_gpu():
     imgs = (HfreImage * 1)()
     imgs[0].n_levels = 0
     imgs[0].n_boxes = 1
-    p = HfreParams(64, 7, 1, 0)
+    p = HfreParams(64, 7, 1)
     rc = L.fo1_hfre_forward(imgs, 1, ctypes.byref(p), None, 0, None)
     assert rc != 0 and len(L.fo1_last_error()) > 0
-    p2 = HfreParams(64, 7, 1, 9)
+    p2 = HfreParams(66, 7, 1)   # out_dim not a multiple of 4
     assert L.fo1_hfre_forward(imgs, 1, ctypes.byref(p2), None, 0, None) == -1

@@ -29,7 +29,7 @@ def test_separable_weights_equal_oracle(golden_dir, tag):
 
 @pytest.mark.parametrize("tag", ["small", "rect"])
 def test_tensor_sweep_weight_split_stays_inside_the_parity_budget(golden_dir, tag):
-    """algo 3 feeds the fp32 column weights to the tensor pipe as hi + lo bf16 halves: on bf16-exact maps that must agree
+    """The sweep feeds the fp32 column weights to the tensor pipe as hi + lo bf16 halves: on bf16-exact maps that must agree
     with the fp64 separable sum to ~1e-5 (two orders inside the 1e-3 parity tolerance); a single bf16 half would not."""
     z = np.load(os.path.join(golden_dir, f"hfre_{tag}.npz"))
     aux = [KM._bf16_round(z[f"aux{i}"]) for i in range(4)]

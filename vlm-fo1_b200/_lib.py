@@ -31,8 +31,7 @@ class HfreImage(C.Structure):
 
 
 class HfreParams(C.Structure):
-    _fields_ = [("out_dim", C.c_int32), ("roi_size", C.c_int32), ("apply_pos_embed", C.c_int32),
-                ("algo", C.c_int32)]
+    _fields_ = [("out_dim", C.c_int32), ("roi_size", C.c_int32), ("apply_pos_embed", C.c_int32)]
 
 
 class GemmDesc(C.Structure):

@@ -11,25 +11,21 @@
 // because the up-sampling is linear and separable too, U[c] = Mh L[c] Mw^T, the whole thing is
 //        out[c] = (Mh^T a)^T L[c] (Mw^T b)
 // over the NATIVE-resolution bf16 level L (channels-last).  hfre_axis_weights_kernel builds the two weight vectors
-// per (box, level, axis) with torchvision's exact per-sample rules.  Three interchangeable reductions follow
-// (fo1_hfre_params.algo): the per-box gather (coalesced 16-byte channel vectors, fp32 FMA), the SIMT map sweep (every
-// cell read once, FMA per covering box) and -- the default above a handful of boxes -- the map sweep whose row sums
-// run as mma.sync m16n8k16 tiles (boxes x cells, column weights split hi + lo in bf16): the bytes are still read
-// exactly once with coalesced accesses, the legacy tensor path only replaces the FMA issue slots that cap the SIMT
-// sweep (DESIGN.md section 4).
+// per (box, level, axis) with torchvision's exact per-sample rules.  The reduction is a map sweep: a CTA owns a region
+// of one level's cells, reads each of them once with coalesced accesses, and runs the row sums of every box that covers
+// the region as mma.sync m16n8k16 tiles (boxes x cells, column weights split hi + lo in bf16).  The regions' partial
+// sums meet in fixed-point accumulators, so an image's features do not depend on the order of the CTAs nor on the
+// other images of the call (DESIGN.md sections 2 and 4).
 #include "common.cuh"
 
 namespace fo1 {
 
 constexpr int kMaxBatch = 32;          // images per launch: the batch descriptor travels as a kernel parameter (< 32 KB)
-constexpr int kGatherThreads = 256;
-constexpr int kChunk = 256;            // channels per gather block: 32 lanes x 8 bf16 (16 B) each
-constexpr int kRegion = 32;            // sweep: a CTA owns a kRegion x kRegion block of cells of one level
-constexpr int kSweepCh = 256;          // sweep: channels per CTA (4 warps x 32 lanes x 2 channels)
-constexpr int kSlots = 32;             // sweep: boxes accumulated concurrently per pass over the region
+constexpr int kRegion = 32;            // sweep: a CTA owns a kMmaRows x kRegion block of cells of one level
+constexpr int kSweepCh = 256;          // sweep: channels per CTA (4 warps x 64 channels)
 constexpr int kSweepThreads = 128;
-constexpr int kMmaRows = 8;            // tensor sweep: region = kMmaRows x kRegion cells, one 16-box m-tile per pass
-constexpr int kMmaSlots = 16;
+constexpr int kMmaRows = 8;
+constexpr int kMmaSlots = 16;          // boxes per pass over the region: one m16 tile
 
 struct LevelDev {
   const __nv_bfloat16* data;
@@ -39,30 +35,28 @@ struct LevelDev {
   int out_off;
   int wofs;      // float offset of this level's weight records inside the image's workspace slice
   int wstride;   // floats per box record: 4 header words + H + W, rounded up to 4
-  int lofs;      // int offset of this level's region box lists inside the image's list slice
-  int rh, rw;    // regions (kRegion x kRegion cells) per axis
+  int lofs;      // int offset of this level's region records inside the image's record slice
+  int rh, rw;    // regions (kMmaRows x kRegion cells) per axis
 };
 struct ImageDev {
   LevelDev lv[FO1_HFRE_MAX_LEVELS];
   const float* boxes[2];
   float* out;
   __nv_bfloat16* out_bf16;
-  long long* acc;    // sweeps: [n_boxes][out_dim] fixed-point (2^-32) accumulators -- integer atomics commute, so the sum does
+  long long* acc;    // [n_boxes][out_dim] fixed-point (2^-32) accumulators -- integer atomics commute, so the sum does
                      // not depend on the order in which the region CTAs arrive (bit-reproducible, unlike fp32 atomics)
   long long ws_ofs;  // float offset of this image's workspace slice
-  long long ls_ofs;  // int offset of this image's region-list slice (after all weight records)
-  int lstride;       // ints per region list: 1 count + n_boxes ids, rounded up to 4
+  long long ls_ofs;  // int offset of this image's region-record slice (after all weight records)
+  int lstride;       // ints per region: 4 header words (word 0 = count) + one kRecWords record per box
   int n_items;       // sweep work items: sum over levels of regions * ceil(C / kSweepCh)
   float pos_w, pos_h;
   int pos_box_set;
   int n_levels;
   int n_boxes;
-  int n_chunks;  // sum over levels of ceil(C / kChunk)
 };
 struct BatchDev {
   ImageDev img[kMaxBatch];
   int n_images;
-  int rrows;     // region height in cells used by the region lists / sweep of this launch (kRegion or kMmaRows)
   int out_dim;
   int roi;
   int pos;
@@ -225,142 +219,27 @@ __global__ void __launch_bounds__(256) hfre_pos_init_kernel(const BatchDev B) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// Kernel 3 (algo 1, per-box gather): one block per (image, box, level, 256-channel chunk).
-// 8 warps stride over the window's rows; each lane owns 8 consecutive channels (one 16-byte load per
-// cell, a warp reads 512 contiguous bytes per cell); fp32 accumulate; cross-warp reduce in smem.
+// Kernel 3: the map sweep.  Pooling box by box would re-read every cell once per covering box (~8x the unique bytes
+// at 100 boxes per image); the sweep inverts the loops: a CTA owns a region of one level, reads each of its cells ONCE
+// and reduces it against every box whose support meets the region.  At C2's box density every cell is covered by ~7
+// boxes, i.e. ~7.5 FLOP per loaded byte: on the FMA pipe, with the bf16 -> fp32 unpacking, that is bound by FMA issue,
+// not by HBM.  The reduction is a contraction,
+//     out[box][c] += sum_y a_y[box] * ( sum_x b_x[box] * L[y][x][c] ),
+// so the inner sum over a region row runs as mma.sync m16n8k16 (A = b_x of 16 boxes, B = 16 cells x 8 channels of
+// the bf16 map, fp32 accumulate) and only the per-row scaling by a_y stays on the FMA pipe (1 FMA per 32 MACs).
+// The fp32 weights are fed as hi + lo bf16 halves (two MMAs): the map is bf16 already, so products are exact and
+// the weights keep 16 mantissa bits -- inside the 1e-3 parity budget with three orders of margin.
+// Work split: CTA = (level, 8 x 32 cell region, 256 channels), warp = 64 channels, a pass accumulates 16 boxes (one
+// m-tile; regions with more boxes take further passes whose rows come from L2 -- 8-row regions keep the footprint of
+// all resident CTAs below the L2 size).  A fragments depend on the boxes only and are built once per pass from the
+// region's weight records (hfre_region_records_kernel).  Every region row is copied ONCE per pass into a per-warp
+// cp.async ring (3 rows, two in flight behind the one being reduced; 16-byte chunks XOR-swizzled by cell) and its
+// B fragments are taken with ldmatrix.trans.  The partial sums of the pass leave through shared memory (aliasing the
+// ring) as coalesced fixed-point reductions into acc[box][channel].
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kGatherThreads) hfre_gather_kernel(const BatchDev B, const float* __restrict__ ws) {
-  const ImageDev& im = B.img[blockIdx.z];
-  const int box = blockIdx.y;
-  if (box >= im.n_boxes || (int)blockIdx.x >= im.n_chunks) return;
-  // (level, chunk) of this block
-  int lvl = 0, chunk = blockIdx.x;
-  for (; lvl < im.n_levels; ++lvl) {
-    const int nc = (im.lv[lvl].C + kChunk - 1) / kChunk;
-    if (chunk < nc) break;
-    chunk -= nc;
-  }
-  const LevelDev& L = im.lv[lvl];
-  const float* rec = ws + im.ws_ofs + L.wofs + (long long)box * L.wstride;
-  const int* hdr = reinterpret_cast<const int*>(rec);
-  const int r0 = hdr[0], rl = hdr[1], c0 = hdr[2], cl = hdr[3];
-
-  extern __shared__ float sm[];
-  float* red = sm;                                  // [8][kChunk] (16-byte aligned for float4)
-  float* wa = sm + (kGatherThreads / 32) * kChunk;  // [rl]
-  float* wb = wa + L.H;                             // [cl]
-  for (int i = threadIdx.x; i < rl; i += blockDim.x) wa[i] = rec[4 + i];
-  for (int i = threadIdx.x; i < cl; i += blockDim.x) wb[i] = rec[4 + L.H + i];
-  __syncthreads();
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int cbase = chunk * kChunk + lane * 8;
-  const bool active = cbase < L.C;
-  float acc[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) acc[j] = 0.0f;
-
-  if (active) {
-    const long long rowpitch = (long long)L.W * L.C;
-    for (int r = warp; r < rl; r += kGatherThreads / 32) {
-      const float ar = wa[r];
-      const __nv_bfloat16* p = L.data + (long long)(r0 + r) * rowpitch + (long long)c0 * L.C + cbase;
-      int k = 0;
-      for (; k + 4 <= cl; k += 4) {
-        uint4 v[4];
-#pragma unroll
-        for (int u = 0; u < 4; ++u) v[u] = ldg_nc_v4(p + (long long)(k + u) * L.C);
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const float w = ar * wb[k + u];
-          acc[0] = fmaf(w, bf16_lo(v[u].x), acc[0]); acc[1] = fmaf(w, bf16_hi(v[u].x), acc[1]);
-          acc[2] = fmaf(w, bf16_lo(v[u].y), acc[2]); acc[3] = fmaf(w, bf16_hi(v[u].y), acc[3]);
-          acc[4] = fmaf(w, bf16_lo(v[u].z), acc[4]); acc[5] = fmaf(w, bf16_hi(v[u].z), acc[5]);
-          acc[6] = fmaf(w, bf16_lo(v[u].w), acc[6]); acc[7] = fmaf(w, bf16_hi(v[u].w), acc[7]);
-        }
-      }
-      for (; k < cl; ++k) {
-        const uint4 v = ldg_nc_v4(p + (long long)k * L.C);
-        const float w = ar * wb[k];
-        acc[0] = fmaf(w, bf16_lo(v.x), acc[0]); acc[1] = fmaf(w, bf16_hi(v.x), acc[1]);
-        acc[2] = fmaf(w, bf16_lo(v.y), acc[2]); acc[3] = fmaf(w, bf16_hi(v.y), acc[3]);
-        acc[4] = fmaf(w, bf16_lo(v.z), acc[4]); acc[5] = fmaf(w, bf16_hi(v.z), acc[5]);
-        acc[6] = fmaf(w, bf16_lo(v.w), acc[6]); acc[7] = fmaf(w, bf16_hi(v.w), acc[7]);
-      }
-    }
-  }
-  float4* rv = reinterpret_cast<float4*>(red + warp * kChunk + lane * 8);
-  rv[0] = make_float4(acc[0], acc[1], acc[2], acc[3]);
-  rv[1] = make_float4(acc[4], acc[5], acc[6], acc[7]);
-  __syncthreads();
-  const int c = chunk * kChunk + threadIdx.x;
-  if (c < L.C) {
-    float s = 0.0f;
-#pragma unroll
-    for (int w = 0; w < kGatherThreads / 32; ++w) s += red[w * kChunk + threadIdx.x];
-    float* o = im.out + (long long)box * B.out_dim + L.out_off + c;
-    *o += s;  // exclusive owner of this output element (kernel 2 initialised it)
-  }
-}
-
-
-// ------------------------------------------------------------------------------------------------
-// Kernel 3' (algo 2, map sweep).  The per-box gather above re-reads every cell once per covering box
-// (~8x the unique bytes at 100 boxes/image, L2-bound).  The sweep inverts the loops: a CTA owns a
-// 32x32-cell region x 256 channels of one level, reads each cell ONCE, and for every box whose
-// support meets the region accumulates a^T L b for its part, box accumulators living in shared
-// memory (lane-owned columns: no intra-CTA atomics); one fp32 red.global.add per (region, box,
-// channel) at the end.  Per cell and covering box the work is 2 FMA per bf16 pair -- the SIMT FMA
-// rate, not HBM, is then the co-limiter (DESIGN.md section 4).
-// ------------------------------------------------------------------------------------------------
-// fp32 pair helpers: the two channels a lane owns travel as one 64-bit value ({w, w} pairs broadcast a weight); sm_90 has no
-// packed fp32 FMA, so f2_fma is two scalar FMAs
-__device__ __forceinline__ unsigned long long f2_pack(float lo, float hi) {
-  unsigned long long r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ float2 f2_unpack(unsigned long long v);
-__device__ __forceinline__ unsigned long long f2_fma(unsigned long long a, unsigned long long b, unsigned long long c) {
-  const float2 x = f2_unpack(a), y = f2_unpack(b), z = f2_unpack(c);
-  return f2_pack(fmaf(x.x, y.x, z.x), fmaf(x.y, y.y, z.y));
-}
-__device__ __forceinline__ float2 f2_unpack(unsigned long long v) {
-  float2 r;
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(r.x), "=f"(r.y) : "l"(v));
-  return r;
-}
-
-__global__ void __launch_bounds__(32) hfre_region_lists_kernel(const BatchDev B, const float* __restrict__ ws, int* __restrict__ lists) {
-  const ImageDev& im = B.img[blockIdx.z];
-  const int lvl = blockIdx.y;
-  if (lvl >= im.n_levels) return;
-  const LevelDev& L = im.lv[lvl];
-  const int reg = blockIdx.x;
-  if (reg >= L.rh * L.rw) return;
-  const int ry = reg / L.rw, rx = reg % L.rw;
-  const int row0 = ry * B.rrows, row1 = min(row0 + B.rrows, L.H) - 1;
-  const int col0 = rx * kRegion, col1 = min(col0 + kRegion, L.W) - 1;
-  int* out = lists + im.ls_ofs + L.lofs + (long long)reg * im.lstride;
-  int count = 0;
-  for (int b0 = 0; b0 < im.n_boxes; b0 += 32) {
-    const int b = b0 + threadIdx.x;
-    bool hit = false;
-    if (b < im.n_boxes) {
-      const int* hdr = reinterpret_cast<const int*>(ws + im.ws_ofs + L.wofs + (long long)b * L.wstride);
-      const int r0 = hdr[0], r1 = hdr[0] + hdr[1] - 1, c0 = hdr[2], c1 = hdr[2] + hdr[3] - 1;
-      hit = r0 <= row1 && r1 >= row0 && c0 <= col1 && c1 >= col0;
-    }
-    const unsigned m = __ballot_sync(0xffffffffu, hit);
-    if (hit) out[1 + count + __popc(m & ((1u << threadIdx.x) - 1u))] = b;
-    count += __popc(m);
-  }
-  if (threadIdx.x == 0) out[0] = count;
-}
-
-// Tensor sweep variant of the region lists: besides the ids, every listed box gets its weights over the region's rows
-// and columns as one contiguous 48-word record (word 0 = box id, words 4..4+kMmaRows-1 = a_y, words 12..43 = b_x), so a
-// sweep pass stages its 16 boxes with ONE round of coalesced loads instead of the id -> header -> weights chain.
+// Region records, built before the sweep: every box whose support meets the region gets its weights over the region's
+// rows and columns as one contiguous 48-word record (word 0 = box id, words 4..4+kMmaRows-1 = a_y, words 12..43 = b_x),
+// so a sweep pass stages its 16 boxes with ONE round of coalesced loads instead of the id -> header -> weights chain.
 constexpr int kRecWords = 48;
 static_assert(kMmaRows <= 8 && kRegion == 32, "record layout: words 4..11 = a_y, words 12..43 = b_x");
 __global__ void __launch_bounds__(128) hfre_region_records_kernel(const BatchDev B, const float* __restrict__ ws, int* __restrict__ lists) {
@@ -406,124 +285,6 @@ __global__ void __launch_bounds__(128) hfre_region_records_kernel(const BatchDev
   }
 }
 
-__global__ void __launch_bounds__(kSweepThreads) hfre_sweep_kernel(const BatchDev B, const float* __restrict__ ws, const int* __restrict__ lists) {
-  const ImageDev& im = B.img[blockIdx.z];
-  if ((int)blockIdx.x >= im.n_items) return;
-  int lvl = 0, item = blockIdx.x;
-  for (; lvl < im.n_levels; ++lvl) {
-    const int n = im.lv[lvl].rh * im.lv[lvl].rw * ((im.lv[lvl].C + kSweepCh - 1) / kSweepCh);
-    if (item < n) break;
-    item -= n;
-  }
-  const LevelDev& L = im.lv[lvl];
-  const int n_reg = L.rh * L.rw;
-  const int cgroup = item / n_reg, reg = item % n_reg;
-  const int* list = lists + im.ls_ofs + L.lofs + (long long)reg * im.lstride;
-  const int n_list = list[0];
-  if (n_list == 0) return;  // no box touches this region: its cells are never read
-  const int ry = reg / L.rw, rx = reg % L.rw;
-  const int row0 = ry * kRegion, col0 = rx * kRegion;
-
-  __shared__ __align__(16) float s_acc[kSlots][kSweepCh];
-  __shared__ __align__(16) float s_wa[kSlots][kRegion];
-  __shared__ __align__(16) float s_wb[kSlots][kRegion];
-  __shared__ int s_box[kSlots];
-  __shared__ int s_rmask[kSlots], s_cmask[kSlots];   // which 8-row / 8-col tile bands carry non-zero weights
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int cbase = cgroup * kSweepCh + warp * 64 + lane * 2;
-  const bool active = cbase < L.C;
-  const long long rowpitch = (long long)L.W * L.C;
-
-  for (int base = 0; base < n_list; base += kSlots) {
-    const int ns = min(kSlots, n_list - base);
-    // ---- stage this pass's boxes: ids, dense weights over the region's rows / cols, band masks ----
-    if (threadIdx.x < kSlots) {
-      s_box[threadIdx.x] = threadIdx.x < ns ? list[1 + base + threadIdx.x] : -1;
-      s_rmask[threadIdx.x] = 0; s_cmask[threadIdx.x] = 0;
-    }
-    __syncthreads();
-    for (int i = threadIdx.x; i < ns * kRegion * 2; i += kSweepThreads) {
-      const int sl = i / (kRegion * 2), j = i % (kRegion * 2);
-      const int axis = j / kRegion, k = j % kRegion;
-      const float* rec = ws + im.ws_ofs + L.wofs + (long long)s_box[sl] * L.wstride;
-      const int* hdr = reinterpret_cast<const int*>(rec);
-      const int start = hdr[axis * 2], len = hdr[axis * 2 + 1];
-      const int idx = (axis ? col0 : row0) + k - start;
-      const float w = (idx >= 0 && idx < len) ? rec[4 + (axis ? L.H : 0) + idx] : 0.0f;
-      (axis ? s_wb : s_wa)[sl][k] = w;
-      if (w != 0.0f) atomicOr(axis ? &s_cmask[sl] : &s_rmask[sl], 1 << (k >> 3));
-    }
-    for (int i = threadIdx.x; i < ns * kSweepCh; i += kSweepThreads) s_acc[i / kSweepCh][i % kSweepCh] = 0.0f;
-    __syncthreads();
-
-    if (active) {
-      for (int tile = 0; tile < 16; ++tile) {
-        const int ty = tile >> 2, tx = tile & 3;
-        const int r_base = row0 + ty * 8, c_base = col0 + tx * 8;
-        if (r_base >= L.H || c_base >= L.W) continue;
-        bool any = false;
-        for (int sl = 0; sl < ns; ++sl) any |= ((s_rmask[sl] >> ty) & 1) && ((s_cmask[sl] >> tx) & 1);
-        if (!any) continue;  // warp-uniform
-        unsigned long long v2[8][8];   // (channel 0, channel 1) of the 64 cells, packed fp32x2
-        const __nv_bfloat16* p0 = L.data + (long long)r_base * rowpitch + (long long)c_base * L.C + cbase;
-#pragma unroll
-        for (int r = 0; r < 8; ++r) {
-#pragma unroll
-          for (int k = 0; k < 8; ++k) {
-            uint32_t u = 0;
-            if (r_base + r < L.H && c_base + k < L.W) u = __ldg(reinterpret_cast<const uint32_t*>(p0 + (long long)r * rowpitch + (long long)k * L.C));
-            v2[r][k] = f2_pack(bf16_lo(u), bf16_hi(u));
-          }
-        }
-        for (int sl = 0; sl < ns; ++sl) {
-          if (!(((s_rmask[sl] >> ty) & 1) && ((s_cmask[sl] >> tx) & 1))) continue;
-          const float4 b0 = *reinterpret_cast<const float4*>(&s_wb[sl][tx * 8]), b1 = *reinterpret_cast<const float4*>(&s_wb[sl][tx * 8 + 4]);
-          const float4 a0 = *reinterpret_cast<const float4*>(&s_wa[sl][ty * 8]), a1 = *reinterpret_cast<const float4*>(&s_wa[sl][ty * 8 + 4]);
-          const float wb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-          const float wa[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-          unsigned long long a2 = 0ull;
-#pragma unroll
-          for (int r = 0; r < 8; ++r) {
-            unsigned long long t2 = 0ull;
-#pragma unroll
-            for (int k = 0; k < 8; ++k) t2 = f2_fma(f2_pack(wb[k], wb[k]), v2[r][k], t2);
-            a2 = f2_fma(f2_pack(wa[r], wa[r]), t2, a2);
-          }
-          const float2 part = f2_unpack(a2);
-          float2* acc = reinterpret_cast<float2*>(&s_acc[sl][warp * 64 + lane * 2]);  // lane-owned: no atomics
-          float2 cur = *acc;
-          cur.x += part.x; cur.y += part.y;
-          *acc = cur;
-        }
-      }
-    }
-    __syncthreads();
-    // ---- flush: one fp32 reduction per (box, channel) of this region ----
-    for (int i = threadIdx.x; i < ns * kSweepCh; i += kSweepThreads) {
-      const int sl = i / kSweepCh, c = cgroup * kSweepCh + (i % kSweepCh);
-      if (c < L.C) acc_add(im.acc + (long long)s_box[sl] * B.out_dim + L.out_off + c, s_acc[sl][i % kSweepCh]);
-    }
-    __syncthreads();
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// Kernel 3'' (algo 3, map sweep on the tensor pipe).  At C2's box density every cell is covered by ~7 boxes, i.e.
-// ~7.5 FLOP per loaded byte: with the bf16 -> fp32 unpacking the SIMT sweep is bound by FMA issue, not by HBM.  The reduction is a contraction,
-//     out[box][c] += sum_y a_y[box] * ( sum_x b_x[box] * L[y][x][c] ),
-// so the inner sum over a region row runs as mma.sync m16n8k16 (A = b_x of 16 boxes, B = 16 cells x 8 channels of
-// the bf16 map, fp32 accumulate) and only the per-row scaling by a_y stays on the FMA pipe (1 FMA per 32 MACs).
-// The fp32 weights are fed as hi + lo bf16 halves (two MMAs): the map is bf16 already, so products are exact and
-// the weights keep 16 mantissa bits -- inside the 1e-3 parity budget with three orders of margin.
-// Work split: CTA = (level, 8 x 32 cell region, 256 channels), warp = 64 channels, a pass accumulates 16 boxes (one
-// m-tile; regions with more boxes take further passes whose rows come from L2 -- 8-row regions keep the footprint of
-// all resident CTAs below the L2 size).  A fragments depend on the boxes only and are built once per pass from the
-// region's weight records (hfre_region_records_kernel).  Every region row is copied ONCE per pass into a per-warp
-// cp.async ring (3 rows, two in flight behind the one being reduced; 16-byte chunks XOR-swizzled by cell) and its
-// B fragments are taken with ldmatrix.trans.  The partial sums of the pass leave through shared memory (aliasing the
-// ring) as coalesced fp32 reductions into out[box][channel].
-// ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void mma_bf16_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
   asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
                : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
@@ -725,19 +486,15 @@ __global__ void __launch_bounds__(kSweepThreads, 4) hfre_sweep_mma_kernel(const 
   }
 }
 
-// Kernel 4: finish -- sweeps: out = box embedding (already in out) + pooled feature (the fixed-point sum, rounded to fp32 once:
+// Kernel 4: finish -- out = box embedding (already in out) + pooled feature (the fixed-point sum, rounded to fp32 once:
 // the reference adds the embedding to the finished feature, hybrid_finegrained_region_encoder.py:464-467); then the optional
 // bf16 copy (the reference casts to the tower dtype before mm_projector_aux, omchat_qwen2_5_vl.py:106).
-__global__ void __launch_bounds__(256) hfre_finish_kernel(const BatchDev B, int from_acc) {
+__global__ void __launch_bounds__(256) hfre_finish_kernel(const BatchDev B) {
   const ImageDev& im = B.img[blockIdx.z];
-  if (!from_acc && im.out_bf16 == nullptr) return;
   const long long n = (long long)im.n_boxes * B.out_dim;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    float v = im.out[i];
-    if (from_acc) {
-      v = __fadd_rn((float)((double)im.acc[i] * (1.0 / 4294967296.0)), v);
-      im.out[i] = v;
-    }
+    const float v = __fadd_rn((float)((double)im.acc[i] * (1.0 / 4294967296.0)), im.out[i]);
+    im.out[i] = v;
     if (im.out_bf16 != nullptr) im.out_bf16[i] = __float2bfloat16_rn(v);
   }
 }
@@ -750,12 +507,11 @@ static size_t image_ws_floats(const fo1_hfre_image& im) {
   for (int l = 0; l < im.n_levels; ++l) f += (size_t)im.n_boxes * level_wstride(im.levels[l]);
   return f;
 }
-static int list_stride(int n_boxes) { return (1 + n_boxes + 3) & ~3; }                 // SIMT sweep: count + ids
-static int record_stride(int n_boxes) { return 4 + n_boxes * kRecWords; }             // tensor sweep: count + 48-word records
+static int record_stride(int n_boxes) { return 4 + n_boxes * kRecWords; }             // count + 48-word records
 static size_t image_list_ints(const fo1_hfre_image& im) {
   size_t n = 0;
   for (int l = 0; l < im.n_levels; ++l)
-    n += (size_t)ceil_div(im.levels[l].H, kMmaRows) * ceil_div(im.levels[l].W, kRegion) * record_stride(im.n_boxes);   // finest region grid / widest list of any algo
+    n += (size_t)ceil_div(im.levels[l].H, kMmaRows) * ceil_div(im.levels[l].W, kRegion) * record_stride(im.n_boxes);
   return n;
 }
 
@@ -781,7 +537,6 @@ extern "C" int fo1_hfre_forward(const fo1_hfre_image* images, int32_t n_images, 
   if (n_images == 0) return FO1_OK;
   FO1_CHECK_ARG(p->roi_size >= 1 && p->roi_size <= 32, "fo1_hfre_forward: roi_size %d unsupported", p->roi_size);
   FO1_CHECK_ARG(p->out_dim > 0 && p->out_dim % 4 == 0, "fo1_hfre_forward: out_dim %d must be a positive multiple of 4", p->out_dim);
-  FO1_CHECK_ARG(p->algo >= 0 && p->algo <= 3, "fo1_hfre_forward: algo %d not available", p->algo);
   const size_t need = fo1_hfre_workspace_bytes(images, n_images, p);
   if (workspace == nullptr || workspace_bytes < need) {
     set_error("fo1_hfre_forward: workspace %zu B < required %zu B", workspace_bytes, need);
@@ -791,7 +546,7 @@ extern "C" int fo1_hfre_forward(const fo1_hfre_image* images, int32_t n_images, 
   float* ws = static_cast<float*>(workspace);
   size_t total_w = 0;
   for (int i = 0; i < n_images; ++i) total_w += image_ws_floats(images[i]);
-  int* lists = reinterpret_cast<int*>(ws + total_w);   // region box lists live after all weight records
+  int* lists = reinterpret_cast<int*>(ws + total_w);   // region records live after all weight records
   size_t ls_ofs = 0;
   size_t total_f = 0;
   for (int i = 0; i < n_images; ++i) total_f += image_ws_floats(images[i]) + image_list_ints(images[i]);
@@ -807,14 +562,7 @@ extern "C" int fo1_hfre_forward(const fo1_hfre_image* images, int32_t n_images, 
     B.out_dim = p->out_dim;
     B.roi = p->roi_size;
     B.pos = p->apply_pos_embed ? 1 : 0;
-    int batch_boxes = 0;
-    for (int i = 0; i < B.n_images; ++i) batch_boxes += images[base + i].n_boxes > 0 ? images[base + i].n_boxes : 0;
-    // algo 0: a sweep wins as soon as boxes overlap (its traffic is the union of the windows, the gather's their sum),
-    // and the tensor-pipe sweep takes the FMA issue slots out of the SIMT one
-    const bool sweep = p->algo == 2 || p->algo == 3 || (p->algo == 0 && batch_boxes >= 8 * B.n_images);
-    const bool tensor = p->algo == 3 || (p->algo == 0 && sweep);
-    B.rrows = tensor ? kMmaRows : kRegion;
-    int max_boxes = 0, max_levels = 0, max_chunks = 0, max_up = 0, max_hw = 0, max_items = 0, max_regions = 0;
+    int max_boxes = 0, max_levels = 0, max_up = 0, max_items = 0, max_regions = 0;
     for (int i = 0; i < B.n_images; ++i) {
       const fo1_hfre_image& src = images[base + i];
       ImageDev& d = B.img[i];
@@ -833,9 +581,9 @@ extern "C" int fo1_hfre_forward(const fo1_hfre_image* images, int32_t n_images, 
       d.pos_h = src.pos_img_h;
       d.pos_box_set = src.pos_box_set ? 1 : 0;
       d.ws_ofs = (long long)ws_ofs;
-      int wofs = 0, chunks = 0, lofs = 0, items = 0;
+      int wofs = 0, lofs = 0, items = 0;
       d.ls_ofs = (long long)ls_ofs;
-      d.lstride = tensor ? record_stride(src.n_boxes) : list_stride(src.n_boxes);
+      d.lstride = record_stride(src.n_boxes);
       for (int l = 0; l < src.n_levels; ++l) {
         const fo1_hfre_level& sl = src.levels[l];
         FO1_CHECK_ARG(sl.data != nullptr && sl.H > 0 && sl.W > 0 && sl.C > 0, "image %d level %d: bad shape", base + i, l);
@@ -852,24 +600,20 @@ extern "C" int fo1_hfre_forward(const fo1_hfre_image* images, int32_t n_images, 
         dl.wofs = wofs;
         dl.wstride = level_wstride(sl);
         wofs += src.n_boxes * dl.wstride;
-        chunks += ceil_div(sl.C, kChunk);
-        dl.rh = ceil_div(sl.H, B.rrows); dl.rw = ceil_div(sl.W, kRegion);
+        dl.rh = ceil_div(sl.H, kMmaRows); dl.rw = ceil_div(sl.W, kRegion);
         dl.lofs = lofs;
         lofs += dl.rh * dl.rw * d.lstride;
         items += dl.rh * dl.rw * ceil_div(sl.C, kSweepCh);
         max_regions = max_regions > dl.rh * dl.rw ? max_regions : dl.rh * dl.rw;
         max_up = max_up > sl.up_H ? max_up : sl.up_H;
         max_up = max_up > sl.up_W ? max_up : sl.up_W;
-        max_hw = max_hw > sl.H + sl.W ? max_hw : sl.H + sl.W;
       }
-      d.n_chunks = chunks;
       d.n_items = items;
       max_items = max_items > items ? max_items : items;
       ws_ofs += (size_t)wofs;
       ls_ofs += (size_t)lofs;
       max_boxes = max_boxes > src.n_boxes ? max_boxes : src.n_boxes;
       max_levels = max_levels > src.n_levels ? max_levels : src.n_levels;
-      max_chunks = max_chunks > chunks ? max_chunks : chunks;
     }
     if (max_boxes == 0) continue;
     {
@@ -883,41 +627,29 @@ extern "C" int fo1_hfre_forward(const fo1_hfre_image* images, int32_t n_images, 
       hfre_pos_init_kernel<<<grid, 256, 0, stream>>>(B);
       FO1_LAUNCH_CHECK();
     }
-    if (sweep) {
-      if (!acc_zeroed) {   // one memset for every image of the call
-        FO1_CUDA(cudaMemsetAsync(acc_base, 0, acc_bytes(images, n_images, p), stream));
-        acc_zeroed = true;
-      }
-      {
-        dim3 grid(max_regions, max_levels, B.n_images);
-        if (tensor) hfre_region_records_kernel<<<grid, 128, 0, stream>>>(B, ws, lists);
-        else hfre_region_lists_kernel<<<grid, 32, 0, stream>>>(B, ws, lists);
-        FO1_LAUNCH_CHECK();
-      }
-      dim3 grid(max_items, 1, B.n_images);
-      ProfScope prof(tensor ? "hfre_sweep_mma" : "hfre_sweep", 0.0, 0.0, stream);
-      if (tensor) {
-        static bool attr_set = false;
-        if (!attr_set) {
-          FO1_CUDA(cudaFuncSetAttribute(hfre_sweep_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMmaSmemBytes));
-          attr_set = true;
-        }
-        hfre_sweep_mma_kernel<<<grid, kSweepThreads, kMmaSmemBytes, stream>>>(B, ws, lists);
-      }
-      else hfre_sweep_kernel<<<grid, kSweepThreads, 0, stream>>>(B, ws, lists);
-      FO1_LAUNCH_CHECK();
-    } else {
-      dim3 grid(max_chunks, max_boxes, B.n_images);
-      const size_t smem = ((size_t)max_hw + (kGatherThreads / 32) * kChunk) * sizeof(float);
-      ProfScope prof("hfre_gather", 0.0, 0.0, stream);
-      hfre_gather_kernel<<<grid, kGatherThreads, smem, stream>>>(B, ws);
+    if (!acc_zeroed) {   // one memset for every image of the call
+      FO1_CUDA(cudaMemsetAsync(acc_base, 0, acc_bytes(images, n_images, p), stream));
+      acc_zeroed = true;
+    }
+    {
+      dim3 grid(max_regions, max_levels, B.n_images);
+      hfre_region_records_kernel<<<grid, 128, 0, stream>>>(B, ws, lists);
       FO1_LAUNCH_CHECK();
     }
-    bool any_bf16 = false;
-    for (int i = 0; i < B.n_images; ++i) any_bf16 |= (B.img[i].out_bf16 != nullptr);
-    if (any_bf16 || sweep) {
+    {
+      dim3 grid(max_items, 1, B.n_images);
+      ProfScope prof("hfre_sweep_mma", 0.0, 0.0, stream);
+      static bool attr_set = false;
+      if (!attr_set) {
+        FO1_CUDA(cudaFuncSetAttribute(hfre_sweep_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMmaSmemBytes));
+        attr_set = true;
+      }
+      hfre_sweep_mma_kernel<<<grid, kSweepThreads, kMmaSmemBytes, stream>>>(B, ws, lists);
+      FO1_LAUNCH_CHECK();
+    }
+    {
       dim3 grid(ceil_div(max_boxes * p->out_dim, 256 * 8), 1, B.n_images);
-      hfre_finish_kernel<<<grid, 256, 0, stream>>>(B, sweep ? 1 : 0);
+      hfre_finish_kernel<<<grid, 256, 0, stream>>>(B);
       FO1_LAUNCH_CHECK();
     }
   }

@@ -29,7 +29,6 @@ class HfreConfig:
     vt_mode: str = "fpn"                  # 'fpn' (mm_use_simpleFPN_for_vt) | 'concat'
     roi_size: int = 7                     # mm_roi_output_size
     apply_pos_embed: bool = True          # mm_apply_position_embedding (bbox_based)
-    algo: int = 0
 
 
 class HfreWorkspace:
@@ -47,28 +46,45 @@ class HfreWorkspace:
 _default_ws = HfreWorkspace()
 
 
-def _fill_image(img: HfreImage, aux_feats, vt_feats, boxes_aux, boxes_vt, out, out_bf16, cfg, vt_grid_hw):
+def _level_list(aux_maps, vt_maps, cfg: HfreConfig) -> list:
+    """``(map, up_H, up_W, spatial_scale, box_set, out_offset)`` per level for maps shaped ``[..., H, W, C]``: the aux
+    levels, then the primary tower's FPN or concat levels, their channels back to back in the output row."""
     levels = []
-    H0 = max(f.shape[0] for f in aux_feats)
-    W0 = max(f.shape[1] for f in aux_feats)
+    H0 = max(f.shape[-3] for f in aux_maps)
+    W0 = max(f.shape[-2] for f in aux_maps)
     off = 0
-    for f in aux_feats:  # aux levels are up-sampled to level 0's grid by the reference (:338-350)
+    for f in aux_maps:  # aux levels are up-sampled to level 0's grid by the reference (:338-350)
         levels.append((f, H0, W0, AUX_SCALE, 0, off))
-        off += f.shape[2]
+        off += f.shape[-1]
     if cfg.vt_mode == "fpn":
-        for i, f in enumerate(vt_feats):
-            levels.append((f, f.shape[0], f.shape[1], 1.0 / FPN_STRIDES[i], 1, off))
-            off += f.shape[2]
+        for i, f in enumerate(vt_maps):
+            levels.append((f, f.shape[-3], f.shape[-2], 1.0 / FPN_STRIDES[i], 1, off))
+            off += f.shape[-1]
     elif cfg.vt_mode == "concat":
-        for f in vt_feats:
-            levels.append((f, f.shape[0], f.shape[1], VT_SCALE, 1, off))
-            off += f.shape[2]
+        for f in vt_maps:
+            levels.append((f, f.shape[-3], f.shape[-2], VT_SCALE, 1, off))
+            off += f.shape[-1]
     else:
         raise ValueError(f"unknown vt_mode {cfg.vt_mode!r}")
     if off > cfg.region_dim:
         raise ValueError(f"levels provide {off} channels > region_dim {cfg.region_dim}")
     if len(levels) > _lib.FO1_HFRE_MAX_LEVELS:
         raise ValueError("too many feature levels")
+    return levels
+
+
+def _launch(imgs, n_images: int, cfg: HfreConfig, device, workspace: Optional[HfreWorkspace]) -> None:
+    """Size the workspace for the filled descriptors and enqueue fo1_hfre_forward on the current stream."""
+    p = HfreParams(cfg.region_dim, cfg.roi_size, 1 if cfg.apply_pos_embed else 0)
+    L = lib()
+    need = L.fo1_hfre_workspace_bytes(imgs, n_images, C.byref(p))
+    ws = (workspace or _default_ws).get(need, device)
+    check(L.fo1_hfre_forward(imgs, n_images, C.byref(p), C.c_void_p(ws.data_ptr()), ws.numel(),
+                             C.c_void_p(torch.cuda.current_stream().cuda_stream)), "fo1_hfre_forward")
+
+
+def _fill_image(img: HfreImage, aux_feats, vt_feats, boxes_aux, boxes_vt, out, out_bf16, cfg, vt_grid_hw):
+    levels = _level_list(aux_feats, vt_feats, cfg)
     for i, (f, uh, uw, sc, bs, o) in enumerate(levels):
         if f.dtype != torch.bfloat16 or not f.is_contiguous() or f.dim() != 3 or not f.is_cuda:
             raise _lib.Fo1Error("HFRE levels must be contiguous channels-last bf16 CUDA tensors [H, W, C]")
@@ -107,13 +123,7 @@ def hfre_forward(aux_feats: Sequence[Sequence[torch.Tensor]], vt_feats: Sequence
         o16 = torch.empty((n, cfg.region_dim), dtype=torch.bfloat16, device=ba.device) if want_bf16 else None
         outs.append(o); outs16.append(o16)
         _fill_image(imgs[b], aux_feats[b], vt_feats[b], ba, bv, o, o16, cfg, vt_grid_hw[b])
-    p = HfreParams(cfg.region_dim, cfg.roi_size, 1 if cfg.apply_pos_embed else 0, cfg.algo)
-    L = lib()
-    need = L.fo1_hfre_workspace_bytes(imgs, B, C.byref(p))
-    dev = outs[0].device if outs else torch.device("cuda")
-    ws = (workspace or _default_ws).get(need, dev)
-    check(L.fo1_hfre_forward(imgs, B, C.byref(p), C.c_void_p(ws.data_ptr()), ws.numel(),
-                             C.c_void_p(torch.cuda.current_stream().cuda_stream)), "fo1_hfre_forward")
+    _launch(imgs, B, cfg, outs[0].device if outs else torch.device("cuda"), workspace)
     return (outs, outs16) if want_bf16 else outs
 
 
@@ -137,23 +147,7 @@ def hfre_forward_packed(aux_levels: Sequence[torch.Tensor], vt_levels: Sequence[
     total = int(sum(counts))
     if boxes_aux.shape != (total, 4) or boxes_vt.shape != (total, 4):
         raise _lib.Fo1Error("HFRE packed boxes do not match counts")
-    H0 = max(f.shape[1] for f in aux_levels); W0 = max(f.shape[2] for f in aux_levels)
-    levels = []
-    off = 0
-    for f in aux_levels:
-        levels.append((f, H0, W0, AUX_SCALE, 0, off)); off += f.shape[3]
-    if cfg.vt_mode == "fpn":
-        for i, f in enumerate(vt_levels):
-            levels.append((f, f.shape[1], f.shape[2], 1.0 / FPN_STRIDES[i], 1, off)); off += f.shape[3]
-    elif cfg.vt_mode == "concat":
-        for f in vt_levels:
-            levels.append((f, f.shape[1], f.shape[2], VT_SCALE, 1, off)); off += f.shape[3]
-    else:
-        raise ValueError(f"unknown vt_mode {cfg.vt_mode!r}")
-    if off > cfg.region_dim:
-        raise ValueError(f"levels provide {off} channels > region_dim {cfg.region_dim}")
-    if len(levels) > _lib.FO1_HFRE_MAX_LEVELS:
-        raise ValueError("too many feature levels")
+    levels = _level_list(aux_levels, vt_levels, cfg)
     out = torch.empty((total, cfg.region_dim), dtype=torch.float32, device=dev)
     out16 = torch.empty((total, cfg.region_dim), dtype=torch.bfloat16, device=dev) if want_bf16 else None
     imgs = (HfreImage * B)()
@@ -177,12 +171,7 @@ def hfre_forward_packed(aux_levels: Sequence[torch.Tensor], vt_levels: Sequence[
     a["pos_img_w"] = gw / VT_SCALE      # :447-448 (python float, rounded to fp32 at the division like the reference)
     a["pos_img_h"] = gh / VT_SCALE
     a["pos_box_set"] = 1
-    p = HfreParams(cfg.region_dim, cfg.roi_size, 1 if cfg.apply_pos_embed else 0, cfg.algo)
-    L = lib()
-    need = L.fo1_hfre_workspace_bytes(imgs, B, C.byref(p))
-    ws = (workspace or _default_ws).get(need, dev)
-    check(L.fo1_hfre_forward(imgs, B, C.byref(p), C.c_void_p(ws.data_ptr()), ws.numel(),
-                             C.c_void_p(torch.cuda.current_stream().cuda_stream)), "fo1_hfre_forward")
+    _launch(imgs, B, cfg, dev, workspace)
     return (out, out16) if want_bf16 else out
 
 
