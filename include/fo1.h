@@ -355,6 +355,30 @@ typedef struct {
  * The K/V cache and the decode loop state live on the device; the host only launches. */
 int fo1_llm_generate(fo1_model* m, fo1_generate_desc* d, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Sampled decoding (replaces HF generate's sampling branch as the reference drives it, mm_utils.py:630-654 ->
+ * GenerationMixin._sample with the warpers TemperatureLogitsWarper -> TopKLogitsWarper -> TopPLogitsWarper and
+ * torch.multinomial, transformers/generation/logits_process.py).  Per row: x = logits / T (fp32); keep the tokens whose
+ * x >= the k-th largest (ties kept); keep the tokens whose softmax mass ranked above them is < p; draw with
+ * u = (x0 >> 8) * 2^-24 of Philox4x32-10(key = seed, counter = (step, 0, 0, 0)), ranking by x descending, then index
+ * ascending.  top_k == 1 is greedy (lowest index among equal maxima).  A row's token depends only on its logits, its
+ * parameters and its step.  The parameter arrays are validated on the host before any CUDA call.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct {
+  const float* temperature;  /* HOST [n]: > 0 and finite; 1.0 = no scaling */
+  const float* top_p;        /* HOST [n]: (0, 1]; 1.0 = off */
+  const int32_t* top_k;      /* HOST [n]: >= 0; 0 or >= vocab = off */
+  const uint64_t* seed;      /* HOST [n]: Philox key of each row / sequence */
+} fo1_sampling_desc;
+size_t fo1_sample_tokens_workspace_bytes(int32_t n_rows);
+/* One token per row of fp32 logits [n_rows][ld] (device); step: DEVICE int32 [n_rows], the Philox counter of each row. */
+int fo1_sample_tokens(const float* logits, int64_t ld, int32_t n_rows, int32_t vocab, const fo1_sampling_desc* sp,
+                      const int32_t* step /* DEVICE [n_rows] */, int32_t* out_tokens /* DEVICE [n_rows] */,
+                      void* workspace, size_t workspace_bytes, void* stream);
+/* fo1_llm_generate with per-sequence sampling (the step of a sequence's token is its output column); sp == NULL is exactly
+ * fo1_llm_generate (greedy). */
+int fo1_llm_generate_sampled(fo1_model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

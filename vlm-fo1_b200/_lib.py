@@ -56,6 +56,21 @@ class DecodeAttnDesc(C.Structure):
                 ("scale", C.c_float), ("out", C.c_void_p), ("ldo", C.c_int64), ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t)]
 
 
+class SamplingDesc(C.Structure):
+    """fo1_sampling_desc: HOST arrays of per-row temperature, top_p, top_k, seed."""
+    _fields_ = [("temperature", C.POINTER(C.c_float)), ("top_p", C.POINTER(C.c_float)), ("top_k", C.POINTER(C.c_int32)),
+                ("seed", C.POINTER(C.c_uint64))]
+
+
+def sampling_desc(temperature, top_p, top_k, seed):
+    """-> (SamplingDesc, the ctypes arrays it points into: keep them alive for the call)."""
+    n = len(temperature)
+    assert len(top_p) == n and len(top_k) == n and len(seed) == n, "one temperature / top_p / top_k / seed per row"
+    arrs = ((C.c_float * n)(*[float(x) for x in temperature]), (C.c_float * n)(*[float(x) for x in top_p]),
+            (C.c_int32 * n)(*[int(x) for x in top_k]), (C.c_uint64 * n)(*[int(x) & 0xFFFFFFFFFFFFFFFF for x in seed]))
+    return SamplingDesc(*arrs), arrs
+
+
 _lib = None
 
 
@@ -87,6 +102,13 @@ def lib() -> C.CDLL:
     L.fo1_gemm_bf16.argtypes = [C.POINTER(GemmDesc), C.c_void_p]
     L.fo1_attention_varlen.restype = C.c_int
     L.fo1_attention_varlen.argtypes = [C.POINTER(AttnDesc), C.c_void_p]
+    L.fo1_sample_tokens_workspace_bytes.restype = C.c_size_t
+    L.fo1_sample_tokens_workspace_bytes.argtypes = [C.c_int32]
+    L.fo1_sample_tokens.restype = C.c_int
+    L.fo1_sample_tokens.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.POINTER(SamplingDesc), C.c_void_p, C.c_void_p,
+                                    C.c_void_p, C.c_size_t, C.c_void_p]
+    L.fo1_llm_generate_sampled.restype = C.c_int
+    L.fo1_llm_generate_sampled.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(SamplingDesc), C.c_void_p]
     _lib = L
     return L
 

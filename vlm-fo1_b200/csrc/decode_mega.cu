@@ -196,7 +196,7 @@ struct MgRing {
 };
 
 // -------------------------------------------------------------------------------------------------------- epilogues
-enum { MG_EPI_QKV = 0, MG_EPI_RESID = 1, MG_EPI_GATEUP = 2, MG_EPI_HEAD = 3 };
+enum { MG_EPI_QKV = 0, MG_EPI_RESID = 1, MG_EPI_GATEUP = 2, MG_EPI_HEAD = 3, MG_EPI_LOGITS = 4 };
 
 struct MgEpi {
   bf16* out; int ldo;                 // QKV / RESID / GATEUP
@@ -317,12 +317,17 @@ __device__ __forceinline__ void mg_gemm_phase(const MegaArgs& a, uint8_t* smem, 
           sq += __shfl_xor_sync(0xffffffffu, sq, 2);
           sq += __shfl_xor_sync(0xffffffffu, sq, 4);
           if (q == 0) sSsq[row] += sq;                                        // one writer per row, tiles in order
-        } else {   // MG_EPI_HEAD: running arg-max of this thread's two columns (lowest index wins ties)
+        } else if (EPI == MG_EPI_HEAD) {   // running arg-max of this thread's two columns (lowest index wins ties)
           if (row < a.B) {
             const float rs = sRs[row];
             const float y0 = v0 * rs, y1 = v1 * rs;
             if (y0 > *best_val) { *best_val = y0; *best_idx = c; }
             if (y1 > *best_val) { *best_val = y1; *best_idx = c + 1; }
+          }
+        } else {   // MG_EPI_LOGITS: the same fp32 values, stored for the sampler
+          if (row < a.B) {
+            const float rs = sRs[row];
+            *reinterpret_cast<float2*>(a.logits + (long long)row * a.V + c) = make_float2(v0 * rs, v1 * rs);
           }
         }
       }
@@ -584,7 +589,9 @@ __device__ __forceinline__ void mg_attention_phase(const MegaArgs& a, uint8_t* s
 }
 
 // ----------------------------------------------------------------------------------------------------------- kernel
-template <int MT>
+// SAMPLE = false: the greedy loop.  SAMPLE = true: the head stores its logits, CTA b < B draws sequence b's token with the
+// row routine of sampling.cuh (one more grid barrier per step), CTA 0 records the drawn tokens.
+template <int MT, bool SAMPLE>
 __global__ void __launch_bounds__(kMgThreads, 1) decode_mega_kernel(const MegaArgs a) {
   using Lay = MgLay<MT>;
   extern __shared__ __align__(128) uint8_t mg_smem[];
@@ -685,10 +692,25 @@ __global__ void __launch_bounds__(kMgThreads, 1) decode_mega_kernel(const MegaAr
       ring.fill(work, lane);
       MG_STAMP(slot, 0); mg_grid_sync(a.bar, gen); MG_STAMP(slot, 1); ++slot;
     }
-    // ---- LM head: running arg-max of this CTA's columns ----
-    float best_val = -INFINITY;
-    int best_idx = 0x7fffffff;
-    {
+    // ---- LM head: running arg-max of this CTA's columns (SAMPLE: the logits rows) ----
+    [[maybe_unused]] float best_val = -INFINITY;
+    [[maybe_unused]] int best_idx = 0x7fffffff;
+    if constexpr (SAMPLE) {
+      MgEpi e;
+      e.out = nullptr; e.ldo = 0; e.bias = nullptr; e.resid = nullptr; e.ssq_slot = nullptr; e.scale_rows = true;
+      mg_row_scale(a, mg_smem, ssq_x);
+      mg_gemm_phase<MG_EPI_LOGITS, MT, false>(a, mg_smem, a.x, a.H, a.H, a.V, work, ring, e, a_par, nullptr, nullptr);
+      MG_STAMP(slot, 0); mg_grid_sync(a.bar, gen); MG_STAMP(slot, 1); ++slot;
+      // ---- CTA b draws sequence b's token.  Its scratch aliases the weight ring: the head phase consumed every stage it
+      // issued and the next step's first fill comes after the barriers below, so no cp.async is in flight here ----
+      if ((int)blockIdx.x < a.B) {
+        mg_wait<0>();
+        SampleSmem<kMgThreads>& sm = *reinterpret_cast<SampleSmem<kMgThreads>*>(mg_smem);
+        const int b = blockIdx.x;
+        const int tok = sample_row<kMgThreads>(a.logits + (long long)b * a.V, a.V, a.samp[b], __ldcg(a.step), sm);
+        if (threadIdx.x == 0) a.samp_tok[b] = tok;
+      }
+    } else {
       MgEpi e;
       e.out = nullptr; e.ldo = 0; e.bias = nullptr; e.resid = nullptr; e.ssq_slot = nullptr; e.scale_rows = true;
       mg_row_scale(a, mg_smem, ssq_x);
@@ -709,16 +731,20 @@ __global__ void __launch_bounds__(kMgThreads, 1) decode_mega_kernel(const MegaAr
       const int step = *a.step;
       __syncthreads();
       for (int b = warp; b < a.B; b += kMgWarps) {
-        float bv = -INFINITY; int bi = 0x7fffffff;
-        for (int c = lane; c < (int)gridDim.x; c += 32) {
-          const float v = __ldcg(a.amax_val + c * 32 + b); const int i = __ldcg(a.amax_idx + c * 32 + b);
-          if (v > bv || (v == bv && i < bi)) { bv = v; bi = i; }
-        }
+        [[maybe_unused]] float bv = -INFINITY; int bi = 0x7fffffff;
+        if constexpr (SAMPLE) {
+          bi = __ldcg(a.samp_tok + b);
+        } else {
+          for (int c = lane; c < (int)gridDim.x; c += 32) {
+            const float v = __ldcg(a.amax_val + c * 32 + b); const int i = __ldcg(a.amax_idx + c * 32 + b);
+            if (v > bv || (v == bv && i < bi)) { bv = v; bi = i; }
+          }
 #pragma unroll
-        for (int o2 = 16; o2 > 0; o2 >>= 1) {
-          const float ov = __shfl_xor_sync(0xffffffffu, bv, o2);
-          const int oi = __shfl_xor_sync(0xffffffffu, bi, o2);
-          if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+          for (int o2 = 16; o2 > 0; o2 >>= 1) {
+            const float ov = __shfl_xor_sync(0xffffffffu, bv, o2);
+            const int oi = __shfl_xor_sync(0xffffffffu, bi, o2);
+            if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+          }
         }
         if (lane == 0) {
           const int tok = bi;
@@ -757,9 +783,12 @@ int decode_mega_grid() {
     grid = 0;
     int dev = 0, coop = 0, per_sm = 0;
     if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev) == cudaSuccess && coop &&
-        cudaFuncSetAttribute(decode_mega_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMgSmemBytes) == cudaSuccess &&
-        cudaFuncSetAttribute(decode_mega_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMgSmemBytes) == cudaSuccess &&
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decode_mega_kernel<2>, kMgThreads, kMgSmemBytes) == cudaSuccess && per_sm >= 1)
+        cudaFuncSetAttribute(decode_mega_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMgSmemBytes) == cudaSuccess &&
+        cudaFuncSetAttribute(decode_mega_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMgSmemBytes) == cudaSuccess &&
+        cudaFuncSetAttribute(decode_mega_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMgSmemBytes) == cudaSuccess &&
+        cudaFuncSetAttribute(decode_mega_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMgSmemBytes) == cudaSuccess &&
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decode_mega_kernel<2, false>, kMgThreads, kMgSmemBytes) == cudaSuccess && per_sm >= 1 &&
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decode_mega_kernel<2, true>, kMgThreads, kMgSmemBytes) == cudaSuccess && per_sm >= 1)
       grid = device_sm_count();
     else
       fprintf(stderr, "[fo1] decode_mega: cooperative launch with %d B of shared memory is not available (%s); using the per-kernel decode path\n",
@@ -780,7 +809,9 @@ int decode_mega_run(const MegaArgs& a, cudaStream_t s) {
   MegaArgs args = a;
   void* params[] = {&args};
   ProfScope prof("decode_mega", 0.0, 0.0, s);
-  void* fn = a.B <= 16 ? reinterpret_cast<void*>(decode_mega_kernel<1>) : reinterpret_cast<void*>(decode_mega_kernel<2>);
+  FO1_CHECK_ARG(a.samp == nullptr || (a.logits != nullptr && a.samp_tok != nullptr && (a.V & 1) == 0), "decode_mega: sampling buffers missing");
+  void* fn = a.samp != nullptr ? (a.B <= 16 ? reinterpret_cast<void*>(decode_mega_kernel<1, true>) : reinterpret_cast<void*>(decode_mega_kernel<2, true>))
+                               : (a.B <= 16 ? reinterpret_cast<void*>(decode_mega_kernel<1, false>) : reinterpret_cast<void*>(decode_mega_kernel<2, false>));
   FO1_CUDA(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(kMgThreads), params, kMgSmemBytes, s));
   count_launch();
   return FO1_OK;

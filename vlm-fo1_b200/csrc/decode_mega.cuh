@@ -1,6 +1,7 @@
 // decode_mega.cuh -- argument block of the persistent decode kernel (decode_mega.cu), filled by llm.cu.
 #pragma once
 #include "engine.cuh"
+#include "sampling.cuh"
 
 namespace fo1 {
 
@@ -34,10 +35,14 @@ struct MegaArgs {
   int n_splits;
   unsigned long long* prof;   // optional [grid][prof_slots][2] barrier enter / leave stamps of the first iteration (nullptr: off)
   int prof_slots;
+  // sampled decoding (decode_mega_kernel<MT, true>; all nullptr for greedy)
+  float* logits;                    // [B][V] fp32 head output
+  const SampleRowParams* samp;      // [B] per-sequence temperature, top-p, top-k, seed
+  int* samp_tok;                    // [B] the token CTA b drew for sequence b
 };
 
 
 int decode_mega_grid();                                   // CTAs of the cooperative launch (0: not available on this device)
-int decode_mega_run(const MegaArgs& a, cudaStream_t s);   // the whole greedy loop, one launch
+int decode_mega_run(const MegaArgs& a, cudaStream_t s);   // the whole decode loop, one launch (sampled when a.samp != nullptr)
 
 }  // namespace fo1

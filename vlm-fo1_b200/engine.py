@@ -245,10 +245,22 @@ def _engine_build_embeds(self, kind: torch.Tensor, index: torch.Tensor, img_feat
     return out
 
 
+@dataclass
+class Sampling:
+    """Per-sequence sampling parameters (fo1_sampling_desc): temperature > 0, top_p in (0, 1] (1 = off), top_k >= 0 (0 = off,
+    1 = greedy), seed = the 64-bit Philox key of the sequence."""
+    temperature: Sequence[float]
+    top_p: Sequence[float]
+    top_k: Sequence[int]
+    seed: Sequence[int]
+
+
 def _engine_generate(self, inputs_embeds: torch.Tensor, position_ids: torch.Tensor, seq_lens: Sequence[int],
                      rope_deltas: Sequence[int], max_new_tokens: int, stop_ids: Sequence[int], pad_id: int,
-                     want_prefill_logits: bool = False, want_all_logits: bool = False, early_exit_interval: int = 8):
-    """Prefill + greedy decode of a packed batch.  position_ids int32 [3, sum L].  Returns a dict of device tensors."""
+                     want_prefill_logits: bool = False, want_all_logits: bool = False, early_exit_interval: int = 8,
+                     sampling: Optional[Sampling] = None):
+    """Prefill + decode of a packed batch: greedy, or sampled per sequence when ``sampling`` is given.  position_ids int32
+    [3, sum L].  Returns a dict of device tensors."""
     B = len(seq_lens)
     V = self.cfg.llm["vocab_size"]
     T = int(sum(seq_lens))
@@ -277,13 +289,37 @@ def _engine_generate(self, inputs_embeds: torch.Tensor, position_ids: torch.Tens
     d.all_logits = al.data_ptr() if al is not None else None
     d.early_exit_interval = early_exit_interval
     L = lib()
-    L.fo1_llm_generate.restype = C.c_int
-    check(L.fo1_llm_generate(self._h, C.byref(d), _stream()), "fo1_llm_generate")
+    if sampling is None:
+        L.fo1_llm_generate.restype = C.c_int
+        check(L.fo1_llm_generate(self._h, C.byref(d), _stream()), "fo1_llm_generate")
+    else:
+        sd, _keep = _lib.sampling_desc(sampling.temperature, sampling.top_p, sampling.top_k, sampling.seed)
+        assert len(sampling.temperature) == B, "one sampling parameter set per sequence"
+        check(L.fo1_llm_generate_sampled(self._h, C.byref(d), C.byref(sd), _stream()), "fo1_llm_generate_sampled")
     return dict(tokens=toks, lens=lens, prefill_logits=pl, all_logits=al, steps_run=d.steps_run)
+
+
+def sample_tokens(logits: torch.Tensor, temperature: Sequence[float], top_p: Sequence[float], top_k: Sequence[int], seed: Sequence[int],
+                  step) -> torch.Tensor:
+    """One sampled token per row of fp32 logits [n, V] on the device (fo1_sample_tokens).  ``step``: int (every row) or a device
+    int32 tensor [n], the Philox counter of each row.  -> int32 [n] on the device."""
+    assert logits.is_cuda and logits.dtype == torch.float32 and logits.dim() == 2 and logits.stride(1) == 1
+    n, V = logits.shape
+    if not isinstance(step, torch.Tensor):
+        step = torch.full((n,), int(step), dtype=torch.int32, device=logits.device)
+    step = step.to(logits.device, torch.int32).contiguous()
+    out = torch.empty((n,), dtype=torch.int32, device=logits.device)
+    L = lib()
+    ws = torch.empty((max(int(L.fo1_sample_tokens_workspace_bytes(n)), 1),), dtype=torch.uint8, device=logits.device)
+    sd, _keep = _lib.sampling_desc(temperature, top_p, top_k, seed)
+    check(L.fo1_sample_tokens(C.c_void_p(logits.data_ptr()), logits.stride(0), n, V, C.byref(sd), C.c_void_p(step.data_ptr()),
+                              C.c_void_p(out.data_ptr()), C.c_void_p(ws.data_ptr()), ws.numel(), _stream()), "fo1_sample_tokens")
+    return out
 
 
 Engine.build_embeds = _engine_build_embeds
 Engine.generate = _engine_generate
+Engine.sample_tokens = staticmethod(sample_tokens)
 
 
 def splice_plan_batch(prompts: Sequence[Sequence[int]], image_grids: Sequence[Sequence[Tuple[int, int]]], n_regions: Sequence[int], device,

@@ -117,9 +117,12 @@ def load_pretrained_model(model_path, load_8bit=False, load_4bit=False, device="
     config.image_token_id = int(g("image_token_id", 151655)); config.video_token_id = int(g("video_token_id", 151656))
     config.vision_start_token_id = int(g("vision_start_token_id", 151652))
     gen_path = os.path.join(model_path, "generation_config.json")
-    eos = json.load(open(gen_path)).get("eos_token_id", []) if os.path.exists(gen_path) else g("eos_token_id", [])
+    gen_cfg = json.load(open(gen_path)) if os.path.exists(gen_path) else {}
+    eos = gen_cfg.get("eos_token_id", []) if os.path.exists(gen_path) else g("eos_token_id", [])
     stop_ids = [int(e) for e in (eos if isinstance(eos, list) else [eos]) if e is not None]
-    model = Fo1ForCausalLM(engine, config, "fpn" if use_fpn else "concat", stop_ids, roi_size=roi_size, apply_pos_embed=apply_pos)
+    # the sampling fields (top_k; the processors sampled decoding refuses) are read here and checked per call, never at load time
+    model = Fo1ForCausalLM(engine, config, "fpn" if use_fpn else "concat", stop_ids, roi_size=roi_size, apply_pos_embed=apply_pos,
+                           generation_config=gen_cfg)
     # the processors run on the engine's GPU (uint8 over PCIe; bit-identical to the host processors); FO1_HOST_PREPROCESS=1 keeps PIL / numpy
     pdev = None if os.environ.get("FO1_HOST_PREPROCESS") else engine.device
     primary = PrimaryImageProcessor(cfg.vit["patch_size"], cfg.vit["spatial_merge_size"], cfg.vit["temporal_patch_size"], 56 * 56, 2048 * 2048, device=pdev)

@@ -4,15 +4,23 @@
 columns are ``inputs``), everything underneath delegated to the H100 engine."""
 from __future__ import annotations
 
+import math
 from importlib import import_module
 from types import SimpleNamespace
-from typing import List
+from typing import List, Optional
 
 import torch
 
 
+# generation_config.json fields of logits processors the engine does not implement, with HF GenerationConfig's neutral defaults.
+# On the sampled path a non-neutral value is refused (honour or refuse, never ignore); greedy decoding does not read them.
+_UNSUPPORTED_PROCESSORS = (("repetition_penalty", 1.0), ("min_p", None), ("typical_p", 1.0), ("epsilon_cutoff", 0.0),
+                           ("eta_cutoff", 0.0), ("no_repeat_ngram_size", 0), ("num_beams", 1), ("num_return_sequences", 1))
+
+
 class Fo1ForCausalLM:
-    def __init__(self, engine, config: SimpleNamespace, vt_mode: str, stop_ids: List[int], roi_size: int = 7, apply_pos_embed: bool = True):
+    def __init__(self, engine, config: SimpleNamespace, vt_mode: str, stop_ids: List[int], roi_size: int = 7, apply_pos_embed: bool = True,
+                 generation_config: Optional[dict] = None):
         P = import_module("vlm-fo1_b200.pipeline")
         self.engine = engine
         self.config = config
@@ -23,6 +31,7 @@ class Fo1ForCausalLM:
         self.default_stop_ids = list(stop_ids)
         self.device = engine.device
         self.dtype = torch.bfloat16
+        self.generation_config = dict(generation_config or {})
 
     # nn.Module-ish no-ops the callers invoke
     def eval(self):
@@ -34,11 +43,31 @@ class Fo1ForCausalLM:
     def get_model(self):
         return self
 
+    def _sampling_params(self, temperature, top_p, top_k, kwargs):
+        """(T, p, k) of a sampled call, validated as HF's warpers validate them; unsupported processors are refused."""
+        gc = self.generation_config
+        for name, neutral in _UNSUPPORTED_PROCESSORS:
+            v = kwargs.get(name, gc.get(name, neutral))
+            if v is not None and v != neutral:
+                raise NotImplementedError(f"{name}={v!r} is not supported by the fo1-b200 engine's sampled decoding "
+                                          "(it implements temperature, top_k and top_p)")
+        T = 1.0 if temperature is None else float(temperature)
+        if not (T > 0.0) or not math.isfinite(T):
+            raise ValueError(f"`temperature` (={temperature}) has to be a strictly positive float when do_sample=True")
+        p = 1.0 if top_p is None else float(top_p)
+        if not (0.0 < p <= 1.0):
+            raise ValueError(f"`top_p` has to be a float in (0, 1], but is {top_p}")
+        k = gc.get("top_k", 50) if top_k is None else top_k
+        k = 0 if k is None else int(k)
+        if k < 0:
+            raise ValueError(f"`top_k` has to be a non-negative integer, but is {top_k}")
+        return T, p, k
+
     def _sample(self, inputs=None, images=None, images_aux=None, image_grid_thws=None, bbox_list=None, do_sample=False, temperature=0.0,
-                stopping_criteria=None, **kwargs):
-        """One ``prepare_inputs`` dict -> (SampleInputs, stop ids): the argument checks of the reference's call contract."""
-        if do_sample or (temperature or 0.0) != 0.0:
-            raise NotImplementedError("the fo1-b200 engine decodes greedily (the reference's callers all pass temperature=0.0)")
+                stopping_criteria=None, top_p=None, top_k=None, **kwargs):
+        """One ``prepare_inputs`` dict -> (SampleInputs, stop ids, (T, p, k) or None): the argument checks of the reference's call
+        contract.  do_sample=False is greedy whatever the temperature, as in HF's generate."""
+        samp = self._sampling_params(temperature, top_p, top_k, kwargs) if do_sample else None
         if inputs is None or inputs.dim() != 2 or inputs.shape[0] != 1:
             raise ValueError("generate expects `inputs` of shape [1, P] (the reference runs one sample per call)")
         if images is None or len(images) != 1:
@@ -60,14 +89,29 @@ class Fo1ForCausalLM:
                     # the device-side stop list, and silently ignoring it would change where generation ends
                     raise NotImplementedError(f"multi-token stop keyword {kw.tolist()} is not supported by the device-side stop test "
                                               "(every caller in the reference stops on the single token <|im_end|>)")
-        return sample, stop
+        return sample, stop, samp
+
+    def _sampling(self, samps):
+        """Per-sample (T, p, k) or None -> engine.Sampling (None when every sample is greedy).  One seed per sampled sample, drawn
+        from torch's default CPU generator in sample order; a greedy sample in a sampled batch is top_k = 1 (the arg-max)."""
+        if all(s is None for s in samps):
+            return None
+        E = import_module("vlm-fo1_b200.engine")
+        T, P, K, seeds = [], [], [], []
+        for s in samps:
+            t, p, k = s if s is not None else (1.0, 1.0, 1)
+            seeds.append(int(torch.empty((), dtype=torch.int64).random_().item()) if s is not None else 0)
+            T.append(t); P.append(p); K.append(k)
+        return E.Sampling(T, P, K, seeds)
 
     @torch.no_grad()
     def generate(self, inputs=None, images=None, images_aux=None, image_grid_thws=None, bbox_list=None, do_sample=False, temperature=0.0,
-                 max_new_tokens=512, streamer=None, top_p=1.0, use_cache=True, stopping_criteria=None, pad_token_id=None, **kwargs):
-        sample, stop = self._sample(inputs, images, images_aux, image_grid_thws, bbox_list, do_sample, temperature, stopping_criteria)
+                 max_new_tokens=512, streamer=None, top_p=1.0, use_cache=True, stopping_criteria=None, pad_token_id=None, top_k=None, **kwargs):
+        sample, stop, samp = self._sample(inputs, images, images_aux, image_grid_thws, bbox_list, do_sample, temperature, stopping_criteria,
+                                          top_p, top_k, **kwargs)
         pad = pad_token_id if pad_token_id is not None else (stop[0] if stop else 0)
-        out = self.pipeline.generate([sample], int(max_new_tokens), sorted(set(stop)), pad_id=int(pad), early_exit_interval=8)
+        out = self.pipeline.generate([sample], int(max_new_tokens), sorted(set(stop)), pad_id=int(pad), early_exit_interval=8,
+                                     sampling=self._sampling([samp]))
         n = int(out["lens"][0].item())
         new = out["tokens"][0, :n].to(torch.long)
         full = torch.cat([inputs[0].to(new.device), new]).unsqueeze(0)
@@ -86,13 +130,14 @@ class Fo1ForCausalLM:
         -> list of LongTensor [1, P_b + T_b], each exactly what ``generate(**batch[b])`` returns."""
         if not batch:
             return []
-        samples, stops = zip(*(self._sample(**{k: v for k, v in kw.items() if k in (
-            "inputs", "images", "images_aux", "image_grid_thws", "bbox_list", "do_sample", "temperature", "stopping_criteria")}) for kw in batch))
+        keys = ("inputs", "images", "images_aux", "image_grid_thws", "bbox_list", "do_sample", "temperature", "stopping_criteria", "top_p",
+                "top_k") + tuple(n for n, _ in _UNSUPPORTED_PROCESSORS)
+        samples, stops, samps = zip(*(self._sample(**{k: v for k, v in kw.items() if k in keys}) for kw in batch))
         stop = sorted(set(x for s in stops for x in s))
         T = int(max_new_tokens if max_new_tokens is not None else max(int(kw.get("max_new_tokens", 512)) for kw in batch))
         pads = [kw.get("pad_token_id") for kw in batch]
         pad = pads[0] if pads[0] is not None else (stop[0] if stop else 0)
-        out = self.pipeline.generate(list(samples), T, stop, pad_id=int(pad), early_exit_interval=8)
+        out = self.pipeline.generate(list(samples), T, stop, pad_id=int(pad), early_exit_interval=8, sampling=self._sampling(samps))
         lens = out["lens"].cpu().tolist()
         res = []
         for b, kw in enumerate(batch):
