@@ -379,6 +379,42 @@ int fo1_sample_tokens(const float* logits, int64_t ld, int32_t n_rows, int32_t v
  * fo1_llm_generate (greedy). */
 int fo1_llm_generate_sampled(fo1_model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Per-token scores (HF generate's return_dict_in_generate with output_logits / output_scores, and the log-probability of each
+ * emitted token that model.compute_transition_scores(..., normalize_logits=True) derives from them).  For sequence b at output
+ * column t (0 <= t < out_lens[b]):
+ *   logits[t][b]  the fp32 row the token was chosen from, as the LM head produced it (persistent kernel: the fp32 head epilogue;
+ *                 per-kernel path: the LM-head GEMM output).  Column 0 is the prefill's last-position row, bit-identical to
+ *                 prefill_logits.  Unlike the reference's outputs.logits.float(), these are not rounded to bf16.
+ *   scores[t][b]  the processed row, as HF's _sample forms next_token_scores: a greedy (raw) row is its logits unchanged; a sampled
+ *                 row is x = logits / T (IEEE fp32 division) where the token is kept and -inf elsewhere.  The kept set is the
+ *                 sampler's: top-k keeps x >= the k-th largest (ties included), top-p the canonical order and fixed-point weights;
+ *                 for top_k == 1 it is every token equal to the maximum (HF's TopK rule; the token drawn is still the
+ *                 lowest-index maximum).
+ *   logprobs[b][t] ln of the emitted token's probability under scores[t][b]: (x_tok - x_max) - ln(Z_kept * 2^-40), Z_kept the
+ *                 sampler's fixed-point sum of exp(x - x_max) over the kept set (a raw row: the whole vocabulary, T = 1).  0 at
+ *                 or past out_lens[b].  Depends only on the row, its parameters and the token (not on the slot, batch or path).
+ * Rows of scores / logits past a sequence's stop column, or of steps an early exit skipped, are unspecified.  Asking for any
+ * of these never changes a token: the tokens are bit-identical to the same call without scoring.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct {
+  float* logprobs;          /* optional DEVICE fp32 [n_seqs][max_new_tokens] */
+  float* scores;            /* optional DEVICE fp32 [max_new_tokens][n_seqs][vocab] (HF output_scores) */
+  float* logits;            /* optional DEVICE fp32 [max_new_tokens][n_seqs][vocab] (HF output_logits) */
+  const int32_t* raw_rows;  /* optional HOST [n_seqs]: 1 = greedy sequence (top_k 1, temperature 1), scored on its raw logits.
+                               Ignored when sp == NULL: every sequence is then greedy and raw. */
+} fo1_score_desc;
+/* fo1_llm_generate_sampled with scoring; sc == NULL or all its outputs NULL is exactly fo1_llm_generate_sampled (sp == NULL:
+ * greedy).  A greedy call with scoring samples with top_k 1, which is bit-identical to greedy. */
+int fo1_llm_generate_scored(fo1_model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp /* NULL: greedy */,
+                            const fo1_score_desc* sc, void* stream);
+/* The scoring of fo1_llm_generate_scored for arbitrary tokens: rows [n_rows] of fp32 logits (DEVICE, pitch ld) -> logprobs[r]
+ * of tokens[r] (-inf for a token outside the kept set) and, optionally, the processed rows scores[r] (pitch ld_scores).
+ * sp == NULL or raw_rows[r] == 1: the row is scored raw (T = 1, nothing cut). */
+int fo1_score_rows(const float* logits, int64_t ld, int32_t n_rows, int32_t vocab, const fo1_sampling_desc* sp /* NULL: raw */,
+                   const int32_t* raw_rows /* HOST, optional */, const int32_t* tokens /* DEVICE [n_rows] */,
+                   float* logprobs /* DEVICE [n_rows] */, float* scores /* DEVICE, optional */, int64_t ld_scores, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -71,6 +71,11 @@ def sampling_desc(temperature, top_p, top_k, seed):
     return SamplingDesc(*arrs), arrs
 
 
+class ScoreDesc(C.Structure):
+    """fo1_score_desc: optional DEVICE outputs logprobs [n][max_new], scores / logits [max_new][n][V]; HOST raw_rows [n]."""
+    _fields_ = [("logprobs", C.c_void_p), ("scores", C.c_void_p), ("logits", C.c_void_p), ("raw_rows", C.POINTER(C.c_int32))]
+
+
 _lib = None
 
 
@@ -109,6 +114,11 @@ def lib() -> C.CDLL:
                                     C.c_void_p, C.c_size_t, C.c_void_p]
     L.fo1_llm_generate_sampled.restype = C.c_int
     L.fo1_llm_generate_sampled.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(SamplingDesc), C.c_void_p]
+    L.fo1_llm_generate_scored.restype = C.c_int
+    L.fo1_llm_generate_scored.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(SamplingDesc), C.POINTER(ScoreDesc), C.c_void_p]
+    L.fo1_score_rows.restype = C.c_int
+    L.fo1_score_rows.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.POINTER(SamplingDesc), C.POINTER(C.c_int32), C.c_void_p,
+                                 C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
     _lib = L
     return L
 

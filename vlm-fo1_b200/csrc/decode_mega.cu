@@ -590,8 +590,10 @@ __device__ __forceinline__ void mg_attention_phase(const MegaArgs& a, uint8_t* s
 
 // ----------------------------------------------------------------------------------------------------------- kernel
 // SAMPLE = false: the greedy loop.  SAMPLE = true: the head stores its logits, CTA b < B draws sequence b's token with the
-// row routine of sampling.cuh (one more grid barrier per step), CTA 0 records the drawn tokens.
-template <int MT, bool SAMPLE>
+// row routine of sampling.cuh (one more grid barrier per step), CTA 0 records the drawn tokens.  SCORE (with SAMPLE): CTA b also
+// scores row b in the same phase -- one more pass over the row for Z_kept, the log-probability and the optional scores / logits
+// rows (a greedy call runs here with top_k = 1, which draws the arg-max).
+template <int MT, bool SAMPLE, bool SCORE = false>
 __global__ void __launch_bounds__(kMgThreads, 1) decode_mega_kernel(const MegaArgs a) {
   using Lay = MgLay<MT>;
   extern __shared__ __align__(128) uint8_t mg_smem[];
@@ -707,8 +709,21 @@ __global__ void __launch_bounds__(kMgThreads, 1) decode_mega_kernel(const MegaAr
         mg_wait<0>();
         SampleSmem<kMgThreads>& sm = *reinterpret_cast<SampleSmem<kMgThreads>*>(mg_smem);
         const int b = blockIdx.x;
-        const int tok = sample_row<kMgThreads>(a.logits + (long long)b * a.V, a.V, a.samp[b], __ldcg(a.step), sm);
-        if (threadIdx.x == 0) a.samp_tok[b] = tok;
+        if constexpr (SCORE) {
+          const float* row = a.logits + (long long)b * a.V;
+          const int step = __ldcg(a.step);
+          const int tok = sample_row<kMgThreads, SMP_DRAW_KEPT>(row, a.V, a.samp[b], step, sm);
+          if (threadIdx.x == 0) a.samp_tok[b] = tok;
+          if (step < a.max_new && !__ldcg(a.finished + b)) {       // past the sequence's stop nothing is recorded
+            const long long o = ((long long)step * a.B + b) * a.V;
+            const float lp = score_row<kMgThreads>(row, a.V, a.samp[b].temperature, tok, sm, a.sc_scores ? a.sc_scores + o : nullptr,
+                                                   a.sc_logits ? a.sc_logits + o : nullptr);
+            if (threadIdx.x == 0 && a.sc_logprobs != nullptr) a.sc_logprobs[(long long)b * a.max_new + step] = lp;
+          }
+        } else {
+          const int tok = sample_row<kMgThreads>(a.logits + (long long)b * a.V, a.V, a.samp[b], __ldcg(a.step), sm);
+          if (threadIdx.x == 0) a.samp_tok[b] = tok;
+        }
       }
     } else {
       MgEpi e;
@@ -787,8 +802,11 @@ int decode_mega_grid() {
         cudaFuncSetAttribute(decode_mega_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMgSmemBytes) == cudaSuccess &&
         cudaFuncSetAttribute(decode_mega_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMgSmemBytes) == cudaSuccess &&
         cudaFuncSetAttribute(decode_mega_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMgSmemBytes) == cudaSuccess &&
+        cudaFuncSetAttribute(decode_mega_kernel<1, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMgSmemBytes) == cudaSuccess &&
+        cudaFuncSetAttribute(decode_mega_kernel<2, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMgSmemBytes) == cudaSuccess &&
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decode_mega_kernel<2, false>, kMgThreads, kMgSmemBytes) == cudaSuccess && per_sm >= 1 &&
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decode_mega_kernel<2, true>, kMgThreads, kMgSmemBytes) == cudaSuccess && per_sm >= 1)
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decode_mega_kernel<2, true>, kMgThreads, kMgSmemBytes) == cudaSuccess && per_sm >= 1 &&
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decode_mega_kernel<2, true, true>, kMgThreads, kMgSmemBytes) == cudaSuccess && per_sm >= 1)
       grid = device_sm_count();
     else
       fprintf(stderr, "[fo1] decode_mega: cooperative launch with %d B of shared memory is not available (%s); using the per-kernel decode path\n",
@@ -810,7 +828,10 @@ int decode_mega_run(const MegaArgs& a, cudaStream_t s) {
   void* params[] = {&args};
   ProfScope prof("decode_mega", 0.0, 0.0, s);
   FO1_CHECK_ARG(a.samp == nullptr || (a.logits != nullptr && a.samp_tok != nullptr && (a.V & 1) == 0), "decode_mega: sampling buffers missing");
-  void* fn = a.samp != nullptr ? (a.B <= 16 ? reinterpret_cast<void*>(decode_mega_kernel<1, true>) : reinterpret_cast<void*>(decode_mega_kernel<2, true>))
+  const bool scored = a.sc_logprobs != nullptr || a.sc_scores != nullptr || a.sc_logits != nullptr;
+  FO1_CHECK_ARG(!scored || a.samp != nullptr, "decode_mega: scoring needs the per-row sampling parameters");
+  void* fn = scored ? (a.B <= 16 ? reinterpret_cast<void*>(decode_mega_kernel<1, true, true>) : reinterpret_cast<void*>(decode_mega_kernel<2, true, true>))
+           : a.samp != nullptr ? (a.B <= 16 ? reinterpret_cast<void*>(decode_mega_kernel<1, true>) : reinterpret_cast<void*>(decode_mega_kernel<2, true>))
                                : (a.B <= 16 ? reinterpret_cast<void*>(decode_mega_kernel<1, false>) : reinterpret_cast<void*>(decode_mega_kernel<2, false>));
   FO1_CUDA(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(kMgThreads), params, kMgSmemBytes, s));
   count_launch();

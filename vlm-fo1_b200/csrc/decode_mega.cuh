@@ -39,6 +39,8 @@ struct MegaArgs {
   float* logits;                    // [B][V] fp32 head output
   const SampleRowParams* samp;      // [B] per-sequence temperature, top-p, top-k, seed
   int* samp_tok;                    // [B] the token CTA b drew for sequence b
+  // scored decoding (decode_mega_kernel<MT, true, true>; any may be nullptr): logprobs [B][max_new], scores / logits [max_new][B][V]
+  float *sc_logprobs, *sc_scores, *sc_logits;
 };
 
 

@@ -500,7 +500,8 @@ static int llm_layer(Model* m, int li, const bf16* x_in, bf16* x_out, const Laye
   return FO1_OK;
 }
 
-static int llm_generate_impl(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, cudaStream_t s, bool dry, const DecodeState& st) {
+static int llm_generate_impl(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, const fo1_score_desc* sc, cudaStream_t s, bool dry,
+                             const DecodeState& st) {
   const fo1_model_config& c = m->cfg;
   Arena& A = m->arena;
   const int B = d->n_seqs, H = c.llm_hidden, hd = c.llm_head_dim, V = c.llm_vocab;
@@ -540,9 +541,11 @@ static int llm_generate_impl(Model* m, fo1_generate_desc* d, const fo1_sampling_
   float* mg_amax_v = A.alloc<float>((size_t)std::max(mega_grid, 1) * 32);
   int* mg_amax_i = A.alloc<int>((size_t)std::max(mega_grid, 1) * 32);
   int* mg_sync = A.alloc<int>((size_t)B * c.llm_kv_heads + 8);      // [0]: grid barrier counter, [8..]: attention arrival counters
-  // sampled decoding: the per-sequence parameters on the device and the persistent kernel's per-row token slots
-  SampleRowParams* d_samp = sp ? A.alloc<SampleRowParams>(B) : nullptr;
-  int* d_samp_tok = sp ? A.alloc<int>(B) : nullptr;
+  // sampled or scored decoding: the per-sequence parameters on the device and the persistent kernel's per-row token slots.  A
+  // scored greedy call samples with top_k 1 (bit-identical to greedy) so that both paths score in the sampler's per-row pass.
+  const bool per_row = sp != nullptr || sc != nullptr;
+  SampleRowParams* d_samp = per_row ? A.alloc<SampleRowParams>(B) : nullptr;
+  int* d_samp_tok = per_row ? A.alloc<int>(B) : nullptr;
 
   // ---- integer tables of the packed batch ----
   const int *d_cu = nullptr, *d_row_seq = nullptr, *d_row_t = nullptr, *d_last = nullptr;
@@ -567,9 +570,9 @@ static int llm_generate_impl(Model* m, fo1_generate_desc* d, const fo1_sampling_
     if (d->rope_deltas_device != nullptr) FO1_CUDA(cudaMemcpyAsync(d_deltas, d->rope_deltas_device, B * sizeof(int), cudaMemcpyDeviceToDevice, s));
     else FO1_CUDA(cudaMemcpyAsync(d_deltas, d->rope_deltas, B * sizeof(int), cudaMemcpyHostToDevice, s));
     if (d->n_stop_ids > 0) FO1_CUDA(cudaMemcpyAsync(st.stop_ids, d->stop_ids, d->n_stop_ids * sizeof(int), cudaMemcpyHostToDevice, s));
-    if (sp) {
+    if (per_row) {
       std::vector<SampleRowParams> h(B);
-      for (int b = 0; b < B; ++b) h[b] = SampleRowParams{sp->temperature[b], sp->top_p[b], sp->top_k[b], 0, sp->seed[b]};
+      for (int b = 0; b < B; ++b) h[b] = score_row_params(sp, sc ? sc->raw_rows : nullptr, b);
       FO1_CUDA(cudaMemcpyAsync(d_samp, h.data(), B * sizeof(SampleRowParams), cudaMemcpyHostToDevice, s));
     }
   }
@@ -598,7 +601,14 @@ static int llm_generate_impl(Model* m, fo1_generate_desc* d, const fo1_sampling_
   decode_init_kernel<<<ceil_div(B, 128), 128, 0, s>>>(st, d_lens, d_deltas, B);
   FO1_LAUNCH_CHECK();
   if (d->max_new_tokens <= 0) return FO1_OK;
-  if (sp) {
+  // the token of column 0 (and, scored, its row's scores); score_rows reads the column from *st.step, as the captured step does
+  auto score_step = [&]() {
+    return score_rows(logits, V, B, V, d_samp, st.step, st.new_tok, true, st.finished, d->max_new_tokens, sc->logprobs, d->max_new_tokens,
+                      sc->scores, sc->logits, V, s);
+  };
+  if (sc) {
+    FO1_TRY(score_step());
+  } else if (sp) {
     FO1_TRY(sample_rows(logits, V, B, V, d_samp, st.step, 0, st.new_tok, s));     // step 0 (decode_init_kernel)
   } else {
     argmax_kernel<<<B, 1024, 0, s>>>(logits, V, st.new_tok);
@@ -627,7 +637,9 @@ static int llm_generate_impl(Model* m, fo1_generate_desc* d, const fo1_sampling_
     }
     FO1_TRY(rmsnorm(xin, H, m->llm.norm, lastn, H, B, H, c.rms_eps, s));
     FO1_TRY(linear(lastn, H, m->llm.lm_head, H, logits, V, FO1_F32, B, V, H, nullptr, 0, FO1_EPI_NONE, nullptr, 0, 0, s));
-    if (sp) {
+    if (sc) {
+      FO1_TRY(score_step());
+    } else if (sp) {
       FO1_TRY(sample_rows(logits, V, B, V, d_samp, st.step, 0, st.new_tok, s));   // the Philox step is read from *st.step on the device
     } else {
       launch_k(argmax_kernel, dim3(B), dim3(1024), 0, s, logits, V, st.new_tok);
@@ -656,13 +668,14 @@ static int llm_generate_impl(Model* m, fo1_generate_desc* d, const fo1_sampling_
     a.stop_ids = st.stop_ids; a.n_stop = d->n_stop_ids; a.pad_id = d->pad_id; a.max_new = d->max_new_tokens;
     a.out_tokens = d->out_tokens; a.out_lens = d->out_lens;
     a.logits = logits; a.samp = d_samp; a.samp_tok = d_samp_tok;
+    if (sc) { a.sc_logprobs = sc->logprobs; a.sc_scores = sc->scores; a.sc_logits = sc->logits; }
     a.n_steps = d->max_new_tokens - 1;
     a.bar = reinterpret_cast<unsigned*>(mg_sync);
     const int pairs = B * c.llm_kv_heads;
     a.n_splits = std::max(1, std::min(kMgMaxSplits, mega_grid / std::max(1, pairs)));
     FO1_CUDA(cudaMemsetAsync(mg_sync, 0, ((size_t)pairs + 8) * sizeof(int), s));
     unsigned long long* d_prof = nullptr;
-    const int prof_slots = 5 * c.llm_layers + 3 + (sp ? 1 : 0) + 8;     // (+ the sampling barrier) + 8 sub-stamps of one attention item (CTA 0, layer 1)
+    const int prof_slots = 5 * c.llm_layers + 3 + (per_row ? 1 : 0) + 8;     // (+ the sampling barrier) + 8 sub-stamps of one attention item (CTA 0, layer 1)
     if (getenv("FO1_MEGA_PROF") != nullptr) {       // diagnostic: where a decode iteration spends its time (stderr)
       FO1_CUDA(cudaMalloc(reinterpret_cast<void**>(&d_prof), (size_t)mega_grid * prof_slots * 2 * sizeof(unsigned long long)));
       FO1_CUDA(cudaMemsetAsync(d_prof, 0, (size_t)mega_grid * prof_slots * 2 * sizeof(unsigned long long), s));
@@ -763,7 +776,10 @@ static int llm_generate_impl(Model* m, fo1_generate_desc* d, const fo1_sampling_
   return rc;
 }
 
-int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, cudaStream_t s) {
+int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, const fo1_score_desc* sc, cudaStream_t s) {
+  // the per-sequence host arrays first: they are the caller's, and need neither the model nor the device
+  if (sp) FO1_TRY(sampling_check(sp, d->n_seqs, sc ? "fo1_llm_generate_scored" : "fo1_llm_generate_sampled"));
+  if (sc) FO1_TRY(raw_rows_check(sp, sc->raw_rows, d->n_seqs, "fo1_llm_generate_scored"));
   FO1_CHECK_ARG(m->llm.ok, "fo1_llm_generate: model not finalized (LLM weights unresolved)");
   const fo1_model_config& c = m->cfg;
   FO1_CHECK_ARG(d->n_seqs > 0 && d->seq_lens && d->inputs_embeds && d->position_ids && (d->rope_deltas || d->rope_deltas_device),
@@ -775,13 +791,12 @@ int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, cu
     FO1_CHECK_ARG(d->seq_lens[b] > 0, "fo1_llm_generate: sequence %d is empty", b);
     max_len = std::max(max_len, d->seq_lens[b]);
   }
-  if (sp) FO1_TRY(sampling_check(sp, d->n_seqs, "fo1_llm_generate_sampled"));
   DecodeState st;
   FO1_TRY(ensure_state(m, d->n_seqs, d->n_stop_ids, &st));
   FO1_TRY(ensure_kv(m, d->n_seqs, max_len + std::max(d->max_new_tokens, 1)));
   FO1_TRY(int_cache_trim(m));
   m->arena.reset(true);
-  FO1_TRY(llm_generate_impl(m, d, sp, s, true, st));
+  FO1_TRY(llm_generate_impl(m, d, sp, sc, s, true, st));
   FO1_TRY(arena_ensure(m, m->arena.peak));
   m->arena.reset(false);
   if (d->max_new_tokens > 0) {  // out_tokens pre-filled with pad so an early exit leaves a clean tail
@@ -789,8 +804,9 @@ int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, cu
     fill_int_kernel<<<(int)std::min<long long>((n + 255) / 256, 1024), 256, 0, s>>>(d->out_tokens, d->pad_id, n);
     FO1_LAUNCH_CHECK();
     FO1_CUDA(cudaMemsetAsync(d->out_lens, 0, d->n_seqs * sizeof(int), s));
+    if (sc && sc->logprobs) FO1_CUDA(cudaMemsetAsync(sc->logprobs, 0, (size_t)n * sizeof(float), s));      // 0 past out_lens
   }
-  return llm_generate_impl(m, d, sp, s, false, st);
+  return llm_generate_impl(m, d, sp, sc, s, false, st);
 }
 
 // -------------------------------------------------------------------------------- splice plan (host, integer)
@@ -903,12 +919,19 @@ extern "C" int fo1_llm_build_embeds(fo1_model* m, const int32_t* src_kind, const
 
 extern "C" int fo1_llm_generate(fo1_model* m, fo1_generate_desc* d, void* stream) {
   FO1_CHECK_ARG(m && d, "fo1_llm_generate: null argument");
-  return llm_generate(m, d, nullptr, static_cast<cudaStream_t>(stream));
+  return llm_generate(m, d, nullptr, nullptr, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int fo1_llm_generate_sampled(fo1_model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, void* stream) {
   FO1_CHECK_ARG(m && d, "fo1_llm_generate_sampled: null argument");
-  return llm_generate(m, d, sp, static_cast<cudaStream_t>(stream));
+  return llm_generate(m, d, sp, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int fo1_llm_generate_scored(fo1_model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, const fo1_score_desc* sc,
+                                       void* stream) {
+  FO1_CHECK_ARG(m && d, "fo1_llm_generate_scored: null argument");
+  if (sc != nullptr && sc->logprobs == nullptr && sc->scores == nullptr && sc->logits == nullptr) sc = nullptr;
+  return llm_generate(m, d, sp, sc, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" size_t fo1_decode_attention_workspace_bytes(int32_t n_seqs, int32_t q_heads) {

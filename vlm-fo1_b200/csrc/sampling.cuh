@@ -16,6 +16,16 @@
 // token; one more pass resolves the tie group of that value by index.  Weights are 1 (top-k) or exp(x - max) rounded to
 // 64-bit fixed point with 40 fraction bits: integer sums do not depend on the order of the additions, so the token is a
 // function of (row, T, p, k, seed, step) alone -- not of the thread count, the batch slot or the decode path.
+//
+// Scoring (HF generate's output_logits / output_scores, and the log-probability of each emitted token) reuses the row routine:
+//   kept set: the domain the draw walks -- top-k keeps x >= the k-th largest (ties included), top-p as above.  For k == 1 it is
+//     every token equal to the maximum (HF's TopK rule; then top-p), while the token drawn stays the lowest-index maximum.  A raw
+//     row (a greedy sequence) keeps the whole vocabulary with T = 1.
+//   scores row: x where kept, -inf elsewhere (a raw row: the logits unchanged).
+//   logprob of token t: (x_t - x_max) - ln(Z_kept * 2^-40), Z_kept the order-free fixed-point sum of exp(x - x_max) over the kept
+//     set; -inf for a token outside it.  Like the token, it depends on (row, T, p, k, t) alone.
+// sample_row<NT, SMP_DRAW> is the sampler; SMP_DRAW_KEPT also leaves the kept set in SampleSmem (the draw is unchanged) and
+// SMP_KEPT stops before the draw; score_row then makes one pass over the row.
 #pragma once
 #include <climits>
 
@@ -26,7 +36,8 @@ namespace fo1 {
 // per-row parameters as the kernels read them (one 24-byte record per row; host-validated by sampling_check)
 struct SampleRowParams {
   float temperature, top_p;
-  int top_k, pad_;
+  int top_k;
+  int raw;        // scored rows only: 1 = a greedy sequence (T = 1, top_k = 1) scored on its raw logits; 0 for the sampler
   unsigned long long seed;
 };
 
@@ -41,12 +52,28 @@ struct SampleSmem {
   unsigned long long tgt, above, res_incl;
   uint32_t res_key;
   int n_mem, res_idx, res_bin, found;
+  // the kept set {key > kept_key} u {key == kept_key, index <= kept_idx} and the row maximum (SMP_DRAW_KEPT / SMP_KEPT only)
+  uint32_t kept_key;
+  int kept_idx;
+  float kept_max;
 };
+
+enum { SMP_DRAW = 0, SMP_DRAW_KEPT = 1, SMP_KEPT = 2 };
 
 int sampling_check(const fo1_sampling_desc* sp, int n, const char* fn);   // host: parameter validation (no CUDA call)
 // rows [n_rows] of `logits` (pitch ld) -> out[r]; step[r * step_stride] is the Philox counter of row r (stride 0: one step)
 int sample_rows(const float* logits, long long ld, int n_rows, int V, const SampleRowParams* prm, const int* step, int step_stride,
                 int* out, cudaStream_t s);
+// scored rows [n_rows] of `logits` (pitch ld).  The output column is *col (nullptr: 0).  draw: tok[r] = the sampled token (the
+// Philox step is the column), else tok[r] is the token to score.  finished (nullptr: none) / max_new: rows to skip (their token is
+// still drawn).  logprobs[r * lp_stride + col]; optional scores / logits_out rows at ((col * n_rows + r) * ld_out).
+int score_rows(const float* logits, long long ld, int n_rows, int V, const SampleRowParams* prm, const int* col, int* tok, bool draw,
+               const int* finished, int max_new, float* logprobs, long long lp_stride, float* scores, float* logits_out, long long ld_out,
+               cudaStream_t s);
+// host: raw_rows (optional, 0 / 1 per row) validation -- with sp, a raw row must be greedy (top_k 1, temperature 1) -- and the
+// device parameters of a scored row (sp == nullptr or a raw row: greedy, scored on the raw logits)
+int raw_rows_check(const fo1_sampling_desc* sp, const int32_t* raw_rows, int n, const char* fn);
+SampleRowParams score_row_params(const fo1_sampling_desc* sp, const int32_t* raw_rows, int r);
 
 #ifdef __CUDACC__
 __device__ __forceinline__ uint32_t smp_key(float x) {
@@ -196,8 +223,9 @@ __device__ void smp_cut(const float* __restrict__ row, int V, float T, float xma
   }
 }
 
-// the token of one row; every thread of the CTA calls it and gets the same value
-template <int NT>
+// the token of one row; every thread of the CTA calls it and gets the same value.  MODE != SMP_DRAW: the kept set is left in
+// sm.kept_* (SMP_KEPT returns the arg-max without drawing)
+template <int NT, int MODE = SMP_DRAW>
 __device__ int sample_row(const float* __restrict__ row, int V, const SampleRowParams& prm, int step, SampleSmem<NT>& sm) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const float T = prm.temperature;
@@ -222,24 +250,75 @@ __device__ int sample_row(const float* __restrict__ row, int V, const SampleRowP
   for (int w = 1; w < NT / 32; ++w)
     if (sm.maxv[w] > bv || (sm.maxv[w] == bv && sm.maxi[w] < bi)) { bv = sm.maxv[w]; bi = sm.maxi[w]; }
   __syncthreads();
-  if (prm.top_k == 1) return bi;
+  if constexpr (MODE == SMP_DRAW) {
+    if (prm.top_k == 1) return bi;
+  }
   uint32_t dk = 0u;
   int di = INT_MAX;
-  if (prm.top_k > 1 && prm.top_k < V) {
+  bool cut = true;
+  if constexpr (MODE != SMP_DRAW) {
+    cut = !prm.raw;
+    if (prm.top_k == 1) dk = smp_key(bv);        // HF's TopK(1): every token equal to the maximum
+  }
+  if (cut && prm.top_k > 1 && prm.top_k < V) {
     smp_cut<NT>(row, V, T, bv, dk, di, 0, (double)prm.top_k, sm);
     dk = sm.res_key;                    // kept: x >= the k-th largest (ties included)
     __syncthreads();
   }
-  if (prm.top_p < 1.0f) {
+  if (cut && prm.top_p < 1.0f) {
     smp_cut<NT>(row, V, T, bv, dk, di, 1, (double)prm.top_p, sm);
     if (sm.found) { dk = sm.res_key; di = sm.res_idx; }
     __syncthreads();
+  }
+  if constexpr (MODE != SMP_DRAW) {
+    if (tid == 0) { sm.kept_key = cut ? dk : 0u; sm.kept_idx = cut ? di : INT_MAX; sm.kept_max = bv; }
+    if (MODE == SMP_KEPT || prm.top_k == 1) { __syncthreads(); return bi; }
   }
   smp_cut<NT>(row, V, T, bv, dk, di, 2, (double)smp_uniform(prm.seed, (uint32_t)step), sm);
   // (the integer target floor(u Z) < Z always crosses; the arg-max stands in if it ever did not)
   const int tok = sm.found ? sm.res_idx : bi;
   __syncthreads();
   return tok;
+}
+
+// After sample_row<NT, SMP_DRAW_KEPT or SMP_KEPT> on the same row: one pass that sums Z_kept and writes the optional scores row
+// (x kept, -inf elsewhere) and copy of the raw row.  Returns the log-probability of `tok` in thread 0 (-inf outside the kept set).
+template <int NT>
+__device__ float score_row(const float* __restrict__ row, int V, float T, int tok, SampleSmem<NT>& sm, float* __restrict__ scores,
+                           float* __restrict__ raw_out) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const bool scale = T != 1.0f;
+  const uint32_t dk = sm.kept_key;
+  const int di = sm.kept_idx;
+  const float xmax = sm.kept_max;
+  unsigned long long z = 0ull;
+  for (int i = tid; i < V; i += NT) {
+    const float raw = __ldcg(row + i);
+    const float x = scale ? __fdiv_rn(raw, T) : raw;
+    const uint32_t k = smp_key(x);
+    const bool kept = !(k < dk || (k == dk && i > di));
+    if (kept) z += __float2ull_rn(expf(x - xmax) * 1099511627776.0f);   // 2^40
+    if (scores != nullptr) scores[i] = kept ? x : -INFINITY;
+    if (raw_out != nullptr) raw_out[i] = raw;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) z += __shfl_xor_sync(0xffffffffu, z, o);
+  if (lane == 0) sm.part[warp] = z;
+  __syncthreads();
+  float lp = 0.f;
+  if (tid == 0) {
+    unsigned long long Z = 0ull;
+    for (int w = 0; w < NT / 32; ++w) Z += sm.part[w];
+    lp = -INFINITY;
+    if (tok >= 0 && tok < V) {
+      const float raw = __ldcg(row + tok);
+      const float x = scale ? __fdiv_rn(raw, T) : raw;
+      const uint32_t k = smp_key(x);
+      if (!(k < dk || (k == dk && tok > di))) lp = (float)(((double)x - (double)xmax) - log((double)Z * 0x1p-40));
+    }
+  }
+  __syncthreads();
+  return lp;
 }
 #endif
 

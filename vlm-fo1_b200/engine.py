@@ -258,9 +258,15 @@ class Sampling:
 def _engine_generate(self, inputs_embeds: torch.Tensor, position_ids: torch.Tensor, seq_lens: Sequence[int],
                      rope_deltas: Sequence[int], max_new_tokens: int, stop_ids: Sequence[int], pad_id: int,
                      want_prefill_logits: bool = False, want_all_logits: bool = False, early_exit_interval: int = 8,
-                     sampling: Optional[Sampling] = None):
+                     sampling: Optional[Sampling] = None, want_logprobs: bool = False, want_scores: bool = False,
+                     want_logits: bool = False, raw_rows: Optional[Sequence[int]] = None):
     """Prefill + decode of a packed batch: greedy, or sampled per sequence when ``sampling`` is given.  position_ids int32
-    [3, sum L].  Returns a dict of device tensors."""
+    [3, sum L].  Returns a dict of device tensors.
+
+    Scoring (include/fo1.h, fo1_score_desc): ``want_logprobs`` adds ``logprobs`` fp32 [B, max_new] (the log-probability of each
+    emitted token, 0 past ``lens``); ``want_scores`` / ``want_logits`` add ``scores`` / ``logits`` fp32 [max_new, B, V] (HF's
+    output_scores / output_logits).  Each buffer is allocated only when asked for.  ``raw_rows`` (one 0 / 1 per sequence, with
+    ``sampling``): 1 marks a greedy sequence (top_k 1, temperature 1) scored on its raw logits.  Tokens never depend on these."""
     B = len(seq_lens)
     V = self.cfg.llm["vocab_size"]
     T = int(sum(seq_lens))
@@ -272,6 +278,9 @@ def _engine_generate(self, inputs_embeds: torch.Tensor, position_ids: torch.Tens
     lens = torch.zeros((B,), dtype=torch.int32, device=self.device)
     pl = torch.empty((B, V), dtype=torch.float32, device=self.device) if want_prefill_logits else None
     al = torch.empty((T, V), dtype=torch.float32, device=self.device) if want_all_logits else None
+    lp = torch.empty((B, max_new_tokens), dtype=torch.float32, device=self.device) if want_logprobs else None
+    sc = torch.empty((max_new_tokens, B, V), dtype=torch.float32, device=self.device) if want_scores else None
+    lg = torch.empty((max_new_tokens, B, V), dtype=torch.float32, device=self.device) if want_logits else None
     d = GenerateDescC()
     d.n_seqs = B
     sl = (C.c_int32 * B)(*[int(x) for x in seq_lens])
@@ -289,14 +298,30 @@ def _engine_generate(self, inputs_embeds: torch.Tensor, position_ids: torch.Tens
     d.all_logits = al.data_ptr() if al is not None else None
     d.early_exit_interval = early_exit_interval
     L = lib()
-    if sampling is None:
+    scored = lp is not None or sc is not None or lg is not None
+    if sampling is not None:
+        sd, _keep = _lib.sampling_desc(sampling.temperature, sampling.top_p, sampling.top_k, sampling.seed)
+        assert len(sampling.temperature) == B, "one sampling parameter set per sequence"
+    if scored:
+        ptr = lambda t: t.data_ptr() if t is not None else None
+        rr = (C.c_int32 * B)(*[int(x) for x in raw_rows]) if raw_rows is not None else None
+        assert raw_rows is None or len(raw_rows) == B, "one raw_rows flag per sequence"
+        desc = _lib.ScoreDesc(ptr(lp), ptr(sc), ptr(lg), rr)
+        check(L.fo1_llm_generate_scored(self._h, C.byref(d), C.byref(sd) if sampling is not None else None, C.byref(desc), _stream()),
+              "fo1_llm_generate_scored")
+    elif sampling is None:
         L.fo1_llm_generate.restype = C.c_int
         check(L.fo1_llm_generate(self._h, C.byref(d), _stream()), "fo1_llm_generate")
     else:
-        sd, _keep = _lib.sampling_desc(sampling.temperature, sampling.top_p, sampling.top_k, sampling.seed)
-        assert len(sampling.temperature) == B, "one sampling parameter set per sequence"
         check(L.fo1_llm_generate_sampled(self._h, C.byref(d), C.byref(sd), _stream()), "fo1_llm_generate_sampled")
-    return dict(tokens=toks, lens=lens, prefill_logits=pl, all_logits=al, steps_run=d.steps_run)
+    out = dict(tokens=toks, lens=lens, prefill_logits=pl, all_logits=al, steps_run=d.steps_run)
+    if want_logprobs:
+        out["logprobs"] = lp
+    if want_scores:
+        out["scores"] = sc
+    if want_logits:
+        out["logits"] = lg
+    return out
 
 
 def sample_tokens(logits: torch.Tensor, temperature: Sequence[float], top_p: Sequence[float], top_k: Sequence[int], seed: Sequence[int],
@@ -317,9 +342,32 @@ def sample_tokens(logits: torch.Tensor, temperature: Sequence[float], top_p: Seq
     return out
 
 
+def score_rows(logits: torch.Tensor, tokens: torch.Tensor, temperature: Optional[Sequence[float]] = None,
+               top_p: Optional[Sequence[float]] = None, top_k: Optional[Sequence[int]] = None, raw_rows: Optional[Sequence[int]] = None,
+               want_scores: bool = False):
+    """The scoring of a decode step for arbitrary tokens (fo1_score_rows): fp32 logits [n, V] on the device, tokens [n] ->
+    (logprobs fp32 [n], scores fp32 [n, V] or None).  Without sampling parameters every row is scored raw; ``raw_rows`` marks
+    single rows raw.  A token outside a row's kept set gets -inf."""
+    assert logits.is_cuda and logits.dtype == torch.float32 and logits.dim() == 2 and logits.stride(1) == 1
+    n, V = logits.shape
+    tokens = tokens.to(logits.device, torch.int32).contiguous()
+    assert tokens.numel() == n, "one token per row"
+    lp = torch.empty((n,), dtype=torch.float32, device=logits.device)
+    sc = torch.empty((n, V), dtype=torch.float32, device=logits.device) if want_scores else None
+    sd = keep = None
+    if temperature is not None:
+        sd, keep = _lib.sampling_desc(temperature, top_p, top_k, [0] * n)
+    rr = (C.c_int32 * n)(*[int(x) for x in raw_rows]) if raw_rows is not None else None
+    check(lib().fo1_score_rows(C.c_void_p(logits.data_ptr()), logits.stride(0), n, V, C.byref(sd) if sd is not None else None, rr,
+                               C.c_void_p(tokens.data_ptr()), C.c_void_p(lp.data_ptr()), C.c_void_p(sc.data_ptr()) if sc is not None else None,
+                               V, _stream()), "fo1_score_rows")
+    return lp, sc
+
+
 Engine.build_embeds = _engine_build_embeds
 Engine.generate = _engine_generate
 Engine.sample_tokens = staticmethod(sample_tokens)
+Engine.score_rows = staticmethod(score_rows)
 
 
 def splice_plan_batch(prompts: Sequence[Sequence[int]], image_grids: Sequence[Sequence[Tuple[int, int]]], n_regions: Sequence[int], device,

@@ -183,8 +183,10 @@ class Fo1Pipeline:
 
     # ---- language side -----------------------------------------------------------------------------------
     def generate(self, samples: Sequence[SampleInputs], max_new_tokens: int, stop_ids: Sequence[int], pad_id: int = 151643,
-                 early_exit_interval: int = 8, want_prefill_logits: bool = False, sampling=None):
-        """``sampling``: None (greedy) or an engine.Sampling with one parameter set per sample."""
+                 early_exit_interval: int = 8, want_prefill_logits: bool = False, sampling=None, want_logprobs: bool = False,
+                 want_scores: bool = False, want_logits: bool = False, raw_rows=None):
+        """``sampling``: None (greedy) or an engine.Sampling with one parameter set per sample.  ``want_logprobs`` / ``want_scores`` /
+        ``want_logits`` / ``raw_rows``: per-token scores, as Engine.generate."""
         eng, dev = self.eng, self.eng.device
         samples = self.preprocess(samples)           # uint8 images -> the towers' input tensors, on the device
         feats, img_off, region_tokens, _ = self.encode(samples)
@@ -203,7 +205,8 @@ class Fo1Pipeline:
         deltas = plan["rope_delta"]
         self._mark("splice")
         out = eng.generate(embeds, pos, lens, deltas, max_new_tokens, stop_ids, pad_id, want_prefill_logits=want_prefill_logits,
-                           early_exit_interval=early_exit_interval, sampling=sampling)
+                           early_exit_interval=early_exit_interval, sampling=sampling, want_logprobs=want_logprobs, want_scores=want_scores,
+                           want_logits=want_logits, raw_rows=raw_rows)
         self._mark("llm_prefill_decode")
         out["prompt_lens"] = lens
         return out

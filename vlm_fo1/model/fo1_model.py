@@ -1,7 +1,8 @@
 """The object ``load_pretrained_model`` returns in place of the reference's ``OmChatQwen25VLForCausalLM``
 (vlm_fo1/model/language_model/omchat_qwen2_5_vl.py:28-41): same ``.config`` attributes the callers read, same
 ``.generate(**kwargs)`` contract (mm_utils.py:640-654 builds the kwargs; returns LongTensor [1, P + T] whose first P
-columns are ``inputs``), everything underneath delegated to the H100 engine."""
+columns are ``inputs``, or HF's GenerateDecoderOnlyOutput with ``return_dict_in_generate=True``), everything underneath
+delegated to the H100 engine."""
 from __future__ import annotations
 
 import math
@@ -63,6 +64,49 @@ class Fo1ForCausalLM:
             raise ValueError(f"`top_k` has to be a non-negative integer, but is {top_k}")
         return T, p, k
 
+    def _outputs(self, kwargs):
+        """None (a bare LongTensor, as today) or (output_scores, output_logits) of a return_dict_in_generate call.  Like HF, the
+        fields come from the call's kwargs, else from generation_config.json, and only the dict carries them.  Attentions and
+        hidden states are refused: the decode loop never materialises them."""
+        gc = self.generation_config
+
+        def get(name):
+            v = kwargs.get(name)
+            return bool(gc.get(name, False) if v is None else v)
+        if not get("return_dict_in_generate"):
+            return None
+        for name in ("output_attentions", "output_hidden_states"):
+            if get(name):
+                raise NotImplementedError(f"{name}=True is not supported by the fo1-b200 engine's generate (its output dict carries "
+                                          "sequences, scores and logits)")
+        return get("output_scores"), get("output_logits")
+
+    def _result(self, out, b, inputs, want):
+        """Sample b of an engine output -> what generate returns: LongTensor [1, P + n], or the output dict when ``want`` is set."""
+        n = int(out["lens"][b])
+        new = out["tokens"][b, :n].to(torch.long)
+        full = torch.cat([inputs[0].to(new.device), new]).unsqueeze(0)
+        if want is None:
+            return full
+        from transformers.generation.utils import GenerateDecoderOnlyOutput
+        rows = lambda key: tuple(out[key][t, b:b + 1] for t in range(n))       # n device views [1, V], the stop token's included
+        # past_key_values is None: the K/V cache lives in the engine and is reused by its next call
+        return GenerateDecoderOnlyOutput(sequences=full, scores=rows("scores") if want[0] else None,
+                                         logits=rows("logits") if want[1] else None, past_key_values=None)
+
+    def compute_transition_scores(self, sequences, scores, beam_indices=None, normalize_logits=False):
+        """HF's GenerationMixin.compute_transition_scores without beams: ``scores`` is the tuple generate returned (n tensors
+        [batch, V]) -> [batch, n], the score of each generated token (its log-probability with ``normalize_logits``).  V is the
+        rows' width (HF reads config.get_text_config(), which this config does not have)."""
+        if beam_indices is not None:
+            raise NotImplementedError("beam_indices: the fo1-b200 engine has no beam search")
+        n, V = len(scores), scores[0].shape[-1]
+        stacked = torch.stack(scores).reshape(n, -1).transpose(0, 1)           # [batch * V, n]
+        if normalize_logits:
+            stacked = torch.nn.functional.log_softmax(stacked.reshape(-1, V, n), dim=1).reshape(-1, n)
+        beams = torch.arange(scores[0].shape[0], device=sequences.device).view(-1, 1)
+        return stacked.gather(0, sequences[:, sequences.shape[-1] - n:] + beams * V)
+
     def _sample(self, inputs=None, images=None, images_aux=None, image_grid_thws=None, bbox_list=None, do_sample=False, temperature=0.0,
                 stopping_criteria=None, top_p=None, top_k=None, **kwargs):
         """One ``prepare_inputs`` dict -> (SampleInputs, stop ids, (T, p, k) or None): the argument checks of the reference's call
@@ -107,29 +151,32 @@ class Fo1ForCausalLM:
     @torch.no_grad()
     def generate(self, inputs=None, images=None, images_aux=None, image_grid_thws=None, bbox_list=None, do_sample=False, temperature=0.0,
                  max_new_tokens=512, streamer=None, top_p=1.0, use_cache=True, stopping_criteria=None, pad_token_id=None, top_k=None, **kwargs):
+        want = self._outputs(kwargs)
         sample, stop, samp = self._sample(inputs, images, images_aux, image_grid_thws, bbox_list, do_sample, temperature, stopping_criteria,
                                           top_p, top_k, **kwargs)
         pad = pad_token_id if pad_token_id is not None else (stop[0] if stop else 0)
         out = self.pipeline.generate([sample], int(max_new_tokens), sorted(set(stop)), pad_id=int(pad), early_exit_interval=8,
-                                     sampling=self._sampling([samp]))
-        n = int(out["lens"][0].item())
-        new = out["tokens"][0, :n].to(torch.long)
-        full = torch.cat([inputs[0].to(new.device), new]).unsqueeze(0)
+                                     sampling=self._sampling([samp]), want_scores=bool(want and want[0]), want_logits=bool(want and want[1]))
+        res = self._result(out, 0, inputs, want)
+        new = (res if want is None else res.sequences)[0, inputs.shape[1]:]
         if streamer is not None:
             # the whole completion is handed over at once (the decode loop is device-resident: no per-token host sync);
             # a streamer error is the caller's to see, as in HF's generate
             streamer.put(inputs.cpu())
             streamer.put(new.cpu())
             streamer.end()
-        return full
+        return res
 
     @torch.no_grad()
-    def generate_batch(self, batch, max_new_tokens=None):
+    def generate_batch(self, batch, max_new_tokens=None, output_logprobs=False):
         """``batch``: a list of the dicts ``prepare_inputs`` returns (one sample each, mm_utils.py:640-654).  All samples run as ONE
         packed batch through the engine (what the reference's evaluation loops do one image at a time, eval_coco.py:36-88).
-        -> list of LongTensor [1, P_b + T_b], each exactly what ``generate(**batch[b])`` returns."""
+        -> list of LongTensor [1, P_b + T_b], each exactly what ``generate(**batch[b])`` returns (the output dict where that dict
+        asks for it).  ``output_logprobs``: each element is (that, fp32 [1, n_b]), the log-probability of each generated token
+        computed on the device, with no vocabulary-wide rows."""
         if not batch:
             return []
+        wants = [self._outputs(kw) for kw in batch]
         keys = ("inputs", "images", "images_aux", "image_grid_thws", "bbox_list", "do_sample", "temperature", "stopping_criteria", "top_p",
                 "top_k") + tuple(n for n, _ in _UNSUPPORTED_PROCESSORS)
         samples, stops, samps = zip(*(self._sample(**{k: v for k, v in kw.items() if k in keys}) for kw in batch))
@@ -137,10 +184,15 @@ class Fo1ForCausalLM:
         T = int(max_new_tokens if max_new_tokens is not None else max(int(kw.get("max_new_tokens", 512)) for kw in batch))
         pads = [kw.get("pad_token_id") for kw in batch]
         pad = pads[0] if pads[0] is not None else (stop[0] if stop else 0)
-        out = self.pipeline.generate(list(samples), T, stop, pad_id=int(pad), early_exit_interval=8, sampling=self._sampling(samps))
-        lens = out["lens"].cpu().tolist()
+        sampling = self._sampling(samps)
+        # a greedy sample in a sampled batch is scored on its raw logits, as HF's greedy search reports them
+        raw = [int(s is None) for s in samps] if sampling is not None else None
+        out = self.pipeline.generate(list(samples), T, stop, pad_id=int(pad), early_exit_interval=8, sampling=sampling,
+                                     want_logprobs=bool(output_logprobs), want_scores=any(w is not None and w[0] for w in wants),
+                                     want_logits=any(w is not None and w[1] for w in wants), raw_rows=raw)
+        out["lens"] = out["lens"].cpu().tolist()
         res = []
         for b, kw in enumerate(batch):
-            new = out["tokens"][b, :lens[b]].to(torch.long)
-            res.append(torch.cat([kw["inputs"][0].to(new.device), new]).unsqueeze(0))
+            r = self._result(out, b, kw["inputs"], wants[b])
+            res.append((r, out["logprobs"][b:b + 1, :out["lens"][b]]) if output_logprobs else r)
         return res
