@@ -415,6 +415,43 @@ int fo1_score_rows(const float* logits, int64_t ld, int32_t n_rows, int32_t voca
                    const int32_t* raw_rows /* HOST, optional */, const int32_t* tokens /* DEVICE [n_rows] */,
                    float* logprobs /* DEVICE [n_rows] */, float* scores /* DEVICE, optional */, int64_t ld_scores, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Streamed decoding (what HF generate's `streamer` needs: each token as it is produced, and a way to stop early).  The decode
+ * loop stays on the device with no per-token host sync; the device publishes every output column into host memory the caller
+ * owns, and the host reads it whenever it chooses.
+ *   Layout: tokens [n_seqs][max_new_tokens] and lens [n_seqs] mirror out_tokens / out_lens; progress is one int32 holding
+ *           columns_published | FO1_STREAM_DONE; cancel is one int32 the host may set.  All are HOST pointers to pinned memory
+ *           mapped for the device (cudaHostAlloc, or cudaHostRegister with cudaHostRegisterMapped); pageable memory is rejected.
+ *   Publication: the code that records column t (the persistent kernel's CTA 0, or the per-kernel path's update kernel, which
+ *           also records column 0 after the prefill on both paths) writes column t of tokens, and lens, with exactly the values
+ *           out_tokens / out_lens get (pad included), fences at system scope, then release-stores progress = (t + 1) | done.
+ *           So after an acquire load of progress == c, columns < c of tokens are final, and lens[b] is final for every
+ *           sequence that stopped before column c (a running sequence may already show the next column's length).
+ *   done:   set at the last column: no sequence is active after this column's stop test, t + 1 == max_new_tokens, or the column
+ *           was cancelled.  Nothing is published after it, so the final progress is done | max(out_lens).  The call stores
+ *           progress = 0 before it enqueues anything, and done | 0 at once when max_new_tokens == 0.
+ *   cancel: read once per column, with a system-scope load, before the column is recorded.  When it is set, column t is still
+ *           recorded normally; then every running sequence ends there (out_lens = t + 1) and the loop stops.  For each sequence
+ *           the tokens before that cut are bit-identical to the same call without a cancel; the tail is pad.  The call never
+ *           clears cancel: the caller zeroes it before the call.
+ * Streaming changes no token, score or logit: the outputs are bit-identical to the same call without it.
+ * ---------------------------------------------------------------------------------------------- */
+#define FO1_STREAM_DONE (1 << 30)
+typedef struct {
+  int32_t* tokens;          /* HOST mapped [n_seqs][max_new_tokens] */
+  int32_t* lens;            /* HOST mapped [n_seqs] */
+  int32_t* progress;        /* HOST mapped [1] */
+  const int32_t* cancel;    /* HOST mapped [1], optional (NULL: the loop cannot be cancelled) */
+} fo1_stream_desc;
+/* fo1_llm_generate_scored with streaming; st == NULL is exactly fo1_llm_generate_scored.  The buffers are validated (non-NULL,
+ * pinned and mapped) before anything is launched; the device uses their cudaHostGetDevicePointer aliases. */
+int fo1_llm_generate_streamed(fo1_model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp /* NULL: greedy */,
+                              const fo1_score_desc* sc /* NULL: unscored */, const fo1_stream_desc* st, void* stream);
+/* Acquire load of *progress and release store of 1 to *cancel: plain host code (no device, no model), for hosts whose language
+ * cannot express the ordering (and for CPUs with a weaker memory model than x86). */
+int32_t fo1_stream_progress(const int32_t* progress);
+void fo1_stream_cancel(int32_t* cancel);
+
 #ifdef __cplusplus
 }
 #endif

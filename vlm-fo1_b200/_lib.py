@@ -76,6 +76,13 @@ class ScoreDesc(C.Structure):
     _fields_ = [("logprobs", C.c_void_p), ("scores", C.c_void_p), ("logits", C.c_void_p), ("raw_rows", C.POINTER(C.c_int32))]
 
 
+class StreamDesc(C.Structure):
+    """fo1_stream_desc: HOST pointers to pinned, mapped memory: tokens [n][max_new], lens [n], progress [1], cancel [1] (optional)."""
+    _fields_ = [("tokens", C.c_void_p), ("lens", C.c_void_p), ("progress", C.c_void_p), ("cancel", C.c_void_p)]
+
+
+FO1_STREAM_DONE = 1 << 30
+
 _lib = None
 
 
@@ -116,6 +123,13 @@ def lib() -> C.CDLL:
     L.fo1_llm_generate_sampled.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(SamplingDesc), C.c_void_p]
     L.fo1_llm_generate_scored.restype = C.c_int
     L.fo1_llm_generate_scored.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(SamplingDesc), C.POINTER(ScoreDesc), C.c_void_p]
+    L.fo1_llm_generate_streamed.restype = C.c_int
+    L.fo1_llm_generate_streamed.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(SamplingDesc), C.POINTER(ScoreDesc), C.POINTER(StreamDesc),
+                                            C.c_void_p]
+    L.fo1_stream_progress.restype = C.c_int32
+    L.fo1_stream_progress.argtypes = [C.c_void_p]
+    L.fo1_stream_cancel.restype = None
+    L.fo1_stream_cancel.argtypes = [C.c_void_p]
     L.fo1_score_rows.restype = C.c_int
     L.fo1_score_rows.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.POINTER(SamplingDesc), C.POINTER(C.c_int32), C.c_void_p,
                                  C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]

@@ -592,8 +592,9 @@ __device__ __forceinline__ void mg_attention_phase(const MegaArgs& a, uint8_t* s
 // SAMPLE = false: the greedy loop.  SAMPLE = true: the head stores its logits, CTA b < B draws sequence b's token with the
 // row routine of sampling.cuh (one more grid barrier per step), CTA 0 records the drawn tokens.  SCORE (with SAMPLE): CTA b also
 // scores row b in the same phase -- one more pass over the row for Z_kept, the log-probability and the optional scores / logits
-// rows (a greedy call runs here with top_k = 1, which draws the arg-max).
-template <int MT, bool SAMPLE, bool SCORE = false>
+// rows (a greedy call runs here with top_k = 1, which draws the arg-max).  STREAM: CTA 0 also mirrors each recorded column into the
+// caller's mapped host buffers and publishes it (a.stream), and honours the host's cancel flag.
+template <int MT, bool SAMPLE, bool SCORE = false, bool STREAM = false>
 __global__ void __launch_bounds__(kMgThreads, 1) decode_mega_kernel(const MegaArgs a) {
   using Lay = MgLay<MT>;
   extern __shared__ __align__(128) uint8_t mg_smem[];
@@ -744,6 +745,18 @@ __global__ void __launch_bounds__(kMgThreads, 1) decode_mega_kernel(const MegaAr
     // ---- CTA 0: merge the arg-max slots, record the token, stop test, advance the loop state (decode_update_kernel) ----
     if (blockIdx.x == 0) {
       const int step = *a.step;
+      // STREAM: publish only while a sequence is active (nothing after `done`); the host's cancel flag is read once per step
+      [[maybe_unused]] bool publish = false, cancel = false;
+      if constexpr (STREAM) {
+        __shared__ int s_stream[2];
+        if (threadIdx.x == 0) {
+          s_stream[0] = __ldcg(a.n_active) > 0 && step < a.max_new;
+          s_stream[1] = stream_cancel_requested(a.stream.cancel);
+        }
+        __syncthreads();
+        publish = s_stream[0] != 0;
+        cancel = publish && s_stream[1] != 0;
+      }
       __syncthreads();
       for (int b = warp; b < a.B; b += kMgWarps) {
         [[maybe_unused]] float bv = -INFINITY; int bi = 0x7fffffff;
@@ -769,9 +782,16 @@ __global__ void __launch_bounds__(kMgThreads, 1) decode_mega_kernel(const MegaAr
               a.out_lens[b] = step + 1;
               bool stop = false;
               for (int i = 0; i < a.n_stop; ++i) stop |= (tok == a.stop_ids[i]);
+              if constexpr (STREAM) stop |= cancel;                  // a cancelled sequence ends after this column
               if (stop) { a.finished[b] = 1; atomicSub(a.n_active, 1); }
+              if constexpr (STREAM) {
+                if (publish) { a.stream.tokens[(long long)b * a.max_new + step] = tok; a.stream.lens[b] = step + 1; }
+              }
             } else {
               a.out_tokens[(long long)b * a.max_new + step] = a.pad_id;
+              if constexpr (STREAM) {
+                if (publish) a.stream.tokens[(long long)b * a.max_new + step] = a.pad_id;
+              }
             }
           }
           a.cur_tok[b] = tok;
@@ -781,6 +801,12 @@ __global__ void __launch_bounds__(kMgThreads, 1) decode_mega_kernel(const MegaAr
       }
       __syncthreads();
       if (threadIdx.x == 0) *a.step = step + 1;
+      if constexpr (STREAM) {
+        if (threadIdx.x == 0 && publish) {
+          const bool done = cancel || __ldcg(a.n_active) <= 0 || step + 1 >= a.max_new;
+          stream_publish(a.stream.progress, (step + 1) | (done ? FO1_STREAM_DONE : 0));     // (after the bar.sync above: covers every warp's mirror writes)
+        }
+      }
     }
     MG_STAMP(slot, 0); mg_grid_sync(a.bar, gen); MG_STAMP(slot, 1); ++slot;
     if (__ldcg(a.n_active) <= 0) break;           // every sequence has emitted a stop id (the tail of out_tokens is pad already)
@@ -792,12 +818,26 @@ __global__ void __launch_bounds__(kMgThreads, 1) decode_mega_kernel(const MegaAr
 
 namespace fo1 {
 
+// the streamed instantiations, [MT - 1][0 greedy | 1 sampled | 2 scored]
+static void* const kMgStreamed[2][3] = {
+    {reinterpret_cast<void*>(decode_mega_kernel<1, false, false, true>), reinterpret_cast<void*>(decode_mega_kernel<1, true, false, true>),
+     reinterpret_cast<void*>(decode_mega_kernel<1, true, true, true>)},
+    {reinterpret_cast<void*>(decode_mega_kernel<2, false, false, true>), reinterpret_cast<void*>(decode_mega_kernel<2, true, false, true>),
+     reinterpret_cast<void*>(decode_mega_kernel<2, true, true, true>)}};
+
 int decode_mega_grid() {
   static int grid = -1;
   if (grid < 0) {
     grid = 0;
     int dev = 0, coop = 0, per_sm = 0;
-    if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev) == cudaSuccess && coop &&
+    bool streamed_ok = true;
+    for (int mt = 0; mt < 2; ++mt)
+      for (int k = 0; k < 3; ++k) {
+        streamed_ok = streamed_ok && cudaFuncSetAttribute(kMgStreamed[mt][k], cudaFuncAttributeMaxDynamicSharedMemorySize, kMgSmemBytes) == cudaSuccess;
+        streamed_ok = streamed_ok && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kMgStreamed[mt][k], kMgThreads, kMgSmemBytes) == cudaSuccess &&
+                      per_sm >= 1;
+      }
+    if (streamed_ok && cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev) == cudaSuccess && coop &&
         cudaFuncSetAttribute(decode_mega_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMgSmemBytes) == cudaSuccess &&
         cudaFuncSetAttribute(decode_mega_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMgSmemBytes) == cudaSuccess &&
         cudaFuncSetAttribute(decode_mega_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMgSmemBytes) == cudaSuccess &&
@@ -833,6 +873,8 @@ int decode_mega_run(const MegaArgs& a, cudaStream_t s) {
   void* fn = scored ? (a.B <= 16 ? reinterpret_cast<void*>(decode_mega_kernel<1, true, true>) : reinterpret_cast<void*>(decode_mega_kernel<2, true, true>))
            : a.samp != nullptr ? (a.B <= 16 ? reinterpret_cast<void*>(decode_mega_kernel<1, true>) : reinterpret_cast<void*>(decode_mega_kernel<2, true>))
                                : (a.B <= 16 ? reinterpret_cast<void*>(decode_mega_kernel<1, false>) : reinterpret_cast<void*>(decode_mega_kernel<2, false>));
+  FO1_CHECK_ARG(a.stream.progress == nullptr || (a.stream.tokens != nullptr && a.stream.lens != nullptr), "decode_mega: stream buffers missing");
+  if (a.stream.progress != nullptr) fn = kMgStreamed[a.B <= 16 ? 0 : 1][scored ? 2 : a.samp != nullptr ? 1 : 0];
   FO1_CUDA(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(kMgThreads), params, kMgSmemBytes, s));
   count_launch();
   return FO1_OK;

@@ -9,6 +9,26 @@ constexpr int kMgMaxSplits = 8;
 
 struct MegaLayer { const bf16 *qkv_w, *qkv_b, *o_w, *gu_w, *down_w; };
 
+// Streamed decoding (fo1_stream_desc, include/fo1.h): the device aliases of the caller's mapped, pinned host buffers.  The code
+// that records output column t mirrors it into tokens / lens, fences at system scope and release-stores progress = (t + 1) | done.
+struct StreamArgs {
+  int* tokens;          // [B][max_new] mirror of out_tokens
+  int* lens;            // [B] mirror of out_lens
+  int* progress;        // columns published | FO1_STREAM_DONE
+  const int* cancel;    // optional: != 0 asks the loop to stop after the column it records next
+};
+__device__ __forceinline__ int stream_cancel_requested(const int* cancel) {
+  int v = 0;
+  if (cancel != nullptr) asm volatile("ld.relaxed.sys.global.b32 %0, [%1];" : "=r"(v) : "l"(cancel) : "memory");
+  return v;
+}
+// by ONE thread after the bar.sync that follows the block's mirror writes: the system-scope fence and the release are cumulative, so
+// they order every thread's writes the barrier made visible to this one (one fence per step instead of one per writing warp)
+__device__ __forceinline__ void stream_publish(int* progress, int v) {
+  __threadfence_system();
+  asm volatile("st.release.sys.global.b32 [%0], %1;" ::"l"(progress), "r"(v) : "memory");
+}
+
 struct MegaArgs {
   int B, layers, H, QD, KD, hd, q_heads, kv_heads, I, V;
   float eps, theta;
@@ -41,10 +61,13 @@ struct MegaArgs {
   int* samp_tok;                    // [B] the token CTA b drew for sequence b
   // scored decoding (decode_mega_kernel<MT, true, true>; any may be nullptr): logprobs [B][max_new], scores / logits [max_new][B][V]
   float *sc_logprobs, *sc_scores, *sc_logits;
+  // streamed decoding (decode_mega_kernel<MT, SAMPLE, SCORE, true>; progress == nullptr otherwise)
+  StreamArgs stream;
 };
 
 
 int decode_mega_grid();                                   // CTAs of the cooperative launch (0: not available on this device)
-int decode_mega_run(const MegaArgs& a, cudaStream_t s);   // the whole decode loop, one launch (sampled when a.samp != nullptr)
+int decode_mega_run(const MegaArgs& a, cudaStream_t s);   // the whole decode loop, one launch (sampled when a.samp != nullptr,
+                                                          // streamed when a.stream.progress != nullptr)
 
 }  // namespace fo1

@@ -318,13 +318,27 @@ __global__ void decode_init_kernel(DecodeState st, const int* __restrict__ seq_l
   st.finished[b] = 0;
 }
 // record the sampled token, test the stop ids, advance the loop state.  ONE block; the output column is the
-// device-resident step counter, so the launch is identical every iteration (CUDA-graph replayable).
+// device-resident step counter, so the launch is identical every iteration (CUDA-graph replayable).  STREAM: the column is also
+// mirrored into the caller's mapped host buffers and published (the same protocol as decode_mega_kernel's record block); steps after
+// `done` publish nothing, and the host's cancel flag ends every sequence after the column recorded.
+template <bool STREAM>
 __global__ void __launch_bounds__(1024) decode_update_kernel(DecodeState st, int n_stop, int pad_id, int max_new,
                                                              int* __restrict__ out_tokens, int* __restrict__ out_lens, int B,
-                                                             int advance_cache) {
+                                                             int advance_cache, StreamArgs sa) {
   griddep_launch();
   griddep_wait();
   const int step = *st.step;
+  [[maybe_unused]] bool publish = false, cancel = false;
+  if constexpr (STREAM) {
+    __shared__ int s_stream[2];
+    if (threadIdx.x == 0) {
+      s_stream[0] = __ldcg(st.n_active) > 0 && step < max_new;
+      s_stream[1] = stream_cancel_requested(sa.cancel);
+    }
+    __syncthreads();
+    publish = s_stream[0] != 0;
+    cancel = publish && s_stream[1] != 0;
+  }
   __syncthreads();
   for (int b = threadIdx.x; b < B; b += blockDim.x) {
     const int tok = st.new_tok[b];
@@ -334,9 +348,16 @@ __global__ void __launch_bounds__(1024) decode_update_kernel(DecodeState st, int
         out_lens[b] = step + 1;
         bool stop = false;
         for (int i = 0; i < n_stop; ++i) stop |= (tok == st.stop_ids[i]);
+        if constexpr (STREAM) stop |= cancel;
         if (stop) { st.finished[b] = 1; atomicSub(st.n_active, 1); }
+        if constexpr (STREAM) {
+          if (publish) { sa.tokens[(long long)b * max_new + step] = tok; sa.lens[b] = step + 1; }
+        }
       } else {
         out_tokens[(long long)b * max_new + step] = pad_id;
+        if constexpr (STREAM) {
+          if (publish) sa.tokens[(long long)b * max_new + step] = pad_id;
+        }
       }
     }
     st.cur_tok[b] = tok;
@@ -347,6 +368,12 @@ __global__ void __launch_bounds__(1024) decode_update_kernel(DecodeState st, int
   }
   __syncthreads();
   if (threadIdx.x == 0) *st.step = step + 1;
+  if constexpr (STREAM) {
+    if (threadIdx.x == 0 && publish) {
+      const bool done = cancel || __ldcg(st.n_active) <= 0 || step + 1 >= max_new;
+      stream_publish(sa.progress, (step + 1) | (done ? FO1_STREAM_DONE : 0));
+    }
+  }
 }
 __global__ void fill_int_kernel(int* p, int v, long long n) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) p[i] = v;
@@ -501,7 +528,7 @@ static int llm_layer(Model* m, int li, const bf16* x_in, bf16* x_out, const Laye
 }
 
 static int llm_generate_impl(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, const fo1_score_desc* sc, cudaStream_t s, bool dry,
-                             const DecodeState& st) {
+                             const DecodeState& st, const StreamArgs& sa, const int32_t* h_progress) {
   const fo1_model_config& c = m->cfg;
   Arena& A = m->arena;
   const int B = d->n_seqs, H = c.llm_hidden, hd = c.llm_head_dim, V = c.llm_vocab;
@@ -615,7 +642,8 @@ static int llm_generate_impl(Model* m, fo1_generate_desc* d, const fo1_sampling_
     FO1_LAUNCH_CHECK();
   }
   const int upd_threads = std::min(1024, std::max(32, (B + 31) / 32 * 32));
-  decode_update_kernel<<<1, upd_threads, 0, s>>>(st, d->n_stop_ids, d->pad_id, d->max_new_tokens, d->out_tokens, d->out_lens, B, 0);
+  auto* const update_kernel = sa.progress != nullptr ? decode_update_kernel<true> : decode_update_kernel<false>;
+  update_kernel<<<1, upd_threads, 0, s>>>(st, d->n_stop_ids, d->pad_id, d->max_new_tokens, d->out_tokens, d->out_lens, B, 0, sa);
   FO1_LAUNCH_CHECK();
 
   // ---- greedy decode: every step is the SAME launch sequence reading its state from device memory; the first
@@ -645,7 +673,7 @@ static int llm_generate_impl(Model* m, fo1_generate_desc* d, const fo1_sampling_
       launch_k(argmax_kernel, dim3(B), dim3(1024), 0, s, logits, V, st.new_tok);
       FO1_LAUNCH_CHECK();
     }
-    launch_k(decode_update_kernel, dim3(1), dim3(upd_threads), 0, s, st, d->n_stop_ids, d->pad_id, d->max_new_tokens, d->out_tokens, d->out_lens, B, 1);
+    launch_k(update_kernel, dim3(1), dim3(upd_threads), 0, s, st, d->n_stop_ids, d->pad_id, d->max_new_tokens, d->out_tokens, d->out_lens, B, 1, sa);
     FO1_LAUNCH_CHECK();
     return FO1_OK;
   };
@@ -669,6 +697,7 @@ static int llm_generate_impl(Model* m, fo1_generate_desc* d, const fo1_sampling_
     a.out_tokens = d->out_tokens; a.out_lens = d->out_lens;
     a.logits = logits; a.samp = d_samp; a.samp_tok = d_samp_tok;
     if (sc) { a.sc_logprobs = sc->logprobs; a.sc_scores = sc->scores; a.sc_logits = sc->logits; }
+    a.stream = sa;
     a.n_steps = d->max_new_tokens - 1;
     a.bar = reinterpret_cast<unsigned*>(mg_sync);
     const int pairs = B * c.llm_kv_heads;
@@ -762,6 +791,8 @@ static int llm_generate_impl(Model* m, fo1_generate_desc* d, const fo1_sampling_
       if ((rc = enqueue_step()) != FO1_OK) break;
     }
     d->steps_run = step;
+    // streamed: `done` is in host memory, so the host loop stops enqueueing without a sync once the device has published it
+    if (h_progress != nullptr && (__atomic_load_n(h_progress, __ATOMIC_ACQUIRE) & FO1_STREAM_DONE)) break;
     if (d->early_exit_interval > 0 && step % d->early_exit_interval == 0) {
       if (cudaMemcpyAsync(ls->h_flag, st.n_active, sizeof(int), cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess) {
         set_error("early-exit poll failed"); rc = FO1_ERR_CUDA; break;
@@ -776,7 +807,29 @@ static int llm_generate_impl(Model* m, fo1_generate_desc* d, const fo1_sampling_
   return rc;
 }
 
-int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, const fo1_score_desc* sc, cudaStream_t s) {
+// the device aliases of the caller's stream buffers; each must be pinned host memory mapped into the device's address space
+static int stream_resolve(const fo1_stream_desc* h, StreamArgs* sa) {
+  const char* names[4] = {"tokens", "lens", "progress", "cancel"};
+  const void* hp[4] = {h->tokens, h->lens, h->progress, h->cancel};
+  void* dp[4] = {nullptr, nullptr, nullptr, nullptr};
+  for (int i = 0; i < 4; ++i) {
+    if (hp[i] == nullptr) continue;          // (only cancel may be NULL: checked by the caller)
+    cudaPointerAttributes at;
+    const bool host = cudaPointerGetAttributes(&at, hp[i]) == cudaSuccess && at.type == cudaMemoryTypeHost;
+    if (!host || cudaHostGetDevicePointer(&dp[i], const_cast<void*>(hp[i]), 0) != cudaSuccess || dp[i] == nullptr) {
+      cudaGetLastError();
+      set_error("fo1_llm_generate_streamed: stream buffer `%s` is not pinned host memory mapped for the device (cudaHostAlloc, "
+                "or cudaHostRegister with cudaHostRegisterMapped)", names[i]);
+      return FO1_ERR_INVALID_ARG;
+    }
+  }
+  sa->tokens = static_cast<int*>(dp[0]); sa->lens = static_cast<int*>(dp[1]); sa->progress = static_cast<int*>(dp[2]);
+  sa->cancel = static_cast<const int*>(dp[3]);
+  return FO1_OK;
+}
+
+int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, const fo1_score_desc* sc, const fo1_stream_desc* stm,
+                 cudaStream_t s) {
   // the per-sequence host arrays first: they are the caller's, and need neither the model nor the device
   if (sp) FO1_TRY(sampling_check(sp, d->n_seqs, sc ? "fo1_llm_generate_scored" : "fo1_llm_generate_sampled"));
   if (sc) FO1_TRY(raw_rows_check(sp, sc->raw_rows, d->n_seqs, "fo1_llm_generate_scored"));
@@ -791,12 +844,17 @@ int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, co
     FO1_CHECK_ARG(d->seq_lens[b] > 0, "fo1_llm_generate: sequence %d is empty", b);
     max_len = std::max(max_len, d->seq_lens[b]);
   }
+  StreamArgs sa = {};
+  if (stm) {
+    FO1_TRY(stream_resolve(stm, &sa));
+    __atomic_store_n(stm->progress, d->max_new_tokens > 0 ? 0 : FO1_STREAM_DONE, __ATOMIC_RELEASE);   // before anything is enqueued
+  }
   DecodeState st;
   FO1_TRY(ensure_state(m, d->n_seqs, d->n_stop_ids, &st));
   FO1_TRY(ensure_kv(m, d->n_seqs, max_len + std::max(d->max_new_tokens, 1)));
   FO1_TRY(int_cache_trim(m));
   m->arena.reset(true);
-  FO1_TRY(llm_generate_impl(m, d, sp, sc, s, true, st));
+  FO1_TRY(llm_generate_impl(m, d, sp, sc, s, true, st, sa, nullptr));
   FO1_TRY(arena_ensure(m, m->arena.peak));
   m->arena.reset(false);
   if (d->max_new_tokens > 0) {  // out_tokens pre-filled with pad so an early exit leaves a clean tail
@@ -806,7 +864,7 @@ int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, co
     FO1_CUDA(cudaMemsetAsync(d->out_lens, 0, d->n_seqs * sizeof(int), s));
     if (sc && sc->logprobs) FO1_CUDA(cudaMemsetAsync(sc->logprobs, 0, (size_t)n * sizeof(float), s));      // 0 past out_lens
   }
-  return llm_generate_impl(m, d, sp, sc, s, false, st);
+  return llm_generate_impl(m, d, sp, sc, s, false, st, sa, stm ? stm->progress : nullptr);
 }
 
 // -------------------------------------------------------------------------------- splice plan (host, integer)
@@ -919,20 +977,33 @@ extern "C" int fo1_llm_build_embeds(fo1_model* m, const int32_t* src_kind, const
 
 extern "C" int fo1_llm_generate(fo1_model* m, fo1_generate_desc* d, void* stream) {
   FO1_CHECK_ARG(m && d, "fo1_llm_generate: null argument");
-  return llm_generate(m, d, nullptr, nullptr, static_cast<cudaStream_t>(stream));
+  return llm_generate(m, d, nullptr, nullptr, nullptr, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int fo1_llm_generate_sampled(fo1_model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, void* stream) {
   FO1_CHECK_ARG(m && d, "fo1_llm_generate_sampled: null argument");
-  return llm_generate(m, d, sp, nullptr, static_cast<cudaStream_t>(stream));
+  return llm_generate(m, d, sp, nullptr, nullptr, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int fo1_llm_generate_scored(fo1_model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, const fo1_score_desc* sc,
                                        void* stream) {
   FO1_CHECK_ARG(m && d, "fo1_llm_generate_scored: null argument");
   if (sc != nullptr && sc->logprobs == nullptr && sc->scores == nullptr && sc->logits == nullptr) sc = nullptr;
-  return llm_generate(m, d, sp, sc, static_cast<cudaStream_t>(stream));
+  return llm_generate(m, d, sp, sc, nullptr, static_cast<cudaStream_t>(stream));
 }
+
+extern "C" int fo1_llm_generate_streamed(fo1_model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, const fo1_score_desc* sc,
+                                         const fo1_stream_desc* st, void* stream) {
+  FO1_CHECK_ARG(m && d, "fo1_llm_generate_streamed: null argument");
+  FO1_CHECK_ARG(st == nullptr || (st->tokens && st->lens && st->progress), "fo1_llm_generate_streamed: null stream buffer (tokens, lens and "
+                "progress are required; cancel may be NULL)");
+  if (sc != nullptr && sc->logprobs == nullptr && sc->scores == nullptr && sc->logits == nullptr) sc = nullptr;
+  return llm_generate(m, d, sp, sc, st, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int32_t fo1_stream_progress(const int32_t* progress) { return __atomic_load_n(progress, __ATOMIC_ACQUIRE); }
+
+extern "C" void fo1_stream_cancel(int32_t* cancel) { __atomic_store_n(cancel, 1, __ATOMIC_RELEASE); }
 
 extern "C" size_t fo1_decode_attention_workspace_bytes(int32_t n_seqs, int32_t q_heads) {
   return (size_t)(n_seqs > 0 ? n_seqs : 0) * (q_heads > 0 ? q_heads : 0) * fo1::kDecSplits * (128 + 4) * sizeof(float);

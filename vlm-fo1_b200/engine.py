@@ -3,8 +3,10 @@ the stage entry points with torch tensors as memory handles."""
 from __future__ import annotations
 
 import ctypes as C
+import threading
+import time
 from dataclasses import dataclass, field
-from typing import Dict, List, Optional, Sequence, Tuple
+from typing import Callable, Dict, List, Optional, Sequence, Tuple
 
 import torch
 
@@ -259,14 +261,21 @@ def _engine_generate(self, inputs_embeds: torch.Tensor, position_ids: torch.Tens
                      rope_deltas: Sequence[int], max_new_tokens: int, stop_ids: Sequence[int], pad_id: int,
                      want_prefill_logits: bool = False, want_all_logits: bool = False, early_exit_interval: int = 8,
                      sampling: Optional[Sampling] = None, want_logprobs: bool = False, want_scores: bool = False,
-                     want_logits: bool = False, raw_rows: Optional[Sequence[int]] = None):
+                     want_logits: bool = False, raw_rows: Optional[Sequence[int]] = None,
+                     on_tokens: Optional[Callable[[int, int, "np.ndarray", "np.ndarray"], Optional[bool]]] = None):
     """Prefill + decode of a packed batch: greedy, or sampled per sequence when ``sampling`` is given.  position_ids int32
     [3, sum L].  Returns a dict of device tensors.
 
     Scoring (include/fo1.h, fo1_score_desc): ``want_logprobs`` adds ``logprobs`` fp32 [B, max_new] (the log-probability of each
     emitted token, 0 past ``lens``); ``want_scores`` / ``want_logits`` add ``scores`` / ``logits`` fp32 [max_new, B, V] (HF's
     output_scores / output_logits).  Each buffer is allocated only when asked for.  ``raw_rows`` (one 0 / 1 per sequence, with
-    ``sampling``): 1 marks a greedy sequence (top_k 1, temperature 1) scored on its raw logits.  Tokens never depend on these."""
+    ``sampling``): 1 marks a greedy sequence (top_k 1, temperature 1) scored on its raw logits.  Tokens never depend on these.
+
+    Streaming (include/fo1.h, fo1_stream_desc): ``on_tokens(lo, hi, tokens, lens)`` is called in the calling thread whenever the
+    device has published new output columns: ``tokens`` int32 [B, hi - lo] (columns lo..hi-1, pad past a sequence's stop),
+    ``lens`` int32 [B] (each sequence's length as of column hi).  Returning True stops every sequence after the next column the
+    device records.  An exception from the callback (KeyboardInterrupt included) stops the device too, and is re-raised once it
+    has stopped.  The outputs are bit-identical to the same call without ``on_tokens`` (up to where a stop was asked for)."""
     B = len(seq_lens)
     V = self.cfg.llm["vocab_size"]
     T = int(sum(seq_lens))
@@ -307,6 +316,12 @@ def _engine_generate(self, inputs_embeds: torch.Tensor, position_ids: torch.Tens
         rr = (C.c_int32 * B)(*[int(x) for x in raw_rows]) if raw_rows is not None else None
         assert raw_rows is None or len(raw_rows) == B, "one raw_rows flag per sequence"
         desc = _lib.ScoreDesc(ptr(lp), ptr(sc), ptr(lg), rr)
+    if on_tokens is not None:
+        sp_arg = C.byref(sd) if sampling is not None else None
+        sc_arg = C.byref(desc) if scored else None
+        self._run_streamed(lambda stream, st: check(L.fo1_llm_generate_streamed(self._h, C.byref(d), sp_arg, sc_arg, C.byref(st), stream),
+                                                    "fo1_llm_generate_streamed"), B, max_new_tokens, on_tokens)
+    elif scored:
         check(L.fo1_llm_generate_scored(self._h, C.byref(d), C.byref(sd) if sampling is not None else None, C.byref(desc), _stream()),
               "fo1_llm_generate_scored")
     elif sampling is None:
@@ -364,8 +379,81 @@ def score_rows(logits: torch.Tensor, tokens: torch.Tensor, temperature: Optional
     return lp, sc
 
 
+_POLL_S = 2e-4      # host poll period of a streamed generate: a fraction of a decode step (about 3 ms at the 3B shape, B = 1)
+
+
+def _engine_stream_buffers(self, B: int, T: int):
+    """The pinned host buffers a streamed generate publishes into (fo1_stream_desc), allocated once and grown when a call needs
+    more: -> (tokens int32 [>= B * T], lens int32 [>= B], control int32 [32]: progress at [0], cancel at [16], a cache line apart)."""
+    buf = getattr(self, "_stream_buf", None)
+    if buf is None or buf[0].numel() < B * T or buf[1].numel() < B:
+        old = buf or (torch.empty(0), torch.empty(0), None)
+        buf = (torch.empty(max(B * T, old[0].numel()), dtype=torch.int32, pin_memory=True),
+               torch.empty(max(B, old[1].numel()), dtype=torch.int32, pin_memory=True),
+               old[2] if old[2] is not None else torch.zeros(32, dtype=torch.int32, pin_memory=True))
+        self._stream_buf = buf
+    return buf
+
+
+def _engine_run_streamed(self, launch, B: int, T: int, on_tokens) -> None:
+    """Run ``launch(stream, StreamDesc)`` (one fo1_llm_generate_streamed call) in a worker thread and deliver the published columns
+    to ``on_tokens`` from this thread.  The worker enqueues on this thread's current stream, on the engine's device (the library
+    does not set the device), and records an event after the call; the per-kernel path's host loop blocks in that call, so it
+    must not run where the polling does.  Polling ends on `done`, on the worker's failure (its Fo1Error is raised), or once the
+    event has completed (after one more drain), so a failed launch never leaves it spinning."""
+    import numpy as np
+    tok_t, lens_t, ctl_t = self._stream_buffers(B, max(T, 1))      # (a buffer is never empty: NULL is refused)
+    tok = tok_t.numpy()[:B * T].reshape(B, T)
+    lens, ctl = lens_t.numpy()[:B], ctl_t.numpy()
+    ctl[0] = 0                       # progress (the call stores 0 too; this keeps a previous call's `done` from being read first)
+    ctl[16] = 0                      # cancel
+    prog, cancel = ctl_t.data_ptr(), ctl_t.data_ptr() + 16 * 4
+    st = _lib.StreamDesc(tok_t.data_ptr(), lens_t.data_ptr(), prog, cancel)
+    L = lib()
+    stream = torch.cuda.current_stream(self.device)
+    finished_ev = torch.cuda.Event()
+    failure: List[BaseException] = []
+
+    def work():
+        try:
+            with torch.cuda.device(self.device):
+                launch(C.c_void_p(stream.cuda_stream), st)
+                finished_ev.record(stream)
+        except BaseException as e:  # noqa: BLE001 -- handed to the polling thread
+            failure.append(e)
+
+    worker = threading.Thread(target=work, name="fo1-generate-streamed", daemon=True)
+    worker.start()
+    seen = 0
+    try:
+        while True:
+            finished = not worker.is_alive() and (bool(failure) or finished_ev.query())     # read BEFORE the last drain
+            if failure:
+                raise failure[0]
+            p = int(L.fo1_stream_progress(prog))
+            cols = p & (_lib.FO1_STREAM_DONE - 1)
+            if cols > seen:
+                lo, seen = seen, cols
+                if on_tokens(lo, cols, tok[:, lo:cols].copy(), np.minimum(lens, cols).astype(np.int32)):
+                    L.fo1_stream_cancel(cancel)
+            if p & _lib.FO1_STREAM_DONE or finished:
+                break
+            time.sleep(_POLL_S)
+    except BaseException:
+        L.fo1_stream_cancel(cancel)     # the device stops within one step; wait for it, then re-raise
+        worker.join()
+        if not failure:
+            stream.synchronize()
+        raise
+    worker.join()
+    if failure:
+        raise failure[0]
+
+
 Engine.build_embeds = _engine_build_embeds
 Engine.generate = _engine_generate
+Engine._stream_buffers = _engine_stream_buffers
+Engine._run_streamed = _engine_run_streamed
 Engine.sample_tokens = staticmethod(sample_tokens)
 Engine.score_rows = staticmethod(score_rows)
 

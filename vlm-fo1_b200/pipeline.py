@@ -184,9 +184,10 @@ class Fo1Pipeline:
     # ---- language side -----------------------------------------------------------------------------------
     def generate(self, samples: Sequence[SampleInputs], max_new_tokens: int, stop_ids: Sequence[int], pad_id: int = 151643,
                  early_exit_interval: int = 8, want_prefill_logits: bool = False, sampling=None, want_logprobs: bool = False,
-                 want_scores: bool = False, want_logits: bool = False, raw_rows=None):
+                 want_scores: bool = False, want_logits: bool = False, raw_rows=None, on_tokens=None):
         """``sampling``: None (greedy) or an engine.Sampling with one parameter set per sample.  ``want_logprobs`` / ``want_scores`` /
-        ``want_logits`` / ``raw_rows``: per-token scores, as Engine.generate."""
+        ``want_logits`` / ``raw_rows``: per-token scores, as Engine.generate.  ``on_tokens``: the streaming callback of
+        Engine.generate (columns of the whole batch, in sample order)."""
         eng, dev = self.eng, self.eng.device
         samples = self.preprocess(samples)           # uint8 images -> the towers' input tensors, on the device
         feats, img_off, region_tokens, _ = self.encode(samples)
@@ -206,7 +207,7 @@ class Fo1Pipeline:
         self._mark("splice")
         out = eng.generate(embeds, pos, lens, deltas, max_new_tokens, stop_ids, pad_id, want_prefill_logits=want_prefill_logits,
                            early_exit_interval=early_exit_interval, sampling=sampling, want_logprobs=want_logprobs, want_scores=want_scores,
-                           want_logits=want_logits, raw_rows=raw_rows)
+                           want_logits=want_logits, raw_rows=raw_rows, on_tokens=on_tokens)
         self._mark("llm_prefill_decode")
         out["prompt_lens"] = lens
         return out

@@ -155,15 +155,21 @@ class Fo1ForCausalLM:
         sample, stop, samp = self._sample(inputs, images, images_aux, image_grid_thws, bbox_list, do_sample, temperature, stopping_criteria,
                                           top_p, top_k, **kwargs)
         pad = pad_token_id if pad_token_id is not None else (stop[0] if stop else 0)
-        out = self.pipeline.generate([sample], int(max_new_tokens), sorted(set(stop)), pad_id=int(pad), early_exit_interval=8,
-                                     sampling=self._sampling([samp]), want_scores=bool(want and want[0]), want_logits=bool(want and want[1]))
-        res = self._result(out, 0, inputs, want)
-        new = (res if want is None else res.sequences)[0, inputs.shape[1]:]
+        on_tokens = None
         if streamer is not None:
-            # the whole completion is handed over at once (the decode loop is device-resident: no per-token host sync);
-            # a streamer error is the caller's to see, as in HF's generate
+            # HF's order: the prompt once, then each generated token (the stop token included, pad not) as the device publishes
+            # it, then end().  The decode loop stays device-resident: the engine reads the published columns from pinned host
+            # memory without a per-token sync.  A streamer error stops the device and propagates, as in HF's generate.
             streamer.put(inputs.cpu())
-            streamer.put(new.cpu())
+
+            def on_tokens(lo, hi, toks, lens):
+                for t in range(lo, min(hi, int(lens[0]))):
+                    streamer.put(torch.tensor([int(toks[0, t - lo])], dtype=torch.long))
+        out = self.pipeline.generate([sample], int(max_new_tokens), sorted(set(stop)), pad_id=int(pad), early_exit_interval=8,
+                                     sampling=self._sampling([samp]), want_scores=bool(want and want[0]), want_logits=bool(want and want[1]),
+                                     on_tokens=on_tokens)
+        res = self._result(out, 0, inputs, want)
+        if streamer is not None:
             streamer.end()
         return res
 
