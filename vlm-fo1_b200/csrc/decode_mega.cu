@@ -371,7 +371,7 @@ __device__ __forceinline__ void mg_attention_phase(const MegaArgs& a, uint8_t* s
   for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
     const int sp = item % a.n_splits, kvh = (item / a.n_splits) % a.kv_heads, b = item / (a.n_splits * a.kv_heads);
     MG_ASTAMP(0);
-    const int n = a.cache_len[b] + 1;
+    const int n = a.sink.st.cache_len[b] + 1;
     const int chunk = ((n + a.n_splits - 1) / a.n_splits + 15) & ~15;
     const int t_begin = sp * chunk, t_end = min(n, t_begin + chunk);
     const float* cosv = a.cs + (long long)b * (HD / 2);
@@ -589,12 +589,12 @@ __device__ __forceinline__ void mg_attention_phase(const MegaArgs& a, uint8_t* s
 }
 
 // ----------------------------------------------------------------------------------------------------------- kernel
-// SAMPLE = false: the greedy loop.  SAMPLE = true: the head stores its logits, CTA b < B draws sequence b's token with the
-// row routine of sampling.cuh (one more grid barrier per step), CTA 0 records the drawn tokens.  SCORE (with SAMPLE): CTA b also
-// scores row b in the same phase -- one more pass over the row for Z_kept, the log-probability and the optional scores / logits
-// rows (a greedy call runs here with top_k = 1, which draws the arg-max).  STREAM: CTA 0 also mirrors each recorded column into the
-// caller's mapped host buffers and publishes it (a.stream), and honours the host's cancel flag.
-template <int MT, bool SAMPLE, bool SCORE = false, bool STREAM = false>
+// MODE (DecodeMode) DEC_GREEDY: the greedy loop.  DEC_SAMPLED: the head stores its logits, CTA b < B draws sequence b's token with
+// the row routine of sampling.cuh (one more grid barrier per step), CTA 0 records the drawn tokens.  DEC_SCORED: CTA b also scores
+// row b in the same phase -- one more pass over the row for Z_kept, the log-probability and the optional scores / logits rows (a
+// scored greedy call runs here with top_k = 1, which draws the arg-max).  STREAM: CTA 0 also mirrors each recorded column into the
+// caller's mapped host buffers and publishes it (a.sink.stream), and honours the host's cancel flag.
+template <int MT, int MODE, bool STREAM>
 __global__ void __launch_bounds__(kMgThreads, 1) decode_mega_kernel(const MegaArgs a) {
   using Lay = MgLay<MT>;
   extern __shared__ __align__(128) uint8_t mg_smem[];
@@ -623,7 +623,7 @@ __global__ void __launch_bounds__(kMgThreads, 1) decode_mega_kernel(const MegaAr
       if (threadIdx.x < 32) ssq_x[blockIdx.x * 32 + threadIdx.x] = 0.f;
       __syncthreads();
       for (int b = blockIdx.x; b < a.B; b += gridDim.x) {
-        const bf16* src = a.embed + (long long)a.cur_tok[b] * a.H;
+        const bf16* src = a.embed + (long long)a.sink.st.cur_tok[b] * a.H;
         float sq = 0.f;
         for (int c = threadIdx.x * 8; c < a.H; c += kMgThreads * 8) {
           const uint4 v = *reinterpret_cast<const uint4*>(src + c);
@@ -644,7 +644,7 @@ __global__ void __launch_bounds__(kMgThreads, 1) decode_mega_kernel(const MegaAr
         for (int j = threadIdx.x; j < half; j += kMgThreads) {
           const int axis = j < a.sec_t ? 0 : (j < a.sec_t + a.sec_h ? 1 : 2);
           const float inv = 1.0f / powf(a.theta, (float)(2 * j) / (float)a.hd);
-          const float ang = (float)a.pos3[axis * a.B + b] * inv;
+          const float ang = (float)a.sink.st.pos3[axis * a.B + b] * inv;
           a.cs[(long long)b * half + j] = cosf(ang);
           a.cs[(long long)a.B * half + (long long)b * half + j] = sinf(ang);
         }
@@ -695,10 +695,10 @@ __global__ void __launch_bounds__(kMgThreads, 1) decode_mega_kernel(const MegaAr
       ring.fill(work, lane);
       MG_STAMP(slot, 0); mg_grid_sync(a.bar, gen); MG_STAMP(slot, 1); ++slot;
     }
-    // ---- LM head: running arg-max of this CTA's columns (SAMPLE: the logits rows) ----
+    // ---- LM head: running arg-max of this CTA's columns (sampled or scored: the logits rows) ----
     [[maybe_unused]] float best_val = -INFINITY;
     [[maybe_unused]] int best_idx = 0x7fffffff;
-    if constexpr (SAMPLE) {
+    if constexpr (MODE != DEC_GREEDY) {
       MgEpi e;
       e.out = nullptr; e.ldo = 0; e.bias = nullptr; e.resid = nullptr; e.ssq_slot = nullptr; e.scale_rows = true;
       mg_row_scale(a, mg_smem, ssq_x);
@@ -710,19 +710,19 @@ __global__ void __launch_bounds__(kMgThreads, 1) decode_mega_kernel(const MegaAr
         mg_wait<0>();
         SampleSmem<kMgThreads>& sm = *reinterpret_cast<SampleSmem<kMgThreads>*>(mg_smem);
         const int b = blockIdx.x;
-        if constexpr (SCORE) {
+        if constexpr (MODE == DEC_SCORED) {
           const float* row = a.logits + (long long)b * a.V;
-          const int step = __ldcg(a.step);
+          const int step = __ldcg(a.sink.st.step);
           const int tok = sample_row<kMgThreads, SMP_DRAW_KEPT>(row, a.V, a.samp[b], step, sm);
           if (threadIdx.x == 0) a.samp_tok[b] = tok;
-          if (step < a.max_new && !__ldcg(a.finished + b)) {       // past the sequence's stop nothing is recorded
+          if (step < a.sink.max_new && !__ldcg(a.sink.st.finished + b)) {       // past the sequence's stop nothing is recorded
             const long long o = ((long long)step * a.B + b) * a.V;
             const float lp = score_row<kMgThreads>(row, a.V, a.samp[b].temperature, tok, sm, a.sc_scores ? a.sc_scores + o : nullptr,
                                                    a.sc_logits ? a.sc_logits + o : nullptr);
-            if (threadIdx.x == 0 && a.sc_logprobs != nullptr) a.sc_logprobs[(long long)b * a.max_new + step] = lp;
+            if (threadIdx.x == 0 && a.sc_logprobs != nullptr) a.sc_logprobs[(long long)b * a.sink.max_new + step] = lp;
           }
         } else {
-          const int tok = sample_row<kMgThreads>(a.logits + (long long)b * a.V, a.V, a.samp[b], __ldcg(a.step), sm);
+          const int tok = sample_row<kMgThreads>(a.logits + (long long)b * a.V, a.V, a.samp[b], __ldcg(a.sink.st.step), sm);
           if (threadIdx.x == 0) a.samp_tok[b] = tok;
         }
       }
@@ -742,25 +742,14 @@ __global__ void __launch_bounds__(kMgThreads, 1) decode_mega_kernel(const MegaAr
       if ((threadIdx.x & 7) == 0) { a.amax_val[blockIdx.x * 32 + row] = best_val; a.amax_idx[blockIdx.x * 32 + row] = best_idx; }
     }
     MG_STAMP(slot, 0); mg_grid_sync(a.bar, gen); MG_STAMP(slot, 1); ++slot;
-    // ---- CTA 0: merge the arg-max slots, record the token, stop test, advance the loop state (decode_update_kernel) ----
+    // ---- CTA 0: merge the arg-max slots (a warp per sequence), then record the column as decode_update_kernel does ----
     if (blockIdx.x == 0) {
-      const int step = *a.step;
-      // STREAM: publish only while a sequence is active (nothing after `done`); the host's cancel flag is read once per step
-      [[maybe_unused]] bool publish = false, cancel = false;
-      if constexpr (STREAM) {
-        __shared__ int s_stream[2];
-        if (threadIdx.x == 0) {
-          s_stream[0] = __ldcg(a.n_active) > 0 && step < a.max_new;
-          s_stream[1] = stream_cancel_requested(a.stream.cancel);
-        }
-        __syncthreads();
-        publish = s_stream[0] != 0;
-        cancel = publish && s_stream[1] != 0;
-      }
-      __syncthreads();
+      const int step = *a.sink.st.step;
+      bool publish = false, cancel = false;
+      column_prologue<STREAM>(a.sink, step, publish, cancel);
       for (int b = warp; b < a.B; b += kMgWarps) {
         [[maybe_unused]] float bv = -INFINITY; int bi = 0x7fffffff;
-        if constexpr (SAMPLE) {
+        if constexpr (MODE != DEC_GREEDY) {
           bi = __ldcg(a.samp_tok + b);
         } else {
           for (int c = lane; c < (int)gridDim.x; c += 32) {
@@ -774,42 +763,12 @@ __global__ void __launch_bounds__(kMgThreads, 1) decode_mega_kernel(const MegaAr
             if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
           }
         }
-        if (lane == 0) {
-          const int tok = bi;
-          if (step < a.max_new) {
-            if (!a.finished[b]) {
-              a.out_tokens[(long long)b * a.max_new + step] = tok;
-              a.out_lens[b] = step + 1;
-              bool stop = false;
-              for (int i = 0; i < a.n_stop; ++i) stop |= (tok == a.stop_ids[i]);
-              if constexpr (STREAM) stop |= cancel;                  // a cancelled sequence ends after this column
-              if (stop) { a.finished[b] = 1; atomicSub(a.n_active, 1); }
-              if constexpr (STREAM) {
-                if (publish) { a.stream.tokens[(long long)b * a.max_new + step] = tok; a.stream.lens[b] = step + 1; }
-              }
-            } else {
-              a.out_tokens[(long long)b * a.max_new + step] = a.pad_id;
-              if constexpr (STREAM) {
-                if (publish) a.stream.tokens[(long long)b * a.max_new + step] = a.pad_id;
-              }
-            }
-          }
-          a.cur_tok[b] = tok;
-          a.cache_len[b] += 1;
-          a.pos3[b] += 1; a.pos3[a.B + b] += 1; a.pos3[2 * a.B + b] += 1;
-        }
+        if (lane == 0) record_token<STREAM>(a.sink, a.B, b, step, bi, true, publish, cancel);
       }
-      __syncthreads();
-      if (threadIdx.x == 0) *a.step = step + 1;
-      if constexpr (STREAM) {
-        if (threadIdx.x == 0 && publish) {
-          const bool done = cancel || __ldcg(a.n_active) <= 0 || step + 1 >= a.max_new;
-          stream_publish(a.stream.progress, (step + 1) | (done ? FO1_STREAM_DONE : 0));     // (after the bar.sync above: covers every warp's mirror writes)
-        }
-      }
+      column_epilogue<STREAM>(a.sink, step, publish, cancel);
     }
     MG_STAMP(slot, 0); mg_grid_sync(a.bar, gen); MG_STAMP(slot, 1); ++slot;
-    if (__ldcg(a.n_active) <= 0) break;           // every sequence has emitted a stop id (the tail of out_tokens is pad already)
+    if (__ldcg(a.sink.st.n_active) <= 0) break;           // every sequence has emitted a stop id (the tail of out_tokens is pad already)
   }
   mg_wait<0>();
 }
@@ -818,35 +777,24 @@ __global__ void __launch_bounds__(kMgThreads, 1) decode_mega_kernel(const MegaAr
 
 namespace fo1 {
 
-// the streamed instantiations, [MT - 1][0 greedy | 1 sampled | 2 scored]
-static void* const kMgStreamed[2][3] = {
-    {reinterpret_cast<void*>(decode_mega_kernel<1, false, false, true>), reinterpret_cast<void*>(decode_mega_kernel<1, true, false, true>),
-     reinterpret_cast<void*>(decode_mega_kernel<1, true, true, true>)},
-    {reinterpret_cast<void*>(decode_mega_kernel<2, false, false, true>), reinterpret_cast<void*>(decode_mega_kernel<2, true, false, true>),
-     reinterpret_cast<void*>(decode_mega_kernel<2, true, true, true>)}};
+// every instantiation, [MT - 1][DecodeMode][STREAM]
+#define MG_KERNELS(MT, MODE) {reinterpret_cast<void*>(decode_mega_kernel<MT, MODE, false>), reinterpret_cast<void*>(decode_mega_kernel<MT, MODE, true>)}
+static void* const kMgKernels[2][3][2] = {{MG_KERNELS(1, DEC_GREEDY), MG_KERNELS(1, DEC_SAMPLED), MG_KERNELS(1, DEC_SCORED)},
+                                          {MG_KERNELS(2, DEC_GREEDY), MG_KERNELS(2, DEC_SAMPLED), MG_KERNELS(2, DEC_SCORED)}};
+#undef MG_KERNELS
 
 int decode_mega_grid() {
   static int grid = -1;
   if (grid < 0) {
     grid = 0;
     int dev = 0, coop = 0, per_sm = 0;
-    bool streamed_ok = true;
-    for (int mt = 0; mt < 2; ++mt)
-      for (int k = 0; k < 3; ++k) {
-        streamed_ok = streamed_ok && cudaFuncSetAttribute(kMgStreamed[mt][k], cudaFuncAttributeMaxDynamicSharedMemorySize, kMgSmemBytes) == cudaSuccess;
-        streamed_ok = streamed_ok && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kMgStreamed[mt][k], kMgThreads, kMgSmemBytes) == cudaSuccess &&
-                      per_sm >= 1;
-      }
-    if (streamed_ok && cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev) == cudaSuccess && coop &&
-        cudaFuncSetAttribute(decode_mega_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMgSmemBytes) == cudaSuccess &&
-        cudaFuncSetAttribute(decode_mega_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMgSmemBytes) == cudaSuccess &&
-        cudaFuncSetAttribute(decode_mega_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMgSmemBytes) == cudaSuccess &&
-        cudaFuncSetAttribute(decode_mega_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMgSmemBytes) == cudaSuccess &&
-        cudaFuncSetAttribute(decode_mega_kernel<1, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMgSmemBytes) == cudaSuccess &&
-        cudaFuncSetAttribute(decode_mega_kernel<2, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMgSmemBytes) == cudaSuccess &&
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decode_mega_kernel<2, false>, kMgThreads, kMgSmemBytes) == cudaSuccess && per_sm >= 1 &&
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decode_mega_kernel<2, true>, kMgThreads, kMgSmemBytes) == cudaSuccess && per_sm >= 1 &&
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decode_mega_kernel<2, true, true>, kMgThreads, kMgSmemBytes) == cudaSuccess && per_sm >= 1)
+    bool ok = cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev) == cudaSuccess && coop;
+    for (const auto& per_mt : kMgKernels)
+      for (const auto& per_mode : per_mt)
+        for (void* fn : per_mode)
+          ok = ok && cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kMgSmemBytes) == cudaSuccess &&
+               cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kMgThreads, kMgSmemBytes) == cudaSuccess && per_sm >= 1;
+    if (ok)
       grid = device_sm_count();
     else
       fprintf(stderr, "[fo1] decode_mega: cooperative launch with %d B of shared memory is not available (%s); using the per-kernel decode path\n",
@@ -856,28 +804,85 @@ int decode_mega_grid() {
   return grid;
 }
 
-// One cooperative launch for the whole greedy loop.  `a.bar` and `a.att_count` must be zero (the caller memsets them on `s`).
-int decode_mega_run(const MegaArgs& a, cudaStream_t s) {
+// FO1_MEGA_PROF: where the first decode iteration spent its time, from its MG_STAMP / MG_ASTAMP slots, on stderr (after a synchronise)
+static int mg_prof_report(const MegaArgs& a, int grid, cudaStream_t s) {
+  const int prof_slots = a.prof_slots;
+  std::vector<unsigned long long> h((size_t)grid * prof_slots * 2);
+  FO1_CUDA(cudaStreamSynchronize(s));
+  FO1_CUDA(cudaMemcpy(h.data(), a.prof, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+  cudaFree(a.prof);
+  // per slot: the last CTA to enter the barrier ends the phase; release = when CTA 0 leaves.  work = last_enter - previous release,
+  // skew = last_enter - first_enter, barrier = release - last_enter
+  const char* names[5] = {"qkv", "attn", "oproj", "gateup", "down"};
+  double tot[5][3] = {{0}}, misc = 0;
+  unsigned long long prev_release = 0;
+  for (int sl = 0; sl < prof_slots - 8; ++sl) {
+    unsigned long long first = ~0ull, last = 0, rel = 0;
+    for (int cta = 0; cta < grid; ++cta) {
+      const unsigned long long e = h[((size_t)cta * prof_slots + sl) * 2], l = h[((size_t)cta * prof_slots + sl) * 2 + 1];
+      if (e < first) first = e;
+      if (e > last) last = e;
+      if (l > rel) rel = l;
+    }
+    if (sl >= 1 && sl <= 5 * a.layers) {
+      const int ph = (sl - 1) % 5;
+      tot[ph][0] += (double)(last - prev_release); tot[ph][1] += (double)(last - first); tot[ph][2] += (double)(rel - last);
+    } else if (sl > 0) misc += (double)(rel - prev_release);
+    prev_release = rel;
+  }
+  fprintf(stderr, "[decode_mega profile, first iteration, B=%d, %d CTAs] per layer (us): ", a.B, grid);
+  for (int ph = 0; ph < 5; ++ph)
+    fprintf(stderr, "%s work %.1f (skew %.1f) barrier %.1f | ", names[ph], tot[ph][0] / a.layers / 1e3, tot[ph][1] / a.layers / 1e3,
+            tot[ph][2] / a.layers / 1e3);
+  fprintf(stderr, "head+update %.1f us\n", misc / 1e3);
+  {   // distribution over CTAs of the time spent in layer 1's attention phase (slot 7: enter of the barrier after it; slot 6: leave before it)
+    std::vector<std::pair<double, int>> dur;
+    for (int cta = 0; cta < grid; ++cta)
+      dur.push_back({(double)(h[((size_t)cta * prof_slots + 7) * 2] - h[((size_t)cta * prof_slots + 6) * 2 + 1]) / 1e3, cta});
+    std::sort(dur.begin(), dur.end());
+    fprintf(stderr, "[decode_mega profile] attention phase per CTA (us): min %.1f p25 %.1f median %.1f p75 %.1f max %.1f; slowest CTAs:", dur[0].first,
+            dur[grid / 4].first, dur[grid / 2].first, dur[3 * grid / 4].first, dur.back().first);
+    for (int k = 0; k < 6; ++k) fprintf(stderr, " %d(%.1f)", dur[grid - 1 - k].second, dur[grid - 1 - k].first);
+    fprintf(stderr, "\n");
+  }
+  fprintf(stderr, "[decode_mega profile] attention item of CTA 0, layer 1 (us since its start): ");
+  const unsigned long long a0 = h[((size_t)0 * prof_slots + prof_slots - 8) * 2];
+  const char* an[8] = {"start", "append+fence", "q rotated", "tiles done", "warps synced", "partials written", "fence+sync", "combined"};
+  for (int k = 0; k < 8; ++k) fprintf(stderr, "%s %.1f | ", an[k], (double)(h[((size_t)0 * prof_slots + prof_slots - 8 + k) * 2] - a0) / 1e3);
+  fprintf(stderr, "\n");
+  return FO1_OK;
+}
+
+// One cooperative launch for the whole decode loop.  `a.bar` and `a.att_count` must be zero (the caller memsets them on `s`).
+int decode_mega_run(MegaArgs a, DecodeMode mode, cudaStream_t s) {
   const int grid = decode_mega_grid();
   FO1_CHECK_ARG(grid > 0, "decode_mega: cooperative launch of a %d-byte-smem CTA per SM is not available on this device", kMgSmemBytes);
   FO1_CHECK_ARG(a.B >= 1 && a.B <= kMgRows && a.hd == 128 && a.q_heads % a.kv_heads == 0 && a.q_heads / a.kv_heads <= 8, "decode_mega: unsupported shape");
   FO1_CHECK_ARG(a.H % kMgChunkK == 0 && a.QD % kMgChunkK == 0 && a.H <= kMgAK && a.QD <= kMgAK && a.I % kMgChunkK == 0 && (a.QD + 2 * a.KD) % kMgTileN == 0 &&
                 a.H % kMgTileN == 0 && (2 * a.I) % kMgTileN == 0 && a.V % kMgTileN == 0 && (a.H / kMgChunkK) >= kMgWarps && (a.QD / kMgChunkK) >= kMgWarps,
                 "decode_mega: widths must be multiples of the 16 x 64 tile (H %d, QD %d, I %d, V %d)", a.H, a.QD, a.I, a.V);
-  MegaArgs args = a;
-  void* params[] = {&args};
-  ProfScope prof("decode_mega", 0.0, 0.0, s);
-  FO1_CHECK_ARG(a.samp == nullptr || (a.logits != nullptr && a.samp_tok != nullptr && (a.V & 1) == 0), "decode_mega: sampling buffers missing");
-  const bool scored = a.sc_logprobs != nullptr || a.sc_scores != nullptr || a.sc_logits != nullptr;
-  FO1_CHECK_ARG(!scored || a.samp != nullptr, "decode_mega: scoring needs the per-row sampling parameters");
-  void* fn = scored ? (a.B <= 16 ? reinterpret_cast<void*>(decode_mega_kernel<1, true, true>) : reinterpret_cast<void*>(decode_mega_kernel<2, true, true>))
-           : a.samp != nullptr ? (a.B <= 16 ? reinterpret_cast<void*>(decode_mega_kernel<1, true>) : reinterpret_cast<void*>(decode_mega_kernel<2, true>))
-                               : (a.B <= 16 ? reinterpret_cast<void*>(decode_mega_kernel<1, false>) : reinterpret_cast<void*>(decode_mega_kernel<2, false>));
-  FO1_CHECK_ARG(a.stream.progress == nullptr || (a.stream.tokens != nullptr && a.stream.lens != nullptr), "decode_mega: stream buffers missing");
-  if (a.stream.progress != nullptr) fn = kMgStreamed[a.B <= 16 ? 0 : 1][scored ? 2 : a.samp != nullptr ? 1 : 0];
-  FO1_CUDA(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(kMgThreads), params, kMgSmemBytes, s));
-  count_launch();
-  return FO1_OK;
+  FO1_CHECK_ARG(mode != DEC_SCORED || a.samp != nullptr, "decode_mega: scoring needs the per-row sampling parameters");
+  FO1_CHECK_ARG(mode == DEC_GREEDY || (a.samp != nullptr && a.logits != nullptr && a.samp_tok != nullptr && (a.V & 1) == 0),
+                "decode_mega: sampling buffers missing");
+  const StreamArgs& sa = a.sink.stream;
+  FO1_CHECK_ARG(sa.progress == nullptr || (sa.tokens != nullptr && sa.lens != nullptr), "decode_mega: stream buffers missing");
+  const bool prof = getenv("FO1_MEGA_PROF") != nullptr;
+  if (prof) {
+    // per CTA: one slot per grid barrier (the embedding, 5 per layer, the sampling barrier of the sampled / scored modes, the
+    // head, the record), then the 8 sub-stamps of one attention item (CTA 0, layer 1)
+    a.prof_slots = 5 * a.layers + 3 + (mode != DEC_GREEDY ? 1 : 0) + 8;
+    const size_t bytes = (size_t)grid * a.prof_slots * 2 * sizeof(unsigned long long);
+    FO1_CUDA(cudaMalloc(reinterpret_cast<void**>(&a.prof), bytes));
+    FO1_CUDA(cudaMemsetAsync(a.prof, 0, bytes, s));
+  }
+  {
+    void* params[] = {&a};
+    ProfScope ps("decode_mega", 0.0, 0.0, s);
+    FO1_CUDA(cudaLaunchCooperativeKernel(kMgKernels[a.B <= 16 ? 0 : 1][mode][sa.progress != nullptr], dim3(grid), dim3(kMgThreads), params,
+                                         kMgSmemBytes, s));
+    count_launch();
+  }
+  return prof ? mg_prof_report(a, grid, s) : FO1_OK;
 }
 
 }  // namespace fo1

@@ -12,6 +12,7 @@
 // prompt position only.
 #include <algorithm>
 
+#include "decode_loop.cuh"
 #include "decode_mega.cuh"
 
 namespace fo1 {
@@ -296,17 +297,6 @@ __global__ void __launch_bounds__(1024) argmax_kernel(const float* __restrict__ 
   }
 }
 
-struct DecodeState {
-  int* cache_len;  // [B] K/V entries in the cache
-  int* pos3;       // [3][B] M-RoPE position of the next input token (all axes equal after the prompt, :1848-1860)
-  int* cur_tok;    // [B] token to feed next
-  int* new_tok;    // [B] argmax output
-  int* finished;   // [B]
-  int* n_active;   // [1] sequences still running
-  int* step;       // [1] index of the next output column
-  int* stop_ids;   // [n_stop]
-};
-
 // after the prefill: lengths, positions, first token
 __global__ void decode_init_kernel(DecodeState st, const int* __restrict__ seq_lens, const int* __restrict__ deltas, int B) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
@@ -317,63 +307,17 @@ __global__ void decode_init_kernel(DecodeState st, const int* __restrict__ seq_l
   st.pos3[b] = p; st.pos3[B + b] = p; st.pos3[2 * B + b] = p;
   st.finished[b] = 0;
 }
-// record the sampled token, test the stop ids, advance the loop state.  ONE block; the output column is the
-// device-resident step counter, so the launch is identical every iteration (CUDA-graph replayable).  STREAM: the column is also
-// mirrored into the caller's mapped host buffers and published (the same protocol as decode_mega_kernel's record block); steps after
-// `done` publish nothing, and the host's cancel flag ends every sequence after the column recorded.
+// record the column of new_tok (decode_loop.cuh).  ONE block; the output column is the device-resident step counter, so the launch is
+// identical every iteration (CUDA-graph replayable).
 template <bool STREAM>
-__global__ void __launch_bounds__(1024) decode_update_kernel(DecodeState st, int n_stop, int pad_id, int max_new,
-                                                             int* __restrict__ out_tokens, int* __restrict__ out_lens, int B,
-                                                             int advance_cache, StreamArgs sa) {
+__global__ void __launch_bounds__(1024) decode_update_kernel(ColumnSink k, int B, int advance_cache) {
   griddep_launch();
   griddep_wait();
-  const int step = *st.step;
-  [[maybe_unused]] bool publish = false, cancel = false;
-  if constexpr (STREAM) {
-    __shared__ int s_stream[2];
-    if (threadIdx.x == 0) {
-      s_stream[0] = __ldcg(st.n_active) > 0 && step < max_new;
-      s_stream[1] = stream_cancel_requested(sa.cancel);
-    }
-    __syncthreads();
-    publish = s_stream[0] != 0;
-    cancel = publish && s_stream[1] != 0;
-  }
-  __syncthreads();
-  for (int b = threadIdx.x; b < B; b += blockDim.x) {
-    const int tok = st.new_tok[b];
-    if (step < max_new) {
-      if (!st.finished[b]) {
-        out_tokens[(long long)b * max_new + step] = tok;
-        out_lens[b] = step + 1;
-        bool stop = false;
-        for (int i = 0; i < n_stop; ++i) stop |= (tok == st.stop_ids[i]);
-        if constexpr (STREAM) stop |= cancel;
-        if (stop) { st.finished[b] = 1; atomicSub(st.n_active, 1); }
-        if constexpr (STREAM) {
-          if (publish) { sa.tokens[(long long)b * max_new + step] = tok; sa.lens[b] = step + 1; }
-        }
-      } else {
-        out_tokens[(long long)b * max_new + step] = pad_id;
-        if constexpr (STREAM) {
-          if (publish) sa.tokens[(long long)b * max_new + step] = pad_id;
-        }
-      }
-    }
-    st.cur_tok[b] = tok;
-    if (advance_cache) {
-      st.cache_len[b] += 1;
-      st.pos3[b] += 1; st.pos3[B + b] += 1; st.pos3[2 * B + b] += 1;
-    }
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) *st.step = step + 1;
-  if constexpr (STREAM) {
-    if (threadIdx.x == 0 && publish) {
-      const bool done = cancel || __ldcg(st.n_active) <= 0 || step + 1 >= max_new;
-      stream_publish(sa.progress, (step + 1) | (done ? FO1_STREAM_DONE : 0));
-    }
-  }
+  const int step = *k.st.step;
+  bool publish = false, cancel = false;
+  column_prologue<STREAM>(k, step, publish, cancel);
+  for (int b = threadIdx.x; b < B; b += blockDim.x) record_token<STREAM>(k, B, b, step, k.st.new_tok[b], advance_cache, publish, cancel);
+  column_epilogue<STREAM>(k, step, publish, cancel);
 }
 __global__ void fill_int_kernel(int* p, int v, long long n) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) p[i] = v;
@@ -527,8 +471,39 @@ static int llm_layer(Model* m, int li, const bf16* x_in, bf16* x_out, const Laye
   return FO1_OK;
 }
 
-static int llm_generate_impl(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, const fo1_score_desc* sc, cudaStream_t s, bool dry,
-                             const DecodeState& st, const StreamArgs& sa, const int32_t* h_progress) {
+// the buffers both decode paths use after the prefill, carved from the arena (the dry run sizes it)
+struct DecodeBufs {
+  int mega_grid;                  // CTAs of the persistent kernel (0: the per-kernel path)
+  LayerBuf layer;
+  bf16 *xa, *xb, *lastn;
+  float *cs_dec, *logits, *mg_ssq, *mg_amax_v;
+  int *mg_amax_i, *mg_sync, *samp_tok;
+  SampleRowParams* samp;
+};
+
+// the tokens of the current output column into new_tok (scored: also the column's scores), then their recording; every kernel reads
+// the column from *st.step, as the captured decode step does.  `advance`: the column came from a decode step (not the prefill)
+static int decode_column(DecodeMode mode, const DecodeBufs& g, const ColumnSink& k, const fo1_score_desc* sc, int B, int V, int advance,
+                         cudaStream_t s) {
+  const DecodeState& st = k.st;
+  if (mode == DEC_SCORED) {
+    FO1_TRY(score_rows(g.logits, V, B, V, g.samp, st.step, st.new_tok, true, st.finished, k.max_new, sc->logprobs, k.max_new, sc->scores,
+                       sc->logits, V, s));
+  } else if (mode == DEC_SAMPLED) {
+    FO1_TRY(sample_rows(g.logits, V, B, V, g.samp, st.step, 0, st.new_tok, s));       // the Philox step is read from *st.step
+  } else {
+    launch_k(argmax_kernel, dim3(B), dim3(1024), 0, s, g.logits, V, st.new_tok);
+    FO1_LAUNCH_CHECK();
+  }
+  const int threads = std::min(1024, std::max(32, (B + 31) / 32 * 32));
+  launch_k(k.stream.progress != nullptr ? decode_update_kernel<true> : decode_update_kernel<false>, dim3(1), dim3(threads), 0, s, k, B, advance);
+  FO1_LAUNCH_CHECK();
+  return FO1_OK;
+}
+
+// buffer plan, integer tables and the prefill; then (unless `dry`, the pass that sizes the arena) the decode state and column 0
+static int llm_prefill(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, const fo1_score_desc* sc, DecodeMode mode,
+                       const ColumnSink& k, cudaStream_t s, bool dry, DecodeBufs& g) {
   const fo1_model_config& c = m->cfg;
   Arena& A = m->arena;
   const int B = d->n_seqs, H = c.llm_hidden, hd = c.llm_head_dim, V = c.llm_vocab;
@@ -539,22 +514,23 @@ static int llm_generate_impl(Model* m, fo1_generate_desc* d, const fo1_sampling_
   for (int b = 0; b < B; ++b) { T += d->seq_lens[b]; max_len = std::max(max_len, d->seq_lens[b]); }
   const int R = (int)std::max<long long>(T, B);
 
-  LayerBuf buf;
-  bf16* xa = A.alloc<bf16>((size_t)R * H);
-  bf16* xb = A.alloc<bf16>((size_t)R * H);
+  g = DecodeBufs();
+  LayerBuf& buf = g.layer;
+  g.xa = A.alloc<bf16>((size_t)R * H);
+  g.xb = A.alloc<bf16>((size_t)R * H);
   buf.xn = A.alloc<bf16>((size_t)R * H);
   buf.qkv = A.alloc<bf16>((size_t)R * ldq);
   buf.att = A.alloc<bf16>((size_t)R * QD);
   buf.x_mid = A.alloc<bf16>((size_t)R * H);
   buf.h = A.alloc<bf16>((size_t)R * Ip);
   float* cs_pre = A.alloc<float>((size_t)R * hd);
-  float* cs_dec = A.alloc<float>((size_t)B * hd);
+  g.cs_dec = A.alloc<float>((size_t)B * hd);
   buf.dec_part = A.alloc<float>((size_t)B * c.llm_heads * kDecSplits * (128 + 4));
   buf.rowseg = A.alloc<int>((size_t)R * 2);
   for (int b = 0; b < B; ++b) buf.attn_flops += 2.0 * (double)d->seq_lens[b] * d->seq_lens[b] * QD;   // causal: half of 4 L^2 d
   bf16* last = A.alloc<bf16>((size_t)B * H);
-  bf16* lastn = A.alloc<bf16>((size_t)B * H);
-  float* logits = A.alloc<float>((size_t)B * V);
+  g.lastn = A.alloc<bf16>((size_t)B * H);
+  g.logits = A.alloc<float>((size_t)B * V);
   bf16* alln = d->all_logits ? A.alloc<bf16>((size_t)T * H) : nullptr;
   int* d_lens = A.alloc<int>(B);
   int* d_deltas = A.alloc<int>(B);
@@ -563,16 +539,14 @@ static int llm_generate_impl(Model* m, fo1_generate_desc* d, const fo1_sampling_
   // FO1_MEGA_MAX_B lowers the threshold, FO1_NO_MEGA disables the kernel.
   int mega_max_b = 32;
   if (const char* e = getenv("FO1_MEGA_MAX_B")) mega_max_b = std::max(0, std::min(32, atoi(e)));
-  const int mega_grid = (m->llm.mega_ok && B <= mega_max_b && getenv("FO1_NO_MEGA") == nullptr) ? decode_mega_grid() : 0;
-  float* mg_ssq = A.alloc<float>((size_t)2 * std::max(mega_grid, 1) * 32);
-  float* mg_amax_v = A.alloc<float>((size_t)std::max(mega_grid, 1) * 32);
-  int* mg_amax_i = A.alloc<int>((size_t)std::max(mega_grid, 1) * 32);
-  int* mg_sync = A.alloc<int>((size_t)B * c.llm_kv_heads + 8);      // [0]: grid barrier counter, [8..]: attention arrival counters
-  // sampled or scored decoding: the per-sequence parameters on the device and the persistent kernel's per-row token slots.  A
-  // scored greedy call samples with top_k 1 (bit-identical to greedy) so that both paths score in the sampler's per-row pass.
-  const bool per_row = sp != nullptr || sc != nullptr;
-  SampleRowParams* d_samp = per_row ? A.alloc<SampleRowParams>(B) : nullptr;
-  int* d_samp_tok = per_row ? A.alloc<int>(B) : nullptr;
+  g.mega_grid = (m->llm.mega_ok && B <= mega_max_b && getenv("FO1_NO_MEGA") == nullptr) ? decode_mega_grid() : 0;
+  g.mg_ssq = A.alloc<float>((size_t)2 * std::max(g.mega_grid, 1) * 32);
+  g.mg_amax_v = A.alloc<float>((size_t)std::max(g.mega_grid, 1) * 32);
+  g.mg_amax_i = A.alloc<int>((size_t)std::max(g.mega_grid, 1) * 32);
+  g.mg_sync = A.alloc<int>((size_t)B * c.llm_kv_heads + 8);
+  // sampled or scored decoding: the per-sequence parameters and the tokens the persistent kernel's CTA b drew
+  g.samp = mode != DEC_GREEDY ? A.alloc<SampleRowParams>(B) : nullptr;
+  g.samp_tok = mode != DEC_GREEDY ? A.alloc<int>(B) : nullptr;
 
   // ---- integer tables of the packed batch ----
   const int *d_cu = nullptr, *d_row_seq = nullptr, *d_row_t = nullptr, *d_last = nullptr;
@@ -596,11 +570,12 @@ static int llm_generate_impl(Model* m, fo1_generate_desc* d, const fo1_sampling_
     FO1_CUDA(cudaMemcpyAsync(d_lens, d->seq_lens, B * sizeof(int), cudaMemcpyHostToDevice, s));
     if (d->rope_deltas_device != nullptr) FO1_CUDA(cudaMemcpyAsync(d_deltas, d->rope_deltas_device, B * sizeof(int), cudaMemcpyDeviceToDevice, s));
     else FO1_CUDA(cudaMemcpyAsync(d_deltas, d->rope_deltas, B * sizeof(int), cudaMemcpyHostToDevice, s));
-    if (d->n_stop_ids > 0) FO1_CUDA(cudaMemcpyAsync(st.stop_ids, d->stop_ids, d->n_stop_ids * sizeof(int), cudaMemcpyHostToDevice, s));
-    if (per_row) {
+    if (d->n_stop_ids > 0) FO1_CUDA(cudaMemcpyAsync(k.st.stop_ids, d->stop_ids, d->n_stop_ids * sizeof(int), cudaMemcpyHostToDevice, s));
+    if (mode != DEC_GREEDY) {
+      // a scored greedy call samples with top_k 1 (bit-identical to greedy) so that both paths score in the sampler's per-row pass
       std::vector<SampleRowParams> h(B);
       for (int b = 0; b < B; ++b) h[b] = score_row_params(sp, sc ? sc->raw_rows : nullptr, b);
-      FO1_CUDA(cudaMemcpyAsync(d_samp, h.data(), B * sizeof(SampleRowParams), cudaMemcpyHostToDevice, s));
+      FO1_CUDA(cudaMemcpyAsync(g.samp, h.data(), B * sizeof(SampleRowParams), cudaMemcpyHostToDevice, s));
     }
   }
 
@@ -609,7 +584,7 @@ static int llm_generate_impl(Model* m, fo1_generate_desc* d, const fo1_sampling_
   const bf16* x = static_cast<const bf16*>(d->inputs_embeds);
   FO1_RUN(mrope_table(d->position_ids, cs_pre, (int)T, hd, c.mrope_section[0], c.mrope_section[1], c.mrope_section[2], c.rope_theta, s));
   for (int li = 0; li < c.llm_layers; ++li) {
-    bf16* xo = (li & 1) ? xb : xa;
+    bf16* xo = (li & 1) ? g.xb : g.xa;
     FO1_TRY(llm_layer(m, li, x, xo, buf, (int)T, cs_pre, true, d_cu, B, max_len, d_row_seq, d_row_t, nullptr, s, dry));
     x = xo;
   }
@@ -618,148 +593,72 @@ static int llm_generate_impl(Model* m, fo1_generate_desc* d, const fo1_sampling_
     FO1_RUN(linear(alln, H, m->llm.lm_head, H, d->all_logits, V, FO1_F32, (int)T, V, H, nullptr, 0, FO1_EPI_NONE, nullptr, 0, 0, s));
   }
   FO1_RUN(gather_rows_bf16(x, H, d_last, last, H, B, H, s));
-  FO1_RUN(rmsnorm(last, H, m->llm.norm, lastn, H, B, H, c.rms_eps, s));
+  FO1_RUN(rmsnorm(last, H, m->llm.norm, g.lastn, H, B, H, c.rms_eps, s));
   {
     SplitKScope sk(true);       // M = number of sequences: weight streaming
-    FO1_RUN(linear(lastn, H, m->llm.lm_head, H, logits, V, FO1_F32, B, V, H, nullptr, 0, FO1_EPI_NONE, nullptr, 0, 0, s));
+    FO1_RUN(linear(g.lastn, H, m->llm.lm_head, H, g.logits, V, FO1_F32, B, V, H, nullptr, 0, FO1_EPI_NONE, nullptr, 0, 0, s));
   }
   if (dry) return FO1_OK;
-  if (d->prefill_logits) FO1_CUDA(cudaMemcpyAsync(d->prefill_logits, logits, (size_t)B * V * sizeof(float), cudaMemcpyDeviceToDevice, s));
-  decode_init_kernel<<<ceil_div(B, 128), 128, 0, s>>>(st, d_lens, d_deltas, B);
+  if (d->prefill_logits) FO1_CUDA(cudaMemcpyAsync(d->prefill_logits, g.logits, (size_t)B * V * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  decode_init_kernel<<<ceil_div(B, 128), 128, 0, s>>>(k.st, d_lens, d_deltas, B);
   FO1_LAUNCH_CHECK();
   if (d->max_new_tokens <= 0) return FO1_OK;
-  // the token of column 0 (and, scored, its row's scores); score_rows reads the column from *st.step, as the captured step does
-  auto score_step = [&]() {
-    return score_rows(logits, V, B, V, d_samp, st.step, st.new_tok, true, st.finished, d->max_new_tokens, sc->logprobs, d->max_new_tokens,
-                      sc->scores, sc->logits, V, s);
-  };
-  if (sc) {
-    FO1_TRY(score_step());
-  } else if (sp) {
-    FO1_TRY(sample_rows(logits, V, B, V, d_samp, st.step, 0, st.new_tok, s));     // step 0 (decode_init_kernel)
-  } else {
-    argmax_kernel<<<B, 1024, 0, s>>>(logits, V, st.new_tok);
-    FO1_LAUNCH_CHECK();
-  }
-  const int upd_threads = std::min(1024, std::max(32, (B + 31) / 32 * 32));
-  auto* const update_kernel = sa.progress != nullptr ? decode_update_kernel<true> : decode_update_kernel<false>;
-  update_kernel<<<1, upd_threads, 0, s>>>(st, d->n_stop_ids, d->pad_id, d->max_new_tokens, d->out_tokens, d->out_lens, B, 0, sa);
-  FO1_LAUNCH_CHECK();
+  return decode_column(mode, g, k, sc, B, V, 0, s);
+}
 
-  // ---- greedy decode: every step is the SAME launch sequence reading its state from device memory; the first
-  // step runs eagerly (warms every kernel), the second is captured into a CUDA graph that is replayed afterwards ----
+// the rest of the decode loop as ONE cooperative launch of the persistent kernel
+static int decode_persistent(Model* m, fo1_generate_desc* d, const fo1_score_desc* sc, DecodeMode mode, const ColumnSink& k,
+                             const DecodeBufs& g, cudaStream_t s) {
+  const fo1_model_config& c = m->cfg;
+  const int B = d->n_seqs;
+  MegaArgs a;
+  memset(&a, 0, sizeof(a));
+  a.B = B; a.layers = c.llm_layers; a.H = c.llm_hidden; a.hd = c.llm_head_dim; a.QD = c.llm_heads * a.hd; a.KD = c.llm_kv_heads * a.hd;
+  a.q_heads = c.llm_heads; a.kv_heads = c.llm_kv_heads; a.I = c.llm_inter; a.V = c.llm_vocab; a.eps = c.rms_eps; a.theta = c.rope_theta; a.sec_t = c.mrope_section[0]; a.sec_h = c.mrope_section[1];
+  a.layer = static_cast<const MegaLayer*>(m->llm.mega_layers);
+  a.head_w = m->llm.head_dec; a.embed = m->llm.embed;
+  a.kv_layer_stride = (long long)m->kv_batch * m->kv_cap * a.KD;
+  a.kc = static_cast<bf16*>(m->kv_cache); a.vc = a.kc + (size_t)c.llm_layers * a.kv_layer_stride; a.cap = m->kv_cap;
+  a.x = g.xa; a.x_mid = g.layer.x_mid; a.qkv = g.layer.qkv; a.att = g.layer.att; a.h = g.layer.h;
+  a.ssq = g.mg_ssq; a.cs = g.cs_dec; a.att_part = g.layer.dec_part; a.att_count = g.mg_sync + 8;
+  a.amax_val = g.mg_amax_v; a.amax_idx = g.mg_amax_i; a.sink = k;
+  a.logits = g.logits; a.samp = g.samp; a.samp_tok = g.samp_tok;
+  if (sc) { a.sc_logprobs = sc->logprobs; a.sc_scores = sc->scores; a.sc_logits = sc->logits; }
+  a.n_steps = d->max_new_tokens - 1; a.bar = reinterpret_cast<unsigned*>(g.mg_sync);
+  const int pairs = B * c.llm_kv_heads;
+  a.n_splits = std::max(1, std::min(kMgMaxSplits, g.mega_grid / std::max(1, pairs)));
+  FO1_CUDA(cudaMemsetAsync(g.mg_sync, 0, ((size_t)pairs + 8) * sizeof(int), s));
+  FO1_TRY(decode_mega_run(a, mode, s));
+  m->last_decode_path = 1;
+  d->steps_run = d->max_new_tokens - 1;
+  return FO1_OK;
+}
+
+// the rest of the decode loop, per kernel: every step is the SAME launch sequence reading its state from device memory; the first step
+// runs eagerly (warms every kernel), the second is captured into a CUDA graph that is replayed afterwards
+static int decode_per_kernel(Model* m, fo1_generate_desc* d, const fo1_score_desc* sc, DecodeMode mode, const ColumnSink& k,
+                             const DecodeBufs& g, const int32_t* h_progress, cudaStream_t s) {
+  const fo1_model_config& c = m->cfg;
+  const int B = d->n_seqs, H = c.llm_hidden, hd = c.llm_head_dim, V = c.llm_vocab;
   LlmState* ls = static_cast<LlmState*>(m->llm_state);
   // programmatic dependent launch: each kernel of the step starts (prologue, weight prefetch) while its predecessor drains
   const bool use_pdl = getenv("FO1_NO_PDL") == nullptr;
   auto enqueue_step = [&]() -> int {
     PdlScope pdl(use_pdl);
     SplitKScope sk(true);       // M = number of sequences in every GEMM of a decode step
-    launch_k(embed_tokens_kernel, dim3(B), dim3(256), 0, s, st.cur_tok, m->llm.embed, xa, H);
+    launch_k(embed_tokens_kernel, dim3(B), dim3(256), 0, s, k.st.cur_tok, m->llm.embed, g.xa, H);
     FO1_LAUNCH_CHECK();
-    FO1_TRY(mrope_table(st.pos3, cs_dec, B, hd, c.mrope_section[0], c.mrope_section[1], c.mrope_section[2], c.rope_theta, s));
-    const bf16* xin = xa;
+    FO1_TRY(mrope_table(k.st.pos3, g.cs_dec, B, hd, c.mrope_section[0], c.mrope_section[1], c.mrope_section[2], c.rope_theta, s));
+    const bf16* xin = g.xa;
     for (int li = 0; li < c.llm_layers; ++li) {
-      bf16* xo = (li & 1) ? xa : xb;
-      FO1_TRY(llm_layer(m, li, xin, xo, buf, B, cs_dec, false, nullptr, B, 0, nullptr, nullptr, &st, s, false));
+      bf16* xo = (li & 1) ? g.xa : g.xb;
+      FO1_TRY(llm_layer(m, li, xin, xo, g.layer, B, g.cs_dec, false, nullptr, B, 0, nullptr, nullptr, &k.st, s, false));
       xin = xo;
     }
-    FO1_TRY(rmsnorm(xin, H, m->llm.norm, lastn, H, B, H, c.rms_eps, s));
-    FO1_TRY(linear(lastn, H, m->llm.lm_head, H, logits, V, FO1_F32, B, V, H, nullptr, 0, FO1_EPI_NONE, nullptr, 0, 0, s));
-    if (sc) {
-      FO1_TRY(score_step());
-    } else if (sp) {
-      FO1_TRY(sample_rows(logits, V, B, V, d_samp, st.step, 0, st.new_tok, s));   // the Philox step is read from *st.step on the device
-    } else {
-      launch_k(argmax_kernel, dim3(B), dim3(1024), 0, s, logits, V, st.new_tok);
-      FO1_LAUNCH_CHECK();
-    }
-    launch_k(update_kernel, dim3(1), dim3(upd_threads), 0, s, st, d->n_stop_ids, d->pad_id, d->max_new_tokens, d->out_tokens, d->out_lens, B, 1, sa);
-    FO1_LAUNCH_CHECK();
-    return FO1_OK;
+    FO1_TRY(rmsnorm(xin, H, m->llm.norm, g.lastn, H, B, H, c.rms_eps, s));
+    FO1_TRY(linear(g.lastn, H, m->llm.lm_head, H, g.logits, V, FO1_F32, B, V, H, nullptr, 0, FO1_EPI_NONE, nullptr, 0, 0, s));
+    return decode_column(mode, g, k, sc, B, V, 1, s);
   };
-  if (mega_grid > 0 && d->max_new_tokens > 1) {
-    // ---- the whole greedy loop as ONE cooperative launch ----
-    MegaArgs a;
-    memset(&a, 0, sizeof(a));
-    a.B = B; a.layers = c.llm_layers; a.H = H; a.QD = QD; a.KD = KD; a.hd = hd; a.q_heads = c.llm_heads; a.kv_heads = c.llm_kv_heads;
-    a.I = c.llm_inter; a.V = V; a.eps = c.rms_eps; a.theta = c.rope_theta; a.sec_t = c.mrope_section[0]; a.sec_h = c.mrope_section[1];
-    a.layer = static_cast<const MegaLayer*>(m->llm.mega_layers);
-    a.head_w = m->llm.head_dec; a.embed = m->llm.embed;
-    a.kv_layer_stride = (long long)m->kv_batch * m->kv_cap * KD;
-    a.kc = static_cast<bf16*>(m->kv_cache);
-    a.vc = static_cast<bf16*>(m->kv_cache) + (size_t)c.llm_layers * a.kv_layer_stride;
-    a.cap = m->kv_cap;
-    a.x = xa; a.x_mid = buf.x_mid; a.qkv = buf.qkv; a.att = buf.att; a.h = buf.h;
-    a.ssq = mg_ssq; a.cs = cs_dec; a.att_part = buf.dec_part; a.att_count = mg_sync + 8;
-    a.amax_val = mg_amax_v; a.amax_idx = mg_amax_i;
-    a.cache_len = st.cache_len; a.pos3 = st.pos3; a.cur_tok = st.cur_tok; a.finished = st.finished; a.n_active = st.n_active; a.step = st.step;
-    a.stop_ids = st.stop_ids; a.n_stop = d->n_stop_ids; a.pad_id = d->pad_id; a.max_new = d->max_new_tokens;
-    a.out_tokens = d->out_tokens; a.out_lens = d->out_lens;
-    a.logits = logits; a.samp = d_samp; a.samp_tok = d_samp_tok;
-    if (sc) { a.sc_logprobs = sc->logprobs; a.sc_scores = sc->scores; a.sc_logits = sc->logits; }
-    a.stream = sa;
-    a.n_steps = d->max_new_tokens - 1;
-    a.bar = reinterpret_cast<unsigned*>(mg_sync);
-    const int pairs = B * c.llm_kv_heads;
-    a.n_splits = std::max(1, std::min(kMgMaxSplits, mega_grid / std::max(1, pairs)));
-    FO1_CUDA(cudaMemsetAsync(mg_sync, 0, ((size_t)pairs + 8) * sizeof(int), s));
-    unsigned long long* d_prof = nullptr;
-    const int prof_slots = 5 * c.llm_layers + 3 + (per_row ? 1 : 0) + 8;     // (+ the sampling barrier) + 8 sub-stamps of one attention item (CTA 0, layer 1)
-    if (getenv("FO1_MEGA_PROF") != nullptr) {       // diagnostic: where a decode iteration spends its time (stderr)
-      FO1_CUDA(cudaMalloc(reinterpret_cast<void**>(&d_prof), (size_t)mega_grid * prof_slots * 2 * sizeof(unsigned long long)));
-      FO1_CUDA(cudaMemsetAsync(d_prof, 0, (size_t)mega_grid * prof_slots * 2 * sizeof(unsigned long long), s));
-      a.prof = d_prof; a.prof_slots = prof_slots;
-    }
-    FO1_TRY(decode_mega_run(a, s));
-    m->last_decode_path = 1;
-    if (d_prof != nullptr) {
-      std::vector<unsigned long long> h((size_t)mega_grid * prof_slots * 2);
-      FO1_CUDA(cudaStreamSynchronize(s));
-      FO1_CUDA(cudaMemcpy(h.data(), d_prof, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-      cudaFree(d_prof);
-      // per slot: the last CTA to enter the barrier ends the phase; release = when CTA 0 leaves.  work = last_enter - previous release,
-      // skew = last_enter - first_enter, barrier = release - last_enter
-      const char* names[5] = {"qkv", "attn", "oproj", "gateup", "down"};
-      double tot[5][3] = {{0}}, misc = 0;
-      unsigned long long prev_release = 0;
-      for (int sl = 0; sl < prof_slots - 8; ++sl) {
-        unsigned long long first = ~0ull, last = 0, rel = 0;
-        for (int cta = 0; cta < mega_grid; ++cta) {
-          const unsigned long long e = h[((size_t)cta * prof_slots + sl) * 2], l = h[((size_t)cta * prof_slots + sl) * 2 + 1];
-          if (e < first) first = e;
-          if (e > last) last = e;
-          if (l > rel) rel = l;
-        }
-        if (sl >= 1 && sl <= 5 * c.llm_layers) {
-          const int ph = (sl - 1) % 5;
-          tot[ph][0] += (double)(last - prev_release); tot[ph][1] += (double)(last - first); tot[ph][2] += (double)(rel - last);
-        } else if (sl > 0) misc += (double)(rel - prev_release);
-        prev_release = rel;
-      }
-      fprintf(stderr, "[decode_mega profile, first iteration, B=%d, %d CTAs] per layer (us): ", B, mega_grid);
-      for (int ph = 0; ph < 5; ++ph)
-        fprintf(stderr, "%s work %.1f (skew %.1f) barrier %.1f | ", names[ph], tot[ph][0] / c.llm_layers / 1e3, tot[ph][1] / c.llm_layers / 1e3,
-                tot[ph][2] / c.llm_layers / 1e3);
-      fprintf(stderr, "head+update %.1f us\n", misc / 1e3);
-      {   // distribution over CTAs of the time spent in layer 1's attention phase (slot 7: enter of the barrier after it; slot 6: leave before it)
-        std::vector<std::pair<double, int>> dur;
-        for (int cta = 0; cta < mega_grid; ++cta)
-          dur.push_back({(double)(h[((size_t)cta * prof_slots + 7) * 2] - h[((size_t)cta * prof_slots + 6) * 2 + 1]) / 1e3, cta});
-        std::sort(dur.begin(), dur.end());
-        fprintf(stderr, "[decode_mega profile] attention phase per CTA (us): min %.1f p25 %.1f median %.1f p75 %.1f max %.1f; slowest CTAs:", dur[0].first,
-                dur[mega_grid / 4].first, dur[mega_grid / 2].first, dur[3 * mega_grid / 4].first, dur.back().first);
-        for (int k = 0; k < 6; ++k) fprintf(stderr, " %d(%.1f)", dur[mega_grid - 1 - k].second, dur[mega_grid - 1 - k].first);
-        fprintf(stderr, "\n");
-      }
-      fprintf(stderr, "[decode_mega profile] attention item of CTA 0, layer 1 (us since its start): ");
-      const unsigned long long a0 = h[((size_t)0 * prof_slots + prof_slots - 8) * 2];
-      const char* an[8] = {"start", "append+fence", "q rotated", "tiles done", "warps synced", "partials written", "fence+sync", "combined"};
-      for (int k = 0; k < 8; ++k) fprintf(stderr, "%s %.1f | ", an[k], (double)(h[((size_t)0 * prof_slots + prof_slots - 8 + k) * 2] - a0) / 1e3);
-      fprintf(stderr, "\n");
-    }
-    d->steps_run = d->max_new_tokens - 1;
-    return FO1_OK;
-  }
   cudaGraphExec_t gexec = nullptr;
   m->last_decode_path = 0;
   const bool want_graph = !g_prof_on && d->max_new_tokens > 3 && getenv("FO1_NO_GRAPH") == nullptr;
@@ -794,7 +693,7 @@ static int llm_generate_impl(Model* m, fo1_generate_desc* d, const fo1_sampling_
     // streamed: `done` is in host memory, so the host loop stops enqueueing without a sync once the device has published it
     if (h_progress != nullptr && (__atomic_load_n(h_progress, __ATOMIC_ACQUIRE) & FO1_STREAM_DONE)) break;
     if (d->early_exit_interval > 0 && step % d->early_exit_interval == 0) {
-      if (cudaMemcpyAsync(ls->h_flag, st.n_active, sizeof(int), cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess) {
+      if (cudaMemcpyAsync(ls->h_flag, k.st.n_active, sizeof(int), cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess) {
         set_error("early-exit poll failed"); rc = FO1_ERR_CUDA; break;
       }
       if (*ls->h_flag <= 0) break;  // every sequence has emitted a stop id; the tail is already pad_id
@@ -830,6 +729,7 @@ static int stream_resolve(const fo1_stream_desc* h, StreamArgs* sa) {
 
 int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, const fo1_score_desc* sc, const fo1_stream_desc* stm,
                  cudaStream_t s) {
+  if (sc != nullptr && sc->logprobs == nullptr && sc->scores == nullptr && sc->logits == nullptr) sc = nullptr;   // nothing to score
   // the per-sequence host arrays first: they are the caller's, and need neither the model nor the device
   if (sp) FO1_TRY(sampling_check(sp, d->n_seqs, sc ? "fo1_llm_generate_scored" : "fo1_llm_generate_sampled"));
   if (sc) FO1_TRY(raw_rows_check(sp, sc->raw_rows, d->n_seqs, "fo1_llm_generate_scored"));
@@ -844,17 +744,20 @@ int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, co
     FO1_CHECK_ARG(d->seq_lens[b] > 0, "fo1_llm_generate: sequence %d is empty", b);
     max_len = std::max(max_len, d->seq_lens[b]);
   }
-  StreamArgs sa = {};
+  ColumnSink k = {};
   if (stm) {
-    FO1_TRY(stream_resolve(stm, &sa));
+    FO1_TRY(stream_resolve(stm, &k.stream));
     __atomic_store_n(stm->progress, d->max_new_tokens > 0 ? 0 : FO1_STREAM_DONE, __ATOMIC_RELEASE);   // before anything is enqueued
   }
-  DecodeState st;
-  FO1_TRY(ensure_state(m, d->n_seqs, d->n_stop_ids, &st));
+  FO1_TRY(ensure_state(m, d->n_seqs, d->n_stop_ids, &k.st));
+  k.n_stop = d->n_stop_ids; k.pad_id = d->pad_id; k.max_new = d->max_new_tokens;
+  k.out_tokens = d->out_tokens; k.out_lens = d->out_lens;
+  const DecodeMode mode = sc ? DEC_SCORED : sp ? DEC_SAMPLED : DEC_GREEDY;
   FO1_TRY(ensure_kv(m, d->n_seqs, max_len + std::max(d->max_new_tokens, 1)));
   FO1_TRY(int_cache_trim(m));
   m->arena.reset(true);
-  FO1_TRY(llm_generate_impl(m, d, sp, sc, s, true, st, sa, nullptr));
+  DecodeBufs g;
+  FO1_TRY(llm_prefill(m, d, sp, sc, mode, k, s, true, g));
   FO1_TRY(arena_ensure(m, m->arena.peak));
   m->arena.reset(false);
   if (d->max_new_tokens > 0) {  // out_tokens pre-filled with pad so an early exit leaves a clean tail
@@ -864,7 +767,10 @@ int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, co
     FO1_CUDA(cudaMemsetAsync(d->out_lens, 0, d->n_seqs * sizeof(int), s));
     if (sc && sc->logprobs) FO1_CUDA(cudaMemsetAsync(sc->logprobs, 0, (size_t)n * sizeof(float), s));      // 0 past out_lens
   }
-  return llm_generate_impl(m, d, sp, sc, s, false, st, sa, stm ? stm->progress : nullptr);
+  FO1_TRY(llm_prefill(m, d, sp, sc, mode, k, s, false, g));
+  if (d->max_new_tokens <= 0) return FO1_OK;
+  if (g.mega_grid > 0 && d->max_new_tokens > 1) return decode_persistent(m, d, sc, mode, k, g, s);
+  return decode_per_kernel(m, d, sc, mode, k, g, stm ? stm->progress : nullptr, s);
 }
 
 // -------------------------------------------------------------------------------- splice plan (host, integer)
@@ -988,7 +894,6 @@ extern "C" int fo1_llm_generate_sampled(fo1_model* m, fo1_generate_desc* d, cons
 extern "C" int fo1_llm_generate_scored(fo1_model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, const fo1_score_desc* sc,
                                        void* stream) {
   FO1_CHECK_ARG(m && d, "fo1_llm_generate_scored: null argument");
-  if (sc != nullptr && sc->logprobs == nullptr && sc->scores == nullptr && sc->logits == nullptr) sc = nullptr;
   return llm_generate(m, d, sp, sc, nullptr, static_cast<cudaStream_t>(stream));
 }
 
@@ -997,7 +902,6 @@ extern "C" int fo1_llm_generate_streamed(fo1_model* m, fo1_generate_desc* d, con
   FO1_CHECK_ARG(m && d, "fo1_llm_generate_streamed: null argument");
   FO1_CHECK_ARG(st == nullptr || (st->tokens && st->lens && st->progress), "fo1_llm_generate_streamed: null stream buffer (tokens, lens and "
                 "progress are required; cancel may be NULL)");
-  if (sc != nullptr && sc->logprobs == nullptr && sc->scores == nullptr && sc->logits == nullptr) sc = nullptr;
   return llm_generate(m, d, sp, sc, st, static_cast<cudaStream_t>(stream));
 }
 

@@ -307,28 +307,25 @@ def _engine_generate(self, inputs_embeds: torch.Tensor, position_ids: torch.Tens
     d.all_logits = al.data_ptr() if al is not None else None
     d.early_exit_interval = early_exit_interval
     L = lib()
-    scored = lp is not None or sc is not None or lg is not None
+    sp_arg = sc_arg = None      # NULL: greedy / unscored (fo1_llm_generate_streamed with NULL arguments is each older entry point)
     if sampling is not None:
         sd, _keep = _lib.sampling_desc(sampling.temperature, sampling.top_p, sampling.top_k, sampling.seed)
         assert len(sampling.temperature) == B, "one sampling parameter set per sequence"
-    if scored:
+        sp_arg = C.byref(sd)
+    if lp is not None or sc is not None or lg is not None:
         ptr = lambda t: t.data_ptr() if t is not None else None
         rr = (C.c_int32 * B)(*[int(x) for x in raw_rows]) if raw_rows is not None else None
         assert raw_rows is None or len(raw_rows) == B, "one raw_rows flag per sequence"
         desc = _lib.ScoreDesc(ptr(lp), ptr(sc), ptr(lg), rr)
-    if on_tokens is not None:
-        sp_arg = C.byref(sd) if sampling is not None else None
-        sc_arg = C.byref(desc) if scored else None
-        self._run_streamed(lambda stream, st: check(L.fo1_llm_generate_streamed(self._h, C.byref(d), sp_arg, sc_arg, C.byref(st), stream),
-                                                    "fo1_llm_generate_streamed"), B, max_new_tokens, on_tokens)
-    elif scored:
-        check(L.fo1_llm_generate_scored(self._h, C.byref(d), C.byref(sd) if sampling is not None else None, C.byref(desc), _stream()),
-              "fo1_llm_generate_scored")
-    elif sampling is None:
-        L.fo1_llm_generate.restype = C.c_int
-        check(L.fo1_llm_generate(self._h, C.byref(d), _stream()), "fo1_llm_generate")
+        sc_arg = C.byref(desc)
+
+    def launch(stream, st=None):
+        check(L.fo1_llm_generate_streamed(self._h, C.byref(d), sp_arg, sc_arg, C.byref(st) if st is not None else None, stream),
+              "fo1_llm_generate_streamed")
+    if on_tokens is None:
+        launch(_stream())
     else:
-        check(L.fo1_llm_generate_sampled(self._h, C.byref(d), C.byref(sd), _stream()), "fo1_llm_generate_sampled")
+        self._run_streamed(launch, B, max_new_tokens, on_tokens)
     out = dict(tokens=toks, lens=lens, prefill_logits=pl, all_logits=al, steps_run=d.steps_run)
     if want_logprobs:
         out["logprobs"] = lp
