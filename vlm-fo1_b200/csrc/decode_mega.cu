@@ -853,14 +853,24 @@ static int mg_prof_report(const MegaArgs& a, int grid, cudaStream_t s) {
   return FO1_OK;
 }
 
+bool decode_mega_supports(int H, int hd, int q_heads, int kv_heads, int I, int V) {
+  const int QD = q_heads * hd, KD = kv_heads * hd;
+  // one GQA group (<= 8 query heads of 128) is the row block of an m16 attention tile
+  const bool heads = hd == 128 && kv_heads >= 1 && q_heads % kv_heads == 0 && q_heads / kv_heads <= 8;
+  // every matrix phase: K in 64-wide chunks over all 8 warps, N in 16-column tiles, A resident up to 2048 wide
+  const bool widths = H % kMgChunkK == 0 && QD % kMgChunkK == 0 && I % kMgChunkK == 0 && H <= kMgAK && QD <= kMgAK &&
+                      H / kMgChunkK >= kMgWarps && QD / kMgChunkK >= kMgWarps && H % kMgTileN == 0 && (QD + 2 * KD) % kMgTileN == 0 &&
+                      (2 * I) % kMgTileN == 0;
+  return heads && widths && V % kMgTileN == 0;
+}
+
 // One cooperative launch for the whole decode loop.  `a.bar` and `a.att_count` must be zero (the caller memsets them on `s`).
 int decode_mega_run(MegaArgs a, DecodeMode mode, cudaStream_t s) {
   const int grid = decode_mega_grid();
   FO1_CHECK_ARG(grid > 0, "decode_mega: cooperative launch of a %d-byte-smem CTA per SM is not available on this device", kMgSmemBytes);
-  FO1_CHECK_ARG(a.B >= 1 && a.B <= kMgRows && a.hd == 128 && a.q_heads % a.kv_heads == 0 && a.q_heads / a.kv_heads <= 8, "decode_mega: unsupported shape");
-  FO1_CHECK_ARG(a.H % kMgChunkK == 0 && a.QD % kMgChunkK == 0 && a.H <= kMgAK && a.QD <= kMgAK && a.I % kMgChunkK == 0 && (a.QD + 2 * a.KD) % kMgTileN == 0 &&
-                a.H % kMgTileN == 0 && (2 * a.I) % kMgTileN == 0 && a.V % kMgTileN == 0 && (a.H / kMgChunkK) >= kMgWarps && (a.QD / kMgChunkK) >= kMgWarps,
-                "decode_mega: widths must be multiples of the 16 x 64 tile (H %d, QD %d, I %d, V %d)", a.H, a.QD, a.I, a.V);
+  FO1_CHECK_ARG(a.B >= 1 && a.B <= kMgRows, "decode_mega: %d sequences (1..%d)", a.B, kMgRows);
+  FO1_CHECK_ARG(a.QD == a.q_heads * a.hd && a.KD == a.kv_heads * a.hd && decode_mega_supports(a.H, a.hd, a.q_heads, a.kv_heads, a.I, a.V),
+                "decode_mega: unsupported shape (H %d, %d q / %d kv heads of %d, I %d, V %d)", a.H, a.q_heads, a.kv_heads, a.hd, a.I, a.V);
   FO1_CHECK_ARG(mode != DEC_SCORED || a.samp != nullptr, "decode_mega: scoring needs the per-row sampling parameters");
   FO1_CHECK_ARG(mode == DEC_GREEDY || (a.samp != nullptr && a.logits != nullptr && a.samp_tok != nullptr && (a.V & 1) == 0),
                 "decode_mega: sampling buffers missing");

@@ -43,6 +43,9 @@ struct MegaArgs {
 
 
 int decode_mega_grid();                                   // CTAs of the cooperative launch (0: not available on this device)
+// the model shapes the persistent kernel runs: hidden H, q / kv heads of hd, intermediate I, vocabulary V.  The one place that
+// decides it; a model outside it decodes on the per-kernel path
+bool decode_mega_supports(int H, int hd, int q_heads, int kv_heads, int I, int V);
 // the whole decode loop, one launch (streamed when a.sink.stream.progress != nullptr); FO1_MEGA_PROF=1 reports where the first
 // iteration spent its time on stderr (a.prof is set here)
 int decode_mega_run(MegaArgs a, DecodeMode mode, cudaStream_t s);

@@ -354,8 +354,9 @@ static int llm_resolve(Model* m) {
   if (!g.err.empty()) { set_error("LLM weights: %s", g.err.c_str()); return FO1_ERR_NOT_FOUND; }
   w.ok = true;
   // optional decode copies (weights.py::prepare_llm): W diag(g) for the two normed projections and the LM head, gate / up in the
-  // decode kernel's 8 + 8 row interleave.  All present -> the persistent decode kernel is used.
-  w.mega_ok = m->find("llm.head_dec") != nullptr;
+  // decode kernel's 8 + 8 row interleave.  All present and a model shape the kernel supports -> the persistent decode kernel is used.
+  w.mega_ok = m->find("llm.head_dec") != nullptr &&
+              decode_mega_supports(c.llm_hidden, c.llm_head_dim, c.llm_heads, c.llm_kv_heads, c.llm_inter, c.llm_vocab);
   for (int i = 0; i < c.llm_layers && w.mega_ok; ++i) {
     const std::string p = "llm.l" + std::to_string(i) + ".";
     w.mega_ok = m->find(p + "qkv_dec.w") != nullptr && m->find(p + "gu_dec.w") != nullptr;
@@ -372,12 +373,10 @@ static int llm_resolve(Model* m) {
       ml[i].qkv_w = L.qkv_dec; ml[i].qkv_b = L.qkv_b; ml[i].o_w = L.o_w; ml[i].gu_w = L.gu_dec; ml[i].down_w = L.down_w;
     }
     if (!g2.err.empty()) { set_error("LLM decode weights: %s", g2.err.c_str()); return FO1_ERR_NOT_FOUND; }
-    if (c.llm_inter != Ip) w.mega_ok = false;      // the decode kernel reads down_w with K = intermediate size (no padding)
-    if (w.mega_ok) {
-      if (w.mega_layers) cudaFree(w.mega_layers);
-      FO1_CUDA(cudaMalloc(&w.mega_layers, ml.size() * sizeof(MegaLayer)));
-      FO1_CUDA(cudaMemcpy(w.mega_layers, ml.data(), ml.size() * sizeof(MegaLayer), cudaMemcpyHostToDevice));
-    }
+    // the kernel reads down_w with K = intermediate size: a supported intermediate (a multiple of 64) is already its own padding
+    if (w.mega_layers) cudaFree(w.mega_layers);
+    FO1_CUDA(cudaMalloc(&w.mega_layers, ml.size() * sizeof(MegaLayer)));
+    FO1_CUDA(cudaMemcpy(w.mega_layers, ml.data(), ml.size() * sizeof(MegaLayer), cudaMemcpyHostToDevice));
   }
   return FO1_OK;
 }
