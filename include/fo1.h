@@ -162,6 +162,14 @@ int fo1_channel_attention(const void* qkv, int32_t n_images, int32_t n_tokens, i
 int fo1_dwconv3x3_residual(const void* x, const void* w9, const void* bias, void* y, int32_t n_images, int32_t height, int32_t width,
                            int32_t channels, void* stream);
 
+/* Row normalisation of bf16 rows x [rows][cols] (pitch ldx) into y (pitch ldy): rms = 1 is Qwen2RMSNorm (modeling_qwen2_5_vl.py:126-140,
+ * the normalised value rounded to bf16 before the gain; beta must be NULL), rms = 0 is nn.LayerNorm (fp32 two-pass statistics).
+ * gamma / beta bf16 [cols] or NULL (1 / 0).  cols and pitches multiples of 8, cols <= 8192; 16-byte aligned pointers.
+ * kernel 0: one warp per row (what the towers and the prefill layers run); kernel 1: one block per row, cols <= 4096 (what the decode
+ * steps and the prefill's last rows run).  Exposed for the parity test of the two kernels; the engine names one per call site. */
+int fo1_row_norm(const void* x, int64_t ldx, const void* gamma, const void* beta, void* y, int64_t ldy, int32_t rows, int32_t cols,
+                 float eps, int32_t rms, int32_t kernel, void* stream);
+
 /* Single-query GQA attention of one decode step over the K/V cache (the per-step attention of the HF generate loop,
  * modeling_qwen2_5_vl.py:731-780 with past_key_values; mm_utils.py:640-654 drives it).  The step's own K/V must already
  * sit in the cache at index cache_len[b].  head_dim 128, q_heads / kv_heads <= 8.  Exposed so the parity tests can

@@ -15,7 +15,7 @@ pytestmark = pytest.mark.gpu
 
 @pytest.fixture(autouse=True)
 def _mega_up_to_32(monkeypatch):
-    """The default threshold is 16 sequences (llm.cu); these tests cover both row-tile variants of the kernel."""
+    """The default threshold is 32 sequences (llm.cu); pinned here so these tests cover both row-tile variants of the kernel."""
     monkeypatch.setenv("FO1_MEGA_MAX_B", "32")
 
 

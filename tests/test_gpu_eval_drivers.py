@@ -69,18 +69,9 @@ def test_generate_batch_equals_one_by_one(setup):
                                              {"type": "text", "text": d["conversations"][0]["value"]}], "bbox_list": d["bbox_list"]}]
         kws.append(prepare_inputs(model_path, model, procs, tokenizer, msg, device="cuda:0", max_tokens=10, top_p=0.05, temperature=0.0, do_sample=False))
     batch = model.generate_batch(kws)
-    first_same, same = 0, 0
-    for kw, got in zip(kws, batch):
+    for i, (kw, got) in enumerate(zip(kws, batch)):
         one = model.generate(**kw)
         P = kw["inputs"].shape[1]
-        assert torch.equal(one[:, :P], got[:, :P])                       # the prompt part is the caller's own ids
-        assert one.shape[1] > P and got.shape[1] > P
-        first_same += int(one[0, P]) == int(got[0, P])
-        same += int(one.shape == got.shape and torch.equal(one, got))
-    # This fabricated checkpoint has ONE random-init decoder layer: its logits are nearly flat, so a last-bit difference anywhere
-    # upstream flips a token (measured: whole-batch equality in about half of the runs while the noise images were still salted per
-    # process, i.e. roughly one flip per 60 tokens; they are crc32-seeded now).  Two row-count heuristics that made a sample's numerics
-    # depend on the batch size (norm kernel choice below 593 rows, split-K by tile count) were removed AFTER the last GPU run of the
-    # round (DESIGN.md section 2); until that is confirmed on a GPU the assertion is: well-formed sequences, first tokens agree for all
-    # but at most one sample, most sequences agree entirely.  TODO(next round): torch.equal for every sample.
-    assert first_same >= len(kws) - 1 and same >= 3, (first_same, same)
+        assert one.shape[1] > P
+        # the one-layer random checkpoint has nearly flat logits, so a last-bit difference anywhere upstream would flip a token
+        assert one.shape == got.shape and torch.equal(one, got), (i, one[0, P:].tolist(), got[0, P:].tolist())

@@ -249,15 +249,10 @@ def test_generate_batch_sampled_equals_one_by_one(fab):
     batch = model.generate_batch(kws)
     torch.manual_seed(21)
     ones = [model.generate(**k) for k in kws]
-    first_same = same = 0
-    for k, one, got in zip(kws, ones, batch):
+    for i, (k, one, got) in enumerate(zip(kws, ones, batch)):
         P = k["inputs"].shape[1]
-        assert torch.equal(one[:, :P], got[:, :P]) and got.shape[1] > P
-        first_same += int(one[0, P]) == int(got[0, P])
-        same += int(one.shape == got.shape and torch.equal(one, got))
-    # as test_gpu_eval_drivers.test_generate_batch_equals_one_by_one: the one-layer random checkpoint has nearly flat logits, where
-    # a last-bit difference upstream of the head (batched against single prefill) can move a draw
-    assert first_same >= len(kws) - 1 and same >= len(kws) - 2, (first_same, same)
+        assert one.shape[1] > P
+        assert one.shape == got.shape and torch.equal(one, got), (i, one[0, P:].tolist(), got[0, P:].tolist())
 
 
 def test_generate_argument_contract(fab, tmp_path):

@@ -117,7 +117,8 @@ def test_region_projector_matches_oracle():
 @pytest.mark.parametrize("grid", [(32, 32), (16, 16), (64, 64)])
 def test_fpn_implicit_conv_equals_im2col_path(grid, monkeypatch):
     """SimpleFPN's 3x3 convs run as an implicit GEMM (4-D TMA patches, zero padding by the out-of-range fill, gemm_wgmma.cu
-    conv3x3_gemm); FO1_FPN_IM2COL forces the explicit column matrix + linear.  Same products in the same k order: bit-identical."""
+    conv3x3_gemm); FO1_FPN_IM2COL forces the explicit column matrix + linear.  Same products in the same k order: bit-identical,
+    whichever tile width each path picks (tests/test_gpu_batch_invariance.py)."""
     E, W = _mods()
     CK = __import__("importlib").import_module("vlm-fo1_b200.checkpoint")
     cfg = E.EngineConfig(); cfg.use_davit = cfg.use_llm = False; cfg.proj_aux_layers = 0
@@ -134,10 +135,4 @@ def test_fpn_implicit_conv_equals_im2col_path(grid, monkeypatch):
     torch.cuda.synchronize()
     for i in range(4):
         assert torch.isfinite(a[i].float()).all()
-        rows = a[i].shape[0] * a[i].shape[1] * a[i].shape[2]
-        diff = (a[i].float() - b[i].float()).abs()
-        if rows >= 132 * 128:      # both paths run the same unsplit 256-wide tiles: same products, same order
-            assert torch.equal(a[i], b[i]), (i, float(diff.max()))
-        else:                      # the explicit path's small GEMM is split over K (other summation order): bf16-ulp flips before the LayerNorm
-            assert float(diff.max()) <= 0.0625 and float(diff.mean()) < 2e-3 and float((diff == 0).float().mean()) > 0.8, \
-                (i, float(diff.max()), float(diff.mean()), float((diff == 0).float().mean()))
+        assert torch.equal(a[i], b[i]), (i, float((a[i].float() - b[i].float()).abs().max()))

@@ -87,10 +87,10 @@ static int davit_forward_impl(Model* m, const float* const* images, int H0, int 
       const int per = Hh * Ww;
       for (int b = 0; b < B; ++b) FO1_RUN(im2col_stem(images[b], col + (size_t)b * per * 152, H0, W0, 152, s));
       FO1_RUN(linear(col, 152, W.conv_w, 152, yb, C, FO1_BF16, tok, C, 152, W.conv_b, FO1_BF16, FO1_EPI_NONE, nullptr, 0, 0, s));
-      FO1_RUN(layernorm(yb, C, W.norm_w, W.norm_b, x, C, tok, C, eps, s));
+      FO1_RUN(layernorm(yb, C, W.norm_w, W.norm_b, x, C, tok, C, eps, NORM_WARP, s));
     } else {
       const int Cin = c.davit_dims[st - 1], Hp = Hs[st - 1], Wp = Ws[st - 1];
-      FO1_RUN(layernorm(x, Cin, W.norm_w, W.norm_b, yb, Cin, B * Hp * Wp, Cin, eps, s));
+      FO1_RUN(layernorm(x, Cin, W.norm_w, W.norm_b, yb, Cin, B * Hp * Wp, Cin, eps, NORM_WARP, s));
       FO1_RUN(im2col3x3(yb, col, B, Hp, Wp, Cin, 2, s));
       FO1_RUN(linear(col, 9 * Cin, W.conv_w, 9 * Cin, x, C, FO1_BF16, tok, C, 9 * Cin, W.conv_b, FO1_BF16, FO1_EPI_NONE, nullptr, 0, 0, s));
     }
@@ -114,7 +114,7 @@ static int davit_forward_impl(Model* m, const float* const* images, int H0, int 
         // conv1: x <- x + dw3x3(x)
         FO1_RUN(dwconv3x3_residual(x, h.conv1_w9, h.conv1_b, xalt, B, Hh, Ww, C, s));
         std::swap(x, xalt);
-        FO1_RUN(layernorm(x, C, h.norm1_w, h.norm1_b, yb, C, tok, C, eps, s));
+        FO1_RUN(layernorm(x, C, h.norm1_w, h.norm1_b, yb, C, tok, C, eps, NORM_WARP, s));
         if (half == 0) {
           // SpatialBlock: window attention (:225-282)
           FO1_RUN(window_partition(yb, wb, B, Hh, Ww, C, ws, s));
@@ -140,7 +140,7 @@ static int davit_forward_impl(Model* m, const float* const* images, int H0, int 
         // conv2 + FFN
         FO1_RUN(dwconv3x3_residual(x, h.conv2_w9, h.conv2_b, xalt, B, Hh, Ww, C, s));
         std::swap(x, xalt);
-        FO1_RUN(layernorm(x, C, h.norm2_w, h.norm2_b, yb, C, tok, C, eps, s));
+        FO1_RUN(layernorm(x, C, h.norm2_w, h.norm2_b, yb, C, tok, C, eps, NORM_WARP, s));
         FO1_RUN(linear(yb, C, h.fc1_w, C, hb, 4 * C, FO1_BF16, tok, 4 * C, C, h.fc1_b, FO1_BF16, FO1_EPI_GELU, nullptr, 0, 0, s));
         FO1_RUN(linear(hb, 4 * C, h.fc2_w, 4 * C, xalt, C, FO1_BF16, tok, C, 4 * C, h.fc2_b, FO1_BF16, FO1_EPI_NONE, x, C, 0, s));
         std::swap(x, xalt);
@@ -211,7 +211,7 @@ static int fpn_forward_impl(Model* m, const bf16* tap, int gh, int gw, int B, vo
       bf16* u1 = A.alloc<bf16>(px * 4 * (D / 2));
       FO1_RUN(linear(tap, D, f.l0_dc1_w, D, g1, 4 * (D / 2), FO1_BF16, (int)px, 4 * (D / 2), D, f.l0_dc1_b, FO1_BF16, FO1_EPI_NONE, nullptr, 0, 0, s));
       FO1_RUN(pixel_shuffle2x(g1, u1, B, gh, gw, D / 2, s));
-      FO1_RUN(layernorm(u1, D / 2, f.l0_ln_w, f.l0_ln_b, g1, D / 2, (int)(px * 4), D / 2, eps, s));
+      FO1_RUN(layernorm(u1, D / 2, f.l0_ln_w, f.l0_ln_b, g1, D / 2, (int)(px * 4), D / 2, eps, NORM_WARP, s));
       FO1_RUN(gelu_bf16(g1, g1, (long long)px * 4 * (D / 2), s));
       bf16* g2 = A.alloc<bf16>(px * 16 * (D / 4));
       bf16* u2 = A.alloc<bf16>(px * 16 * (D / 4));
@@ -232,7 +232,7 @@ static int fpn_forward_impl(Model* m, const bf16* tap, int gh, int gw, int B, vo
     bf16* t1 = A.alloc<bf16>(pl * O);
     bf16* t2 = A.alloc<bf16>(pl * O);
     FO1_RUN(linear(feat, Cin, f.lv[l].conv1_w, Cin, t1, O, FO1_BF16, (int)pl, O, Cin, nullptr, 0, FO1_EPI_NONE, nullptr, 0, 0, s));
-    FO1_RUN(layernorm(t1, O, f.lv[l].ln1_w, f.lv[l].ln1_b, t2, O, (int)pl, O, eps, s));
+    FO1_RUN(layernorm(t1, O, f.lv[l].ln1_w, f.lv[l].ln1_b, t2, O, (int)pl, O, eps, NORM_WARP, s));
     // 3x3 conv: implicit GEMM (the A tiles are TMA patches of t2, zero padding by the out-of-range fill); shapes that do not
     // tile into 128-pixel patches -- or FO1_FPN_IM2COL, the A/B knob of the parity test -- take im2col + linear
     const bool force_im2col = getenv("FO1_FPN_IM2COL") != nullptr;
@@ -254,7 +254,7 @@ static int fpn_forward_impl(Model* m, const bf16* tap, int gh, int gw, int B, vo
         FO1_RUN(linear(colb, 9 * O, f.lv[l].conv2_w, 9 * O, t1 + o * O, O, FO1_BF16, nb * Hl * Wl, O, 9 * O, nullptr, 0, FO1_EPI_NONE, nullptr, 0, 0, s));
       }
     }
-    FO1_RUN(layernorm(t1, O, f.lv[l].ln2_w, f.lv[l].ln2_b, static_cast<bf16*>(dry ? nullptr : level_out[l]), O, (int)pl, O, eps, s));
+    FO1_RUN(layernorm(t1, O, f.lv[l].ln2_w, f.lv[l].ln2_b, static_cast<bf16*>(dry ? nullptr : level_out[l]), O, (int)pl, O, eps, NORM_WARP, s));
     A.release(mark);
   }
   return FO1_OK;

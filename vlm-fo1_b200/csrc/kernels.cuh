@@ -20,11 +20,18 @@ int linear(const bf16* A, long long lda, const bf16* W, long long ldw, void* D, 
            cudaStream_t stream);
 
 // ---- norm.cu ----
+// The two row-norm kernels sum a row in different orders, so the CALL SITE names one and keeps it whatever the number of rows: a
+// row's bits then never depend on how many rows share its launch (a sample alone vs the same sample in a batch).
+//   NORM_WARP:  one warp per row -- token matrices (towers, prefill layers, all-position logits).
+//   NORM_BLOCK: one block per row, cols <= kNormBlockMaxCols -- one row per sequence (decode steps, the prefill's last rows).
+enum NormKernel { NORM_WARP = 0, NORM_BLOCK = 1 };
+constexpr int kNormBlockMaxCols = 4096;
 // Qwen2RMSNorm (modeling_qwen2_5_vl.py:126-140): y = w * bf16(x * rsqrt(mean(x^2) + eps))
-int rmsnorm(const bf16* x, long long ldx, const bf16* w, bf16* y, long long ldy, int rows, int cols, float eps, cudaStream_t s);
+int rmsnorm(const bf16* x, long long ldx, const bf16* w, bf16* y, long long ldy, int rows, int cols, float eps, NormKernel kernel,
+            cudaStream_t s);
 // nn.LayerNorm over the last dim (fp32 statistics), optional gamma/beta
 int layernorm(const bf16* x, long long ldx, const bf16* gamma, const bf16* beta, bf16* y, long long ldy, int rows, int cols,
-              float eps, cudaStream_t s);
+              float eps, NormKernel kernel, cudaStream_t s);
 
 // ---- rope.cu ----
 // ViT 2-D RoPE (modeling_qwen2_5_vl.py:162-169, 436-463): table[t][j] = pos_{h|w}[t] * inv_freq[j mod half]

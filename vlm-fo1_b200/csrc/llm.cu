@@ -429,6 +429,10 @@ static int ensure_state(Model* m, int B, int n_stop, DecodeState* st) {
   return FO1_OK;
 }
 
+// norm kernel of the launches with one row per sequence (decode steps, the prefill's last rows): the block-per-row kernel at any batch
+// size; the width alone decides for models wider than it serves
+static NormKernel seq_norm_kernel(int H) { return H <= kNormBlockMaxCols ? NORM_BLOCK : NORM_WARP; }
+
 // one decoder layer over `rows` packed rows.  x_in -> x_out (x_mid scratch).  prefill: varlen causal attention
 // + cache fill; decode: cache append + single-query attention.
 struct LayerBuf { bf16 *xn, *qkv, *att, *x_mid, *h; float* dec_part; int* rowseg = nullptr; double attn_flops = 0.0; const int* tiles = nullptr; int n_tiles = 0; };
@@ -443,7 +447,8 @@ static int llm_layer(Model* m, int li, const bf16* x_in, bf16* x_out, const Laye
   const size_t layer_stride = (size_t)m->kv_batch * m->kv_cap * KD;
   bf16* kc = static_cast<bf16*>(m->kv_cache) + (size_t)li * layer_stride;
   bf16* vc = static_cast<bf16*>(m->kv_cache) + ((size_t)c.llm_layers + li) * layer_stride;
-  FO1_RUN(rmsnorm(x_in, H, L.ln1, B_.xn, H, rows, H, c.rms_eps, s));
+  const NormKernel nk = prefill ? NORM_WARP : seq_norm_kernel(H);
+  FO1_RUN(rmsnorm(x_in, H, L.ln1, B_.xn, H, rows, H, c.rms_eps, nk, s));
   FO1_RUN(linear(B_.xn, H, L.qkv_w, H, B_.qkv, ldq, FO1_BF16, rows, ldq, H, L.qkv_b, FO1_BF16, FO1_EPI_NONE, nullptr, 0, 0, s));
   if (prefill) {
     FO1_RUN(rope_apply(B_.qkv, ldq, cs, rows, c.llm_heads + c.llm_kv_heads, hd, s));   // q|k heads are contiguous in the packed row
@@ -464,7 +469,7 @@ static int llm_layer(Model* m, int li, const bf16* x_in, bf16* x_out, const Laye
                              1.0f / sqrtf((float)hd), B_.att, QD, B_.dec_part, s));
   }
   FO1_RUN(linear(B_.att, QD, L.o_w, QD, B_.x_mid, H, FO1_BF16, rows, H, QD, nullptr, 0, FO1_EPI_NONE, x_in, H, 0, s));
-  FO1_RUN(rmsnorm(B_.x_mid, H, L.ln2, B_.xn, H, rows, H, c.rms_eps, s));
+  FO1_RUN(rmsnorm(B_.x_mid, H, L.ln2, B_.xn, H, rows, H, c.rms_eps, nk, s));
   FO1_RUN(linear(B_.xn, H, L.gateup_w, H, B_.h, Ip, FO1_BF16, rows, 2 * Ip, H, nullptr, 0, FO1_EPI_SILU, nullptr, 0, 1, s));
   FO1_RUN(linear(B_.h, Ip, L.down_w, Ip, x_out, H, FO1_BF16, rows, H, Ip, nullptr, 0, FO1_EPI_NONE, B_.x_mid, H, 0, s));
   return FO1_OK;
@@ -588,11 +593,11 @@ static int llm_prefill(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* 
     x = xo;
   }
   if (d->all_logits) {
-    FO1_RUN(rmsnorm(x, H, m->llm.norm, alln, H, (int)T, H, c.rms_eps, s));
+    FO1_RUN(rmsnorm(x, H, m->llm.norm, alln, H, (int)T, H, c.rms_eps, NORM_WARP, s));
     FO1_RUN(linear(alln, H, m->llm.lm_head, H, d->all_logits, V, FO1_F32, (int)T, V, H, nullptr, 0, FO1_EPI_NONE, nullptr, 0, 0, s));
   }
   FO1_RUN(gather_rows_bf16(x, H, d_last, last, H, B, H, s));
-  FO1_RUN(rmsnorm(last, H, m->llm.norm, g.lastn, H, B, H, c.rms_eps, s));
+  FO1_RUN(rmsnorm(last, H, m->llm.norm, g.lastn, H, B, H, c.rms_eps, seq_norm_kernel(H), s));
   {
     SplitKScope sk(true);       // M = number of sequences: weight streaming
     FO1_RUN(linear(g.lastn, H, m->llm.lm_head, H, g.logits, V, FO1_F32, B, V, H, nullptr, 0, FO1_EPI_NONE, nullptr, 0, 0, s));
@@ -654,7 +659,7 @@ static int decode_per_kernel(Model* m, fo1_generate_desc* d, const fo1_score_des
       FO1_TRY(llm_layer(m, li, xin, xo, g.layer, B, g.cs_dec, false, nullptr, B, 0, nullptr, nullptr, &k.st, s, false));
       xin = xo;
     }
-    FO1_TRY(rmsnorm(xin, H, m->llm.norm, g.lastn, H, B, H, c.rms_eps, s));
+    FO1_TRY(rmsnorm(xin, H, m->llm.norm, g.lastn, H, B, H, c.rms_eps, seq_norm_kernel(H), s));
     FO1_TRY(linear(g.lastn, H, m->llm.lm_head, H, g.logits, V, FO1_F32, B, V, H, nullptr, 0, FO1_EPI_NONE, nullptr, 0, 0, s));
     return decode_column(mode, g, k, sc, B, V, 1, s);
   };

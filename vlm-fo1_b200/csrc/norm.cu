@@ -168,16 +168,14 @@ __global__ void __launch_bounds__(256) rownorm_block_kernel(const bf16* __restri
 
 template <bool RMS>
 static int launch_rownorm(const bf16* x, long long ldx, const bf16* g, const bf16* b, bf16* y, long long ldy, int rows, int cols,
-                          float eps, cudaStream_t s) {
+                          float eps, NormKernel kernel, cudaStream_t s) {
   FO1_CHECK_ARG(cols % 8 == 0 && ldx % 8 == 0 && ldy % 8 == 0, "rownorm: cols/pitches must be multiples of 8 (cols=%d)", cols);
   FO1_CHECK_ARG(cols <= 8 * 32 * 32, "rownorm: cols=%d too large", cols);
+  FO1_CHECK_ARG(kernel == NORM_WARP || (kernel == NORM_BLOCK && cols <= kNormBlockMaxCols), "rownorm: kernel %d unsupported at cols=%d",
+                (int)kernel, cols);
   if (rows == 0) return FO1_OK;
   const int nvec = cols / 8;
-  // Decode-shaped launches (one row per sequence) spread each row over a block.  The threshold is the decode batch limit, NOT "fewer rows
-  // than the GPU has warps": the two kernels sum a row in different orders, and with a row-count threshold of 592 a 430-token prompt alone
-  // was normalised by one kernel and the same prompt inside a batch by the other -- last-bit differences that flipped near-tie tokens
-  // (tests/test_gpu_eval_drivers.py).  At <= 32 rows both the single and the batched call are decode steps.
-  if (rows <= 32 && nvec <= 512) {
+  if (kernel == NORM_BLOCK) {
     if (nvec <= 256) launch_k(rownorm_block_kernel<1, RMS>, dim3(rows), dim3(256), 0, s, x, ldx, g, b, y, ldy, cols, eps);
     else launch_k(rownorm_block_kernel<2, RMS>, dim3(rows), dim3(256), 0, s, x, ldx, g, b, y, ldy, cols, eps);
     FO1_LAUNCH_CHECK();
@@ -196,12 +194,29 @@ static int launch_rownorm(const bf16* x, long long ldx, const bf16* g, const bf1
   return FO1_ERR_UNSUPPORTED;
 }
 
-int rmsnorm(const bf16* x, long long ldx, const bf16* w, bf16* y, long long ldy, int rows, int cols, float eps, cudaStream_t s) {
-  return launch_rownorm<true>(x, ldx, w, nullptr, y, ldy, rows, cols, eps, s);
+int rmsnorm(const bf16* x, long long ldx, const bf16* w, bf16* y, long long ldy, int rows, int cols, float eps, NormKernel kernel,
+            cudaStream_t s) {
+  return launch_rownorm<true>(x, ldx, w, nullptr, y, ldy, rows, cols, eps, kernel, s);
 }
 int layernorm(const bf16* x, long long ldx, const bf16* gamma, const bf16* beta, bf16* y, long long ldy, int rows, int cols,
-              float eps, cudaStream_t s) {
-  return launch_rownorm<false>(x, ldx, gamma, beta, y, ldy, rows, cols, eps, s);
+              float eps, NormKernel kernel, cudaStream_t s) {
+  return launch_rownorm<false>(x, ldx, gamma, beta, y, ldy, rows, cols, eps, kernel, s);
 }
 
 }  // namespace fo1
+
+extern "C" int fo1_row_norm(const void* x, int64_t ldx, const void* gamma, const void* beta, void* y, int64_t ldy, int32_t rows, int32_t cols,
+                            float eps, int32_t rms, int32_t kernel, void* stream) {
+  using namespace fo1;
+  FO1_CHECK_ARG(x && y && rows >= 0 && cols > 0 && ldx >= cols && ldy >= cols && (kernel == NORM_WARP || kernel == NORM_BLOCK),
+                "fo1_row_norm: bad argument");
+  FO1_CHECK_ARG(!rms || beta == nullptr, "fo1_row_norm: RMSNorm takes no beta");
+  FO1_CHECK_ARG(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(gamma) |
+                  reinterpret_cast<uintptr_t>(beta)) & 15) == 0,
+                "fo1_row_norm: pointers must be 16-byte aligned");
+  const bf16 *xb = static_cast<const bf16*>(x), *g = static_cast<const bf16*>(gamma), *b = static_cast<const bf16*>(beta);
+  const NormKernel k = static_cast<NormKernel>(kernel);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  return rms ? rmsnorm(xb, ldx, g, static_cast<bf16*>(y), ldy, rows, cols, eps, k, s)
+             : layernorm(xb, ldx, g, b, static_cast<bf16*>(y), ldy, rows, cols, eps, k, s);
+}

@@ -177,7 +177,7 @@ static int vit_forward_impl(Model* m, const float* const* pixel_values, const in
     const VitBlockW& b = w.blk[L];
     bool full = false;
     for (int i = 0; i < c.vit_n_fullatt; ++i) full |= (c.vit_fullatt[i] == L);
-    FO1_RUN(rmsnorm(x, H, b.norm1, xn, H, (int)T, H, 1e-6f, s));
+    FO1_RUN(rmsnorm(x, H, b.norm1, xn, H, (int)T, H, 1e-6f, NORM_WARP, s));
     FO1_RUN(linear(xn, H, b.qkv_w, H, qkv, 3 * H, FO1_BF16, (int)T, 3 * H, H, b.qkv_b, FO1_BF16, FO1_EPI_NONE, nullptr, 0, 0, s));
     FO1_RUN(vit_rope_apply(qkv, cs, (int)T, heads, hd, s));
     AttnArgs a;
@@ -195,7 +195,7 @@ static int vit_forward_impl(Model* m, const float* const* pixel_values, const in
     a.causal = 0;
     FO1_RUN(attention_varlen(a, s));
     FO1_RUN(linear(att, H, b.proj_w, H, x2, H, FO1_BF16, (int)T, H, H, b.proj_b, FO1_BF16, FO1_EPI_NONE, x, H, 0, s));
-    FO1_RUN(rmsnorm(x2, H, b.norm2, xn, H, (int)T, H, 1e-6f, s));
+    FO1_RUN(rmsnorm(x2, H, b.norm2, xn, H, (int)T, H, 1e-6f, NORM_WARP, s));
     FO1_RUN(linear(xn, H, b.gateup_w, H, hbuf, c.vit_inter_pad, FO1_BF16, (int)T, 2 * c.vit_inter_pad, H, b.gateup_b, FO1_BF16,
                    FO1_EPI_SILU, nullptr, 0, 1, s));
     FO1_RUN(linear(hbuf, c.vit_inter_pad, b.down_w, c.vit_inter_pad, x, H, FO1_BF16, (int)T, H, c.vit_inter_pad, b.down_b, FO1_BF16,
@@ -207,7 +207,7 @@ static int vit_forward_impl(Model* m, const float* const* pixel_values, const in
     if (full) ++tap_i;
   }
   // ---- merger (:146-159) + inverse window permutation (:155-156) ----
-  FO1_RUN(rmsnorm(x, H, w.ln_q, xn, H, (int)T, H, 1e-6f, s));
+  FO1_RUN(rmsnorm(x, H, w.ln_q, xn, H, (int)T, H, 1e-6f, NORM_WARP, s));
   const int M4 = H * unit;
   FO1_RUN(linear(xn, M4, w.fc1_w, M4, mg, M4, FO1_BF16, Tm, M4, M4, w.fc1_b, FO1_BF16, FO1_EPI_GELU, nullptr, 0, 0, s));
   FO1_RUN(linear(mg, M4, w.fc2_w, M4, mo, c.vit_out_hidden, FO1_BF16, Tm, c.vit_out_hidden, M4, w.fc2_b, FO1_BF16, FO1_EPI_NONE,

@@ -127,6 +127,31 @@ def dwconv3x3_residual(x: torch.Tensor, w9: torch.Tensor, bias: torch.Tensor) ->
     return y
 
 
+NORM_WARP, NORM_BLOCK = 0, 1      # fo1_row_norm's kernel: one warp per row / one block per row
+
+
+def row_norm(x: torch.Tensor, gamma: Optional[torch.Tensor], beta: Optional[torch.Tensor], eps: float, rms: bool, kernel: int,
+             out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """RMSNorm (``rms``; beta None) or LayerNorm of the rows of x bf16 [rows, cols] (any row pitch, unit column stride) with the named
+    kernel (fo1_row_norm).  ``out``: optional bf16 [rows, cols] view (any row pitch) written in place."""
+    _require_cuda(x, gamma, beta, out)
+    assert x.dtype == torch.bfloat16 and x.dim() == 2 and x.stride(1) == 1
+    rows, cols = x.shape
+    for t in (gamma, beta):
+        assert t is None or (t.dtype == torch.bfloat16 and tuple(t.shape) == (cols,) and t.is_contiguous())
+    if out is None:
+        out = torch.empty((rows, cols), dtype=torch.bfloat16, device=x.device)
+    assert out.dtype == torch.bfloat16 and tuple(out.shape) == (rows, cols) and out.stride(1) == 1
+    L = lib()
+    L.fo1_row_norm.restype = C.c_int
+    L.fo1_row_norm.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_float,
+                               C.c_int32, C.c_int32, C.c_void_p]
+    ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
+    check(L.fo1_row_norm(ptr(x), x.stride(0), ptr(gamma), ptr(beta), ptr(out), out.stride(0), rows, cols, eps, 1 if rms else 0, kernel,
+                         C.c_void_p(_stream())), "fo1_row_norm")
+    return out
+
+
 def channel_attention(qkv: torch.Tensor, groups: int) -> torch.Tensor:
     """DaViT channel-group attention: qkv bf16 [B, N, 3C] -> bf16 [B, N, C] (fo1_channel_attention)."""
     _require_cuda(qkv)
