@@ -188,6 +188,25 @@ typedef struct {
 size_t fo1_decode_attention_workspace_bytes(int32_t n_seqs, int32_t q_heads);
 int fo1_decode_attention(const fo1_decode_attn_desc* d, void* stream);
 
+/* Causal attention of a sequence's own rows against its K/V cache, the attention of fo1_llm_generate_prefixed: own row i of
+ * sequence b (query row own_off_b + i of q, own rows of the sequences packed in order) attends the cache keys 0 .. P_b + i of b.
+ * Its own K/V must already sit in the cache at row P_b + i.  Key tiles start at key 0 of the sequence, as in the full-sequence
+ * prefill, so each row's output is bit-identical to what fo1_attention_varlen (causal) gives that row over the whole sequence.
+ * The cache rows P_b + own_b .. up to the next multiple of 64 are read with weight zero and must hold finite values.
+ * head_dim 128.  Exposed so the kernel can be checked on its own. */
+typedef struct {
+  const void* q; int64_t ldq;        /* bf16 [sum own_b][ldq], rotated */
+  const void* k_cache;               /* bf16 [n_seqs][cap][kv_heads*head_dim] */
+  const void* v_cache;
+  int32_t n_seqs, cap;               /* cap: a multiple of 64 */
+  const int32_t* prefix_lens;        /* HOST [n_seqs]: P_b >= 0 */
+  const int32_t* own_lens;           /* HOST [n_seqs]: own_b >= 0, P_b + own_b <= cap */
+  int32_t q_heads, kv_heads, head_dim;
+  float scale;
+  void* out; int64_t ldo;            /* bf16 [sum own_b][ldo] */
+} fo1_prefix_attn_desc;
+int fo1_prefix_attention(const fo1_prefix_attn_desc* d, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Model-level engine.  One handle per GPU / rank; calls on one handle are not re-entrant.
  * Weights are BORROWED device pointers (the caller keeps them alive): the Python loader prepares
@@ -459,6 +478,29 @@ int fo1_llm_generate_streamed(fo1_model* m, fo1_generate_desc* d, const fo1_samp
  * cannot express the ordering (and for CPUs with a weaker memory model than x86). */
 int32_t fo1_stream_progress(const int32_t* progress);
 void fo1_stream_cancel(int32_t* cancel);
+
+/* ------------------------------------------------------------------------------------------------
+ * Shared-prefix prefill (many questions about one image).  Sequences of a group start with the same P_g rows (same embeddings,
+ * same M-RoPE positions).  Those rows are prefilled once: one causal segment per group, packed before the sequences' own rows
+ * through every layer, and their rotated K/V rows are written into the cache slot of every member at rows 0 .. P_g - 1.  The
+ * remaining "own" rows of each sequence attend its cache (fo1_prefix_attention).  Decode is unchanged: each sequence owns a full
+ * copy of its prefix K/V.  Every output (tokens, lengths, prefill logits, scores, logits, streamed columns) is bit-identical to
+ * fo1_llm_generate_streamed on the full sequences.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct {
+  int32_t n_groups;
+  const int32_t* prefix_lens;          /* HOST [n_groups]: P_g >= 1 */
+  const void* prefix_embeds;           /* DEVICE bf16 [sum P_g][llm_hidden], groups back to back */
+  const int32_t* prefix_position_ids;  /* DEVICE int32 [3][sum P_g] */
+  const int32_t* seq_group;            /* HOST [n_seqs]: the sequence's group, or -1 (no shared prefix) */
+} fo1_prefix_desc;
+/* fo1_llm_generate_streamed with shared prefixes.  In d, seq_lens stays the full length L_b; inputs_embeds / position_ids hold
+ * only each sequence's own rows (L_b - P_g, or L_b without a group), packed in sequence order.  px == NULL or n_groups == 0 is
+ * exactly fo1_llm_generate_streamed.  Checked on the host before any CUDA call: group indices in range, at least two members
+ * per group, P_g < L_b for every member, non-NULL pointers, and no all_logits. */
+int fo1_llm_generate_prefixed(fo1_model* m, fo1_generate_desc* d, const fo1_prefix_desc* px, const fo1_sampling_desc* sp /* NULL: greedy */,
+                              const fo1_score_desc* sc /* NULL: unscored */, const fo1_stream_desc* st /* NULL: not streamed */,
+                              void* stream);
 
 #ifdef __cplusplus
 }

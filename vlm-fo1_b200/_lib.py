@@ -81,6 +81,18 @@ class StreamDesc(C.Structure):
     _fields_ = [("tokens", C.c_void_p), ("lens", C.c_void_p), ("progress", C.c_void_p), ("cancel", C.c_void_p)]
 
 
+class PrefixDesc(C.Structure):
+    """fo1_prefix_desc: HOST prefix_lens [n_groups], seq_group [n_seqs]; DEVICE prefix_embeds bf16 [sum P][hidden], position ids [3][sum P]."""
+    _fields_ = [("n_groups", C.c_int32), ("prefix_lens", C.POINTER(C.c_int32)), ("prefix_embeds", C.c_void_p),
+                ("prefix_position_ids", C.c_void_p), ("seq_group", C.POINTER(C.c_int32))]
+
+
+class PrefixAttnDesc(C.Structure):
+    _fields_ = [("q", C.c_void_p), ("ldq", C.c_int64), ("k_cache", C.c_void_p), ("v_cache", C.c_void_p), ("n_seqs", C.c_int32),
+                ("cap", C.c_int32), ("prefix_lens", C.POINTER(C.c_int32)), ("own_lens", C.POINTER(C.c_int32)), ("q_heads", C.c_int32),
+                ("kv_heads", C.c_int32), ("head_dim", C.c_int32), ("scale", C.c_float), ("out", C.c_void_p), ("ldo", C.c_int64)]
+
+
 FO1_STREAM_DONE = 1 << 30
 
 _lib = None
@@ -126,6 +138,11 @@ def lib() -> C.CDLL:
     L.fo1_llm_generate_streamed.restype = C.c_int
     L.fo1_llm_generate_streamed.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(SamplingDesc), C.POINTER(ScoreDesc), C.POINTER(StreamDesc),
                                             C.c_void_p]
+    L.fo1_llm_generate_prefixed.restype = C.c_int
+    L.fo1_llm_generate_prefixed.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(PrefixDesc), C.POINTER(SamplingDesc), C.POINTER(ScoreDesc),
+                                            C.POINTER(StreamDesc), C.c_void_p]
+    L.fo1_prefix_attention.restype = C.c_int
+    L.fo1_prefix_attention.argtypes = [C.POINTER(PrefixAttnDesc), C.c_void_p]
     L.fo1_stream_progress.restype = C.c_int32
     L.fo1_stream_progress.argtypes = [C.c_void_p]
     L.fo1_stream_cancel.restype = None

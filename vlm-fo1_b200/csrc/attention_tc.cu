@@ -388,6 +388,20 @@ void attention_tile_table(const std::vector<int>& group_cu, std::vector<int>& ti
     }
 }
 
+// The key range of an own row starts at key 0 of its sequence, so its 64-key tiles have the alignment of the full-sequence prefill (whose
+// range starts at the segment start); tiles past a row's diagonal are fully masked and add exact zeros.  That makes each own row's output
+// bit-identical to the full prefill's, whatever the query tiling.
+void prefix_attention_tables(const int* prefix, const int* own, int n_seqs, int cap, std::vector<int>& rowseg, std::vector<int>& tiles) {
+  rowseg.clear();
+  std::vector<int> cu(1, 0);
+  for (int b = 0; b < n_seqs; ++b) {
+    const int base = b * cap;
+    for (int i = 0; i < own[b]; ++i) { rowseg.push_back(base); rowseg.push_back(base + prefix[b] + i + 1); }
+    cu.push_back(cu.back() + own[b]);
+  }
+  attention_tile_table(cu, tiles);
+}
+
 int attention_rowseg(const int* cu_seqlens, int n_seqs, int T, int* rowseg /*[T][2]*/, cudaStream_t s) {
   if (T <= 0) return FO1_OK;
   attn_rowseg_kernel<<<ceil_div(T, 256), 256, 0, s>>>(cu_seqlens, n_seqs, T, reinterpret_cast<int2*>(rowseg));
@@ -404,10 +418,11 @@ static int launch_attn_tc(const AttnArgs& a, const int2* rowseg, cudaStream_t s)
     attr_set = true;
   }
   const int T = a.total_rows;
+  const int kv_rows = a.kv_rows > 0 ? a.kv_rows : T;
   CUtensorMap tmQ, tmK, tmV;
   FO1_TRY(make_tmap_3d_bf16(&tmQ, a.q, HD, a.q_heads, T, (uint64_t)HD * 2, (uint64_t)a.ldq * 2, 64, 1, kAtM));
-  FO1_TRY(make_tmap_3d_bf16(&tmK, a.k, HD, a.kv_heads, T, (uint64_t)HD * 2, (uint64_t)a.ldk * 2, 64, 1, kAtN));
-  FO1_TRY(make_tmap_3d_bf16(&tmV, a.v, HD, a.kv_heads, T, (uint64_t)HD * 2, (uint64_t)a.ldv * 2, 64, 1, kAtN));
+  FO1_TRY(make_tmap_3d_bf16(&tmK, a.k, HD, a.kv_heads, kv_rows, (uint64_t)HD * 2, (uint64_t)a.ldk * 2, 64, 1, kAtN));
+  FO1_TRY(make_tmap_3d_bf16(&tmV, a.v, HD, a.kv_heads, kv_rows, (uint64_t)HD * 2, (uint64_t)a.ldv * 2, 64, 1, kAtN));
   AttnTcArgs g;
   g.o = a.o; g.ldo = a.ldo; g.rowseg = rowseg; g.T = T; g.q_heads = a.q_heads; g.kv_heads = a.kv_heads;
   g.tiles = reinterpret_cast<const int2*>(a.tiles);
@@ -415,12 +430,13 @@ static int launch_attn_tc(const AttnArgs& a, const int2* rowseg, cudaStream_t s)
   const long long blocks = (long long)(a.tiles != nullptr ? a.n_tiles : ceil_div(T, kAtM)) * a.q_heads;
   FO1_CHECK_ARG(blocks < (1ll << 31), "attention: grid too large (%lld blocks)", blocks);
   g.n_work = (int)blocks;
-  ProfScope prof(CAUSAL ? "attn_causal" : "attn", a.flops, 0.0, s);
+  ProfScope prof(CAUSAL ? "attn_causal" : a.kv_rows > 0 ? "attn_prefix" : "attn", a.flops, 0.0, s);
   // persistent for the non-causal shapes (equal-cost items): one CTA per SM walks the item list.  Causal prompts have items of very
   // different cost, which a static round robin balances badly, so they keep one CTA per item (the same kernel with a one-item
-  // list) and leave the balancing to the hardware block scheduler.  FO1_ATTN_ONE_ITEM: A/B knob.
+  // list) and leave the balancing to the hardware block scheduler; so do the causal ranges of a cache-reading call.  FO1_ATTN_ONE_ITEM:
+  // A/B knob.
   const long long resident = device_sm_count();
-  const unsigned grid = (unsigned)((CAUSAL || getenv("FO1_ATTN_ONE_ITEM") != nullptr || blocks < resident) ? blocks : resident);
+  const unsigned grid = (unsigned)((CAUSAL || a.kv_rows > 0 || getenv("FO1_ATTN_ONE_ITEM") != nullptr || blocks < resident) ? blocks : resident);
   attn_tc_kernel<HD, CAUSAL><<<grid, kAtThreads, Cfg::kSmemBytes, s>>>(tmQ, tmK, tmV, g);
   FO1_LAUNCH_CHECK();
   return FO1_OK;
@@ -432,6 +448,7 @@ int attention_varlen(const AttnArgs& a, cudaStream_t s) {
   FO1_CHECK_ARG((a.ldq % 8) == 0 && (a.ldk % 8) == 0 && (a.ldv % 8) == 0 && (a.ldo % 8) == 0, "attention: pitches must be multiples of 8");
   FO1_CHECK_ARG(((reinterpret_cast<uintptr_t>(a.q) | reinterpret_cast<uintptr_t>(a.k) | reinterpret_cast<uintptr_t>(a.v) |
                   reinterpret_cast<uintptr_t>(a.o)) & 15) == 0, "attention: q / k / v / o must be 16-byte aligned");
+  FO1_CHECK_ARG(a.kv_rows == 0 || (a.rowseg != nullptr && !a.causal), "attention: a K/V-cache call takes a rowseg table and is not causal by row");
   if (a.n_seqs == 0 || a.total_rows <= 0) return FO1_OK;
   const int2* rowseg = reinterpret_cast<const int2*>(a.rowseg);
   if (rowseg == nullptr) {
@@ -465,4 +482,42 @@ extern "C" int fo1_attention_varlen(const fo1_attn_desc* d, void* stream) {
   a.q_heads = d->q_heads; a.kv_heads = d->kv_heads; a.head_dim = d->head_dim;
   a.scale = d->scale; a.causal = d->causal; a.flops = 0.0;
   return attention_varlen(a, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int fo1_prefix_attention(const fo1_prefix_attn_desc* d, void* stream) {
+  using namespace fo1;
+  FO1_CHECK_ARG(d != nullptr, "fo1_prefix_attention: null descriptor");
+  FO1_CHECK_ARG(d->n_seqs >= 0 && d->cap > 0 && d->cap % kAtN == 0, "fo1_prefix_attention: n_seqs %d / cap %d (a positive multiple of 64)",
+                d->n_seqs, d->cap);
+  if (d->n_seqs == 0) return FO1_OK;
+  FO1_CHECK_ARG(d->q && d->k_cache && d->v_cache && d->out && d->prefix_lens && d->own_lens, "fo1_prefix_attention: null pointer");
+  FO1_CHECK_ARG(d->head_dim == 128, "fo1_prefix_attention: head_dim %d unsupported (128)", d->head_dim);
+  FO1_CHECK_ARG((long long)d->n_seqs * d->cap < (1ll << 31), "fo1_prefix_attention: cache rows overflow");
+  long long T = 0;
+  for (int b = 0; b < d->n_seqs; ++b) {
+    FO1_CHECK_ARG(d->prefix_lens[b] >= 0 && d->own_lens[b] >= 0 && d->prefix_lens[b] + d->own_lens[b] <= d->cap,
+                  "fo1_prefix_attention: sequence %d: prefix %d + own %d rows exceed cap %d", b, d->prefix_lens[b], d->own_lens[b], d->cap);
+    T += d->own_lens[b];
+  }
+  if (T == 0) return FO1_OK;
+  std::vector<int> rowseg, tiles;
+  prefix_attention_tables(d->prefix_lens, d->own_lens, d->n_seqs, d->cap, rowseg, tiles);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int* dev = nullptr;
+  FO1_CUDA(cudaMalloc(reinterpret_cast<void**>(&dev), (rowseg.size() + tiles.size()) * sizeof(int)));
+  FO1_CUDA(cudaMemcpyAsync(dev, rowseg.data(), rowseg.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  FO1_CUDA(cudaMemcpyAsync(dev + rowseg.size(), tiles.data(), tiles.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  const int KD = d->kv_heads * d->head_dim;
+  AttnArgs a;
+  a.q = static_cast<const bf16*>(d->q); a.k = static_cast<const bf16*>(d->k_cache); a.v = static_cast<const bf16*>(d->v_cache);
+  a.o = static_cast<bf16*>(d->out);
+  a.ldq = d->ldq; a.ldk = a.ldv = KD; a.ldo = d->ldo;
+  a.cu_seqlens = nullptr; a.rowseg = dev; a.tiles = dev + rowseg.size(); a.n_tiles = (int)tiles.size() / 2;
+  a.n_seqs = d->n_seqs; a.total_rows = (int)T; a.max_seqlen = 0;
+  a.q_heads = d->q_heads; a.kv_heads = d->kv_heads; a.head_dim = d->head_dim; a.scale = d->scale; a.causal = 0;
+  a.kv_rows = d->n_seqs * d->cap;
+  const int rc = attention_varlen(a, s);
+  cudaStreamSynchronize(s);          // the tables are this call's
+  cudaFree(dev);
+  return rc;
 }

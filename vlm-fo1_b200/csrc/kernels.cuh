@@ -63,12 +63,17 @@ struct AttnArgs {
   float scale;
   int causal;
   double flops = 0.0;               // algorithmic FLOPs of the call for the optional profiler (4 * sum len^2 * hd * heads, / 2 causal)
+  int kv_rows = 0;                  // > 0: k / v are a K/V cache of kv_rows rows, addressed by the rowseg table (which is then required),
+                                    //   and the call is not causal by row index: each row's rowseg range is its causal key range
 };
 int attention_varlen(const AttnArgs& a, cudaStream_t s);
 // (lo, hi) key range of every packed row: callers that reuse one cu_seqlens for many layers build it once
 int attention_rowseg(const int* cu_seqlens, int n_seqs, int T, int* rowseg, cudaStream_t s);
 // host helper: 128-row query tiles that restart at every group boundary (image / prompt) -> flat (row0, rows) pairs
 void attention_tile_table(const std::vector<int>& group_cu, std::vector<int>& tiles);
+// host helper of the cache-reading attention: own row i of sequence b (own rows packed in sequence order) sees the cache rows
+// [b * cap, b * cap + prefix[b] + i + 1) -> flat (lo, hi) pairs, and the query tiles restarting at every sequence's own rows
+void prefix_attention_tables(const int* prefix, const int* own, int n_seqs, int cap, std::vector<int>& rowseg, std::vector<int>& tiles);
 
 // ---- misc.cu ----
 int cast_gather_rows_f32_bf16(const float* src, long long lds, const int* row_idx, bf16* dst, long long ldd, int rows, int cols, cudaStream_t s);

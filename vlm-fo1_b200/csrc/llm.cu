@@ -51,6 +51,31 @@ __global__ void __launch_bounds__(128) kv_store_kernel(const bf16* __restrict__ 
     *reinterpret_cast<uint4*>(vc + slot + c) = *reinterpret_cast<const uint4*>(kp + kv_dim + c);
   }
 }
+// shared-prefix prefill: copy the rotated K and V of prefix row r (position row_gt[r].y of group row_gt[r].x) into the cache slot of
+// every member of the group (members[grp_off[g] .. grp_off[g + 1]))
+__global__ void __launch_bounds__(64) kv_fanout_kernel(const bf16* __restrict__ qkv, long long ld, int q_dim, int kv_dim,
+                                                       const int2* __restrict__ row_gt, const int* __restrict__ grp_off,
+                                                       const int* __restrict__ members, bf16* __restrict__ kc, bf16* __restrict__ vc, int cap) {
+  const int r = blockIdx.x;
+  const int2 gt = row_gt[r];
+  const int m0 = grp_off[gt.x], m1 = grp_off[gt.x + 1];
+  const bf16* kp = qkv + (long long)r * ld + q_dim;            // K | V are contiguous in the packed row
+  for (int c = threadIdx.x * 8; c < 2 * kv_dim; c += blockDim.x * 8) {
+    const uint4 val = *reinterpret_cast<const uint4*>(kp + c);
+    bf16* dst = c < kv_dim ? kc + c : vc + (c - kv_dim);
+    for (int i = m0; i < m1; ++i) *reinterpret_cast<uint4*>(dst + ((long long)members[i] * cap + gt.y) * kv_dim) = val;
+  }
+}
+// shared-prefix prefill: zero the V rows [L_b, L_b rounded up to 64) of every sequence in every layer.  The last 64-key tile of the
+// cache-reading attention reads them with weight zero, which a non-finite leftover would turn into NaN; decode overwrites them.
+__global__ void __launch_bounds__(128) kv_zero_tail_kernel(bf16* __restrict__ vc, long long layer_stride, const int* __restrict__ seq_lens,
+                                                           int cap, int kv_dim) {
+  const int b = blockIdx.x;
+  const int t0 = seq_lens[b], t1 = min(cap, (t0 + 63) & ~63);
+  bf16* base = vc + blockIdx.y * layer_stride + (long long)b * cap * kv_dim;
+  for (long long c = (long long)t0 * kv_dim + threadIdx.x * 8; c < (long long)t1 * kv_dim; c += blockDim.x * 8)
+    *reinterpret_cast<uint4*>(base + c) = make_uint4(0u, 0u, 0u, 0u);
+}
 // Single-query GQA attention over the cache, split over the sequence (flash-decoding) and run on the tensor pipe:
 // one block per (sequence, kv head, split).  The G <= 8 query heads of the kv head are the rows of an m16n8k16 tile
 // (rows G..15 are zero), so K and V are read ONCE per kv head instead of once per query head.  Every warp owns
@@ -433,9 +458,51 @@ static int ensure_state(Model* m, int B, int n_stop, DecodeState* st) {
 // size; the width alone decides for models wider than it serves
 static NormKernel seq_norm_kernel(int H) { return H <= kNormBlockMaxCols ? NORM_BLOCK : NORM_WARP; }
 
+// device tables of a shared-prefix prefill: the packed rows are the groups' prefix rows (one causal segment per group), then every
+// sequence's own rows
+struct PrefixTables {
+  int n_pre = 0, n_groups = 0;
+  const int *cu = nullptr, *tiles = nullptr;                  // prefix segments and their query tiles
+  int n_tiles = 0;
+  const int *row_gt = nullptr, *grp_off = nullptr, *members = nullptr;   // kv_fanout_kernel
+  const int *own_seq = nullptr, *own_t = nullptr;             // kv_store_kernel of the own rows
+  const int *own_rowseg = nullptr, *own_tiles = nullptr;      // the cache-reading attention of the own rows
+  int n_own_tiles = 0;
+};
+
 // one decoder layer over `rows` packed rows.  x_in -> x_out (x_mid scratch).  prefill: varlen causal attention
-// + cache fill; decode: cache append + single-query attention.
-struct LayerBuf { bf16 *xn, *qkv, *att, *x_mid, *h; float* dec_part; int* rowseg = nullptr; double attn_flops = 0.0; const int* tiles = nullptr; int n_tiles = 0; };
+// + cache fill (px: the shared-prefix split of it); decode: cache append + single-query attention.
+struct LayerBuf { bf16 *xn, *qkv, *att, *x_mid, *h; float* dec_part; int* rowseg = nullptr; double attn_flops = 0.0; const int* tiles = nullptr; int n_tiles = 0;
+                  const PrefixTables* px = nullptr; };
+
+// the prefill attention of a shared-prefix layer: prefix K/V into every member's slot, own K/V into the own slot, then the prefix rows
+// as causal segments and the own rows against the cache
+static int prefix_layer_attention(Model* m, const LayerBuf& B_, int rows, bf16* kc, bf16* vc, cudaStream_t s, bool dry) {
+  const fo1_model_config& c = m->cfg;
+  const PrefixTables& p = *B_.px;
+  const int hd = c.llm_head_dim, QD = c.llm_heads * hd, KD = c.llm_kv_heads * hd, ldq = QD + 2 * KD;
+  const int np = p.n_pre, no = rows - np;
+  if (!dry) {
+    kv_fanout_kernel<<<np, 64, 0, s>>>(B_.qkv, ldq, QD, KD, reinterpret_cast<const int2*>(p.row_gt), p.grp_off, p.members, kc, vc, m->kv_cap);
+    FO1_LAUNCH_CHECK();
+    kv_store_kernel<<<no, 128, 0, s>>>(B_.qkv + (size_t)np * ldq, ldq, QD, KD, p.own_seq, p.own_t, kc, vc, m->kv_cap);
+    FO1_LAUNCH_CHECK();
+  }
+  AttnArgs a;
+  a.q = B_.qkv; a.k = B_.qkv + QD; a.v = B_.qkv + QD + KD; a.o = B_.att;
+  a.ldq = a.ldk = a.ldv = ldq; a.ldo = QD;
+  a.cu_seqlens = p.cu; a.n_seqs = p.n_groups; a.max_seqlen = 0; a.total_rows = np; a.rowseg = B_.rowseg; a.tiles = p.tiles; a.n_tiles = p.n_tiles;
+  a.q_heads = c.llm_heads; a.kv_heads = c.llm_kv_heads; a.head_dim = hd;
+  a.scale = 1.0f / sqrtf((float)hd); a.causal = 1;
+  FO1_RUN(attention_varlen(a, s));
+  AttnArgs o = a;
+  o.q = B_.qkv + (size_t)np * ldq; o.k = kc; o.v = vc; o.o = B_.att + (size_t)np * QD;
+  o.ldk = o.ldv = KD;
+  o.cu_seqlens = nullptr; o.n_seqs = m->kv_batch; o.total_rows = no; o.rowseg = p.own_rowseg; o.tiles = p.own_tiles; o.n_tiles = p.n_own_tiles;
+  o.causal = 0; o.kv_rows = m->kv_batch * m->kv_cap;
+  FO1_RUN(attention_varlen(o, s));
+  return FO1_OK;
+}
 
 static int llm_layer(Model* m, int li, const bf16* x_in, bf16* x_out, const LayerBuf& B_, int rows, const float* cs, bool prefill,
                      const int* d_cu, int n_seqs, int max_len, const int* d_row_seq, const int* d_row_t, const DecodeState* st,
@@ -450,7 +517,10 @@ static int llm_layer(Model* m, int li, const bf16* x_in, bf16* x_out, const Laye
   const NormKernel nk = prefill ? NORM_WARP : seq_norm_kernel(H);
   FO1_RUN(rmsnorm(x_in, H, L.ln1, B_.xn, H, rows, H, c.rms_eps, nk, s));
   FO1_RUN(linear(B_.xn, H, L.qkv_w, H, B_.qkv, ldq, FO1_BF16, rows, ldq, H, L.qkv_b, FO1_BF16, FO1_EPI_NONE, nullptr, 0, 0, s));
-  if (prefill) {
+  if (prefill && B_.px != nullptr) {
+    FO1_RUN(rope_apply(B_.qkv, ldq, cs, rows, c.llm_heads + c.llm_kv_heads, hd, s));
+    FO1_TRY(prefix_layer_attention(m, B_, rows, kc, vc, s, dry));
+  } else if (prefill) {
     FO1_RUN(rope_apply(B_.qkv, ldq, cs, rows, c.llm_heads + c.llm_kv_heads, hd, s));   // q|k heads are contiguous in the packed row
     if (!dry) {
       kv_store_kernel<<<rows, 128, 0, s>>>(B_.qkv, ldq, QD, KD, d_row_seq, d_row_t, kc, vc, m->kv_cap);
@@ -506,16 +576,55 @@ static int decode_column(DecodeMode mode, const DecodeBufs& g, const ColumnSink&
 }
 
 // buffer plan, integer tables and the prefill; then (unless `dry`, the pass that sizes the arena) the decode state and column 0
-static int llm_prefill(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, const fo1_score_desc* sc, DecodeMode mode,
-                       const ColumnSink& k, cudaStream_t s, bool dry, DecodeBufs& g) {
+// the own rows of sequence b in a shared-prefix prefill (L_b without a group)
+static int prefix_of(const fo1_prefix_desc* px, int b) { return px && px->seq_group[b] >= 0 ? px->prefix_lens[px->seq_group[b]] : 0; }
+
+// host and device tables of a shared-prefix prefill (PrefixTables); n_pre: sum P_g
+static int prefix_tables(Model* m, const fo1_generate_desc* d, const fo1_prefix_desc* px, int n_pre, PrefixTables& p, cudaStream_t s) {
+  const int B = d->n_seqs, G = px->n_groups;
+  p.n_pre = n_pre; p.n_groups = G;
+  std::vector<int> cu(1, 0), row_gt, grp_off(1, 0), members, own_seq, own_t, pre(B), own(B), rowseg, tiles;
+  std::string key = "llmpx:" + std::to_string(m->kv_cap);
+  for (int g = 0; g < G; ++g) {
+    cu.push_back(cu.back() + px->prefix_lens[g]);
+    for (int t = 0; t < px->prefix_lens[g]; ++t) { row_gt.push_back(g); row_gt.push_back(t); }
+    for (int b = 0; b < B; ++b) if (px->seq_group[b] == g) members.push_back(b);
+    grp_off.push_back((int)members.size());
+    key += ":" + std::to_string(px->prefix_lens[g]);
+  }
+  for (int b = 0; b < B; ++b) {
+    pre[b] = prefix_of(px, b); own[b] = d->seq_lens[b] - pre[b];
+    for (int i = 0; i < own[b]; ++i) { own_seq.push_back(b); own_t.push_back(pre[b] + i); }
+    key += "/" + std::to_string(px->seq_group[b]) + ":" + std::to_string(d->seq_lens[b]);
+  }
+  FO1_TRY(cached_ints(m, key + ":cu", cu, &p.cu, s));
+  attention_tile_table(cu, tiles);
+  p.n_tiles = (int)tiles.size() / 2;
+  FO1_TRY(cached_ints(m, key + ":til", tiles, &p.tiles, s));
+  FO1_TRY(cached_ints(m, key + ":gt", row_gt, &p.row_gt, s));
+  FO1_TRY(cached_ints(m, key + ":go", grp_off, &p.grp_off, s));
+  FO1_TRY(cached_ints(m, key + ":mem", members, &p.members, s));
+  FO1_TRY(cached_ints(m, key + ":os", own_seq, &p.own_seq, s));
+  FO1_TRY(cached_ints(m, key + ":ot", own_t, &p.own_t, s));
+  prefix_attention_tables(pre.data(), own.data(), B, m->kv_cap, rowseg, tiles);
+  p.n_own_tiles = (int)tiles.size() / 2;
+  FO1_TRY(cached_ints(m, key + ":ors", rowseg, &p.own_rowseg, s));
+  FO1_TRY(cached_ints(m, key + ":otil", tiles, &p.own_tiles, s));
+  return FO1_OK;
+}
+
+static int llm_prefill(Model* m, fo1_generate_desc* d, const fo1_prefix_desc* px, const fo1_sampling_desc* sp, const fo1_score_desc* sc,
+                       DecodeMode mode, const ColumnSink& k, cudaStream_t s, bool dry, DecodeBufs& g) {
   const fo1_model_config& c = m->cfg;
   Arena& A = m->arena;
   const int B = d->n_seqs, H = c.llm_hidden, hd = c.llm_head_dim, V = c.llm_vocab;
   const int QD = c.llm_heads * hd, KD = c.llm_kv_heads * hd, ldq = QD + 2 * KD;
   const int Ip = (c.llm_inter + 31) / 32 * 32;
-  long long T = 0;
-  int max_len = 0;
-  for (int b = 0; b < B; ++b) { T += d->seq_lens[b]; max_len = std::max(max_len, d->seq_lens[b]); }
+  long long T = 0;      // packed rows through the layers: every sequence's rows, or (px) the prefix rows then the own rows
+  int max_len = 0, n_pre = 0;
+  for (int b = 0; b < B; ++b) { T += d->seq_lens[b] - prefix_of(px, b); max_len = std::max(max_len, d->seq_lens[b]); }
+  for (int gi = 0; px && gi < px->n_groups; ++gi) n_pre += px->prefix_lens[gi];
+  T += n_pre;
   const int R = (int)std::max<long long>(T, B);
 
   g = DecodeBufs();
@@ -538,6 +647,7 @@ static int llm_prefill(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* 
   bf16* alln = d->all_logits ? A.alloc<bf16>((size_t)T * H) : nullptr;
   int* d_lens = A.alloc<int>(B);
   int* d_deltas = A.alloc<int>(B);
+  int* pos_all = px ? A.alloc<int>((size_t)3 * T) : nullptr;      // prefix positions, then the own rows'
   // persistent decode kernel (decode_mega.cu): per-CTA slots + the grid barrier
   // the persistent kernel serves every batch it supports (1..32 sequences; scripts/mega_prof.py times the two paths alternately).
   // FO1_MEGA_MAX_B lowers the threshold, FO1_NO_MEGA disables the kernel.
@@ -554,23 +664,35 @@ static int llm_prefill(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* 
 
   // ---- integer tables of the packed batch ----
   const int *d_cu = nullptr, *d_row_seq = nullptr, *d_row_t = nullptr, *d_last = nullptr;
+  PrefixTables ptab;
+  if (!dry && px) {
+    FO1_TRY(prefix_tables(m, d, px, n_pre, ptab, s));
+    std::vector<int> lastrow;
+    int r = n_pre;
+    std::string key = "llmpx";
+    for (int b = 0; b < B; ++b) { r += d->seq_lens[b] - prefix_of(px, b); lastrow.push_back(r - 1); key += ":" + std::to_string(r); }
+    FO1_TRY(cached_ints(m, key + ":last", lastrow, &d_last, s));
+  }
+  if (px) buf.px = &ptab;
   if (!dry) {
     std::vector<int> cu(1, 0), row_seq, row_t, lastrow;
     std::string key = "llm";
-    for (int b = 0; b < B; ++b) {
+    for (int b = 0; b < B && !px; ++b) {
       for (int t = 0; t < d->seq_lens[b]; ++t) { row_seq.push_back(b); row_t.push_back(t); }
       cu.push_back(cu.back() + d->seq_lens[b]);
       lastrow.push_back(cu.back() - 1);
       key += ":" + std::to_string(d->seq_lens[b]);
     }
-    FO1_TRY(cached_ints(m, key + ":cu", cu, &d_cu, s));
-    FO1_TRY(cached_ints(m, key + ":rs", row_seq, &d_row_seq, s));
-    FO1_TRY(cached_ints(m, key + ":rt", row_t, &d_row_t, s));
-    FO1_TRY(cached_ints(m, key + ":last", lastrow, &d_last, s));
-    std::vector<int> tiles;
-    attention_tile_table(cu, tiles);        // query tiles restart at every prompt
-    FO1_TRY(cached_ints(m, key + ":til", tiles, &buf.tiles, s));
-    buf.n_tiles = (int)tiles.size() / 2;
+    if (!px) {
+      FO1_TRY(cached_ints(m, key + ":cu", cu, &d_cu, s));
+      FO1_TRY(cached_ints(m, key + ":rs", row_seq, &d_row_seq, s));
+      FO1_TRY(cached_ints(m, key + ":rt", row_t, &d_row_t, s));
+      FO1_TRY(cached_ints(m, key + ":last", lastrow, &d_last, s));
+      std::vector<int> tiles;
+      attention_tile_table(cu, tiles);        // query tiles restart at every prompt
+      FO1_TRY(cached_ints(m, key + ":til", tiles, &buf.tiles, s));
+      buf.n_tiles = (int)tiles.size() / 2;
+    }
     FO1_CUDA(cudaMemcpyAsync(d_lens, d->seq_lens, B * sizeof(int), cudaMemcpyHostToDevice, s));
     if (d->rope_deltas_device != nullptr) FO1_CUDA(cudaMemcpyAsync(d_deltas, d->rope_deltas_device, B * sizeof(int), cudaMemcpyDeviceToDevice, s));
     else FO1_CUDA(cudaMemcpyAsync(d_deltas, d->rope_deltas, B * sizeof(int), cudaMemcpyHostToDevice, s));
@@ -584,9 +706,29 @@ static int llm_prefill(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* 
   }
 
   // ---- prefill ----
-  FO1_RUN(attention_rowseg(d_cu, B, (int)T, buf.rowseg, s));
   const bf16* x = static_cast<const bf16*>(d->inputs_embeds);
-  FO1_RUN(mrope_table(d->position_ids, cs_pre, (int)T, hd, c.mrope_section[0], c.mrope_section[1], c.mrope_section[2], c.rope_theta, s));
+  const int* pos = d->position_ids;
+  if (px) {   // one packed matrix (prefix rows, then own rows) and one position table; rowseg of the prefix segments
+    const size_t no = (size_t)T - n_pre;
+    FO1_RUN(attention_rowseg(ptab.cu, px->n_groups, n_pre, buf.rowseg, s));
+    if (!dry) {
+      FO1_CUDA(cudaMemcpyAsync(g.xb, px->prefix_embeds, (size_t)n_pre * H * sizeof(bf16), cudaMemcpyDeviceToDevice, s));
+      FO1_CUDA(cudaMemcpyAsync(g.xb + (size_t)n_pre * H, d->inputs_embeds, no * H * sizeof(bf16), cudaMemcpyDeviceToDevice, s));
+      FO1_CUDA(cudaMemcpy2DAsync(pos_all, (size_t)T * sizeof(int), px->prefix_position_ids, (size_t)n_pre * sizeof(int), (size_t)n_pre * sizeof(int),
+                                 3, cudaMemcpyDeviceToDevice, s));
+      FO1_CUDA(cudaMemcpy2DAsync(pos_all + n_pre, (size_t)T * sizeof(int), d->position_ids, no * sizeof(int), no * sizeof(int), 3,
+                                 cudaMemcpyDeviceToDevice, s));
+      const size_t layer_stride = (size_t)m->kv_batch * m->kv_cap * KD;
+      kv_zero_tail_kernel<<<dim3(B, c.llm_layers), 128, 0, s>>>(static_cast<bf16*>(m->kv_cache) + (size_t)c.llm_layers * layer_stride,
+                                                                 (long long)layer_stride, d_lens, m->kv_cap, KD);
+      FO1_LAUNCH_CHECK();
+    }
+    x = g.xb;
+    pos = pos_all;
+  } else {
+    FO1_RUN(attention_rowseg(d_cu, B, (int)T, buf.rowseg, s));
+  }
+  FO1_RUN(mrope_table(pos, cs_pre, (int)T, hd, c.mrope_section[0], c.mrope_section[1], c.mrope_section[2], c.rope_theta, s));
   for (int li = 0; li < c.llm_layers; ++li) {
     bf16* xo = (li & 1) ? g.xb : g.xa;
     FO1_TRY(llm_layer(m, li, x, xo, buf, (int)T, cs_pre, true, d_cu, B, max_len, d_row_seq, d_row_t, nullptr, s, dry));
@@ -731,8 +873,28 @@ static int stream_resolve(const fo1_stream_desc* h, StreamArgs* sa) {
   return FO1_OK;
 }
 
+// host checks of a shared-prefix call (fo1_llm_generate_prefixed): before the model or the device is touched
+static int prefix_check(const fo1_generate_desc* d, const fo1_prefix_desc* px) {
+  FO1_CHECK_ARG(px->n_groups > 0 && px->prefix_lens && px->prefix_embeds && px->prefix_position_ids && px->seq_group,
+                "fo1_llm_generate_prefixed: null prefix argument");
+  FO1_CHECK_ARG(d->n_seqs > 0 && d->seq_lens, "fo1_llm_generate_prefixed: null argument");
+  FO1_CHECK_ARG(d->all_logits == nullptr, "fo1_llm_generate_prefixed: all_logits is not available with a shared prefix");
+  std::vector<int> members(px->n_groups, 0);
+  for (int b = 0; b < d->n_seqs; ++b) {
+    const int g = px->seq_group[b];
+    FO1_CHECK_ARG(g >= -1 && g < px->n_groups, "fo1_llm_generate_prefixed: sequence %d: group %d out of range [-1, %d)", b, g, px->n_groups);
+    if (g < 0) continue;
+    ++members[g];
+    FO1_CHECK_ARG(px->prefix_lens[g] >= 1 && px->prefix_lens[g] < d->seq_lens[b],
+                  "fo1_llm_generate_prefixed: sequence %d: prefix %d rows, length %d (1 <= P < L)", b, px->prefix_lens[g], d->seq_lens[b]);
+  }
+  for (int g = 0; g < px->n_groups; ++g)
+    FO1_CHECK_ARG(members[g] >= 2, "fo1_llm_generate_prefixed: group %d has %d member(s) (at least 2)", g, members[g]);
+  return FO1_OK;
+}
+
 int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, const fo1_score_desc* sc, const fo1_stream_desc* stm,
-                 cudaStream_t s) {
+                 cudaStream_t s, const fo1_prefix_desc* px = nullptr) {
   if (sc != nullptr && sc->logprobs == nullptr && sc->scores == nullptr && sc->logits == nullptr) sc = nullptr;   // nothing to score
   // the per-sequence host arrays first: they are the caller's, and need neither the model nor the device
   if (sp) FO1_TRY(sampling_check(sp, d->n_seqs, sc ? "fo1_llm_generate_scored" : "fo1_llm_generate_sampled"));
@@ -757,11 +919,13 @@ int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, co
   k.n_stop = d->n_stop_ids; k.pad_id = d->pad_id; k.max_new = d->max_new_tokens;
   k.out_tokens = d->out_tokens; k.out_lens = d->out_lens;
   const DecodeMode mode = sc ? DEC_SCORED : sp ? DEC_SAMPLED : DEC_GREEDY;
-  FO1_TRY(ensure_kv(m, d->n_seqs, max_len + std::max(d->max_new_tokens, 1)));
+  // a shared-prefix call rounds the slot up to 64 rows: the cache-reading attention's last key tile stays inside the slot
+  const int cap = max_len + std::max(d->max_new_tokens, 1);
+  FO1_TRY(ensure_kv(m, d->n_seqs, px ? (cap + 63) / 64 * 64 : cap));
   FO1_TRY(int_cache_trim(m));
   m->arena.reset(true);
   DecodeBufs g;
-  FO1_TRY(llm_prefill(m, d, sp, sc, mode, k, s, true, g));
+  FO1_TRY(llm_prefill(m, d, px, sp, sc, mode, k, s, true, g));
   FO1_TRY(arena_ensure(m, m->arena.peak));
   m->arena.reset(false);
   if (d->max_new_tokens > 0) {  // out_tokens pre-filled with pad so an early exit leaves a clean tail
@@ -771,7 +935,7 @@ int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, co
     FO1_CUDA(cudaMemsetAsync(d->out_lens, 0, d->n_seqs * sizeof(int), s));
     if (sc && sc->logprobs) FO1_CUDA(cudaMemsetAsync(sc->logprobs, 0, (size_t)n * sizeof(float), s));      // 0 past out_lens
   }
-  FO1_TRY(llm_prefill(m, d, sp, sc, mode, k, s, false, g));
+  FO1_TRY(llm_prefill(m, d, px, sp, sc, mode, k, s, false, g));
   if (d->max_new_tokens <= 0) return FO1_OK;
   if (g.mega_grid > 0 && d->max_new_tokens > 1) return decode_persistent(m, d, sc, mode, k, g, s);
   return decode_per_kernel(m, d, sc, mode, k, g, stm ? stm->progress : nullptr, s);
@@ -907,6 +1071,16 @@ extern "C" int fo1_llm_generate_streamed(fo1_model* m, fo1_generate_desc* d, con
   FO1_CHECK_ARG(st == nullptr || (st->tokens && st->lens && st->progress), "fo1_llm_generate_streamed: null stream buffer (tokens, lens and "
                 "progress are required; cancel may be NULL)");
   return llm_generate(m, d, sp, sc, st, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int fo1_llm_generate_prefixed(fo1_model* m, fo1_generate_desc* d, const fo1_prefix_desc* px, const fo1_sampling_desc* sp,
+                                         const fo1_score_desc* sc, const fo1_stream_desc* st, void* stream) {
+  if (px != nullptr && px->n_groups == 0) px = nullptr;
+  FO1_CHECK_ARG(m && d, "fo1_llm_generate_prefixed: null argument");
+  FO1_CHECK_ARG(st == nullptr || (st->tokens && st->lens && st->progress), "fo1_llm_generate_prefixed: null stream buffer (tokens, lens and "
+                "progress are required; cancel may be NULL)");
+  if (px) FO1_TRY(prefix_check(d, px));
+  return llm_generate(m, d, sp, sc, st, static_cast<cudaStream_t>(stream), px);
 }
 
 extern "C" int32_t fo1_stream_progress(const int32_t* progress) { return __atomic_load_n(progress, __ATOMIC_ACQUIRE); }

@@ -257,12 +257,24 @@ class Sampling:
     seed: Sequence[int]
 
 
+@dataclass
+class Prefix:
+    """Shared prompt prefixes of a generate call (fo1_prefix_desc): group g's sequences start with the same ``lens[g]`` rows, whose
+    embeddings ``embeds`` bf16 [sum lens, hidden] and positions ``position_ids`` int32 [3, sum lens] are given once, groups back to
+    back.  ``seq_group[b]``: sequence b's group, or -1."""
+    lens: Sequence[int]
+    embeds: torch.Tensor
+    position_ids: torch.Tensor
+    seq_group: Sequence[int]
+
+
 def _engine_generate(self, inputs_embeds: torch.Tensor, position_ids: torch.Tensor, seq_lens: Sequence[int],
                      rope_deltas: Sequence[int], max_new_tokens: int, stop_ids: Sequence[int], pad_id: int,
                      want_prefill_logits: bool = False, want_all_logits: bool = False, early_exit_interval: int = 8,
                      sampling: Optional[Sampling] = None, want_logprobs: bool = False, want_scores: bool = False,
                      want_logits: bool = False, raw_rows: Optional[Sequence[int]] = None,
-                     on_tokens: Optional[Callable[[int, int, "np.ndarray", "np.ndarray"], Optional[bool]]] = None):
+                     on_tokens: Optional[Callable[[int, int, "np.ndarray", "np.ndarray"], Optional[bool]]] = None,
+                     prefix: Optional[Prefix] = None):
     """Prefill + decode of a packed batch: greedy, or sampled per sequence when ``sampling`` is given.  position_ids int32
     [3, sum L].  Returns a dict of device tensors.
 
@@ -275,10 +287,18 @@ def _engine_generate(self, inputs_embeds: torch.Tensor, position_ids: torch.Tens
     device has published new output columns: ``tokens`` int32 [B, hi - lo] (columns lo..hi-1, pad past a sequence's stop),
     ``lens`` int32 [B] (each sequence's length as of column hi).  Returning True stops every sequence after the next column the
     device records.  An exception from the callback (KeyboardInterrupt included) stops the device too, and is re-raised once it
-    has stopped.  The outputs are bit-identical to the same call without ``on_tokens`` (up to where a stop was asked for)."""
+    has stopped.  The outputs are bit-identical to the same call without ``on_tokens`` (up to where a stop was asked for).
+
+    Shared prefixes (include/fo1.h, fo1_prefix_desc): with ``prefix``, ``seq_lens`` stay the full lengths and ``inputs_embeds`` /
+    ``position_ids`` hold only each sequence's rows after its group's prefix.  Every output is bit-identical to the call on the
+    full sequences; ``want_all_logits`` is refused."""
     B = len(seq_lens)
     V = self.cfg.llm["vocab_size"]
-    T = int(sum(seq_lens))
+    pre = [0] * B
+    if prefix is not None:
+        assert len(prefix.seq_group) == B, "one group index per sequence"
+        pre = [int(prefix.lens[g]) if g >= 0 else 0 for g in prefix.seq_group]
+    T = int(sum(seq_lens)) - sum(pre)
     assert inputs_embeds.shape == (T, self.cfg.llm["hidden_size"]) and inputs_embeds.dtype == torch.bfloat16
     inputs_embeds = inputs_embeds.contiguous()
     position_ids = position_ids.to(self.device, torch.int32).contiguous()
@@ -319,9 +339,23 @@ def _engine_generate(self, inputs_embeds: torch.Tensor, position_ids: torch.Tens
         desc = _lib.ScoreDesc(ptr(lp), ptr(sc), ptr(lg), rr)
         sc_arg = C.byref(desc)
 
+    px_arg = None
+    if prefix is not None:
+        G = len(prefix.lens)
+        pe = prefix.embeds.contiguous()
+        pp = prefix.position_ids.to(self.device, torch.int32).contiguous()
+        assert pe.dtype == torch.bfloat16 and pe.shape == (sum(int(x) for x in prefix.lens), self.cfg.llm["hidden_size"])
+        assert pp.shape == (3, pe.shape[0])
+        px = _lib.PrefixDesc(G, (C.c_int32 * max(G, 1))(*[int(x) for x in prefix.lens]), pe.data_ptr(), pp.data_ptr(),
+                             (C.c_int32 * B)(*[int(g) for g in prefix.seq_group]))
+        px_arg = C.byref(px)
+
     def launch(stream, st=None):
-        check(L.fo1_llm_generate_streamed(self._h, C.byref(d), sp_arg, sc_arg, C.byref(st) if st is not None else None, stream),
-              "fo1_llm_generate_streamed")
+        sa = C.byref(st) if st is not None else None
+        if px_arg is None:
+            check(L.fo1_llm_generate_streamed(self._h, C.byref(d), sp_arg, sc_arg, sa, stream), "fo1_llm_generate_streamed")
+        else:
+            check(L.fo1_llm_generate_prefixed(self._h, C.byref(d), px_arg, sp_arg, sc_arg, sa, stream), "fo1_llm_generate_prefixed")
     if on_tokens is None:
         launch(_stream())
     else:
@@ -333,6 +367,19 @@ def _engine_generate(self, inputs_embeds: torch.Tensor, position_ids: torch.Tens
         out["scores"] = sc
     if want_logits:
         out["logits"] = lg
+    return out
+
+
+def prefix_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, prefix_lens: Sequence[int], own_lens: Sequence[int],
+                     q_heads: int, kv_heads: int, scale: float) -> torch.Tensor:
+    """fo1_prefix_attention: own rows q bf16 [sum own, q_heads * 128] (pitch = row stride) against the caches bf16 [n, cap, kv_heads * 128]:
+    own row i of sequence b attends cache keys 0 .. prefix_lens[b] + i of b.  -> bf16 [sum own, q_heads * 128]."""
+    n, cap, kvd = k_cache.shape
+    assert q.dtype == k_cache.dtype == v_cache.dtype == torch.bfloat16 and q.stride(1) == 1 and k_cache.is_contiguous() and v_cache.is_contiguous()
+    out = torch.empty((q.shape[0], q_heads * 128), dtype=torch.bfloat16, device=q.device)
+    d = _lib.PrefixAttnDesc(q.data_ptr(), q.stride(0), k_cache.data_ptr(), v_cache.data_ptr(), n, cap, (C.c_int32 * n)(*[int(x) for x in prefix_lens]),
+                            (C.c_int32 * n)(*[int(x) for x in own_lens]), q_heads, kv_heads, 128, scale, out.data_ptr(), out.stride(0))
+    check(lib().fo1_prefix_attention(C.byref(d), _stream()), "fo1_prefix_attention")
     return out
 
 
@@ -452,15 +499,18 @@ Engine.generate = _engine_generate
 Engine._stream_buffers = _engine_stream_buffers
 Engine._run_streamed = _engine_run_streamed
 Engine.sample_tokens = staticmethod(sample_tokens)
+Engine.prefix_attention = staticmethod(prefix_attention)
 Engine.score_rows = staticmethod(score_rows)
 
 
 def splice_plan_batch(prompts: Sequence[Sequence[int]], image_grids: Sequence[Sequence[Tuple[int, int]]], n_regions: Sequence[int], device,
                       image_token_id: int = 151655, video_token_id: int = 151656, vision_start_token_id: int = 151652, merge: int = 2,
-                      image_placeholder: int = -200, region_placeholder: int = -300):
+                      image_placeholder: int = -200, region_placeholder: int = -300, row_src: Optional[Sequence[int]] = None):
     """The splice + M-RoPE bookkeeping of a whole batch in ONE launch on the device (fo1_splice_plan_batch).  Per sample b:
     ``prompts[b]`` ids with placeholders, ``image_grids[b]`` its images' (gh, gw), ``n_regions[b]`` region rows.  Image rows /
-    region rows of the batch are assumed packed back to back in sample order (what Fo1Pipeline.encode produces).
+    region rows of the batch are assumed packed back to back in sample order (what Fo1Pipeline.encode produces).  ``row_src``:
+    sample b reads the image / region rows of sample row_src[b] <= b (same image and boxes); only the samples with row_src[b] == b
+    have rows of their own, packed in their order.
     -> dict(kind, index, new_ids int32 [T]; position_ids int32 [3, T]; rope_delta int32 [B]) on the device, lens (host list)."""
     import numpy as np
     B = len(prompts)
@@ -475,6 +525,10 @@ def splice_plan_batch(prompts: Sequence[Sequence[int]], image_grids: Sequence[Se
         # every image placeholder expands to its image's rows; more placeholders than images is reported per sample by the kernel
         exp = sum(gh * gw // unit for gh, gw in list(image_grids[b])[:n_img_ph])
         out_off[b + 1] = out_off[b] + len(prompts[b]) - min(n_img_ph, len(image_grids[b])) + exp
+        src = b if row_src is None else int(row_src[b])
+        if src != b:
+            img_row[b] = img_row[src]; reg_row[b] = reg_row[src]
+            continue
         img_row[b] = rows_i; reg_row[b] = rows_r
         rows_i += toks; rows_r += int(n_regions[b])
     T = int(out_off[B])

@@ -15,7 +15,7 @@ import numpy as np
 import torch
 
 from . import hfre as HF
-from .engine import Engine, splice_plan, splice_plan_batch
+from .engine import Engine, Prefix, splice_plan, splice_plan_batch
 
 
 @dataclass
@@ -26,6 +26,72 @@ class SampleInputs:
     image_aux: Optional[torch.Tensor]   # fp32 [3, H, W]      (CLIPImageProcessor, 'dynamic' mode); None with image_u8
     boxes: torch.Tensor                 # fp32 [N, 4] xyxy in aux-tensor pixels
     image_u8: Optional[torch.Tensor] = None   # uint8 [H, W, 3] RGB: pre-processed on the device by Fo1Pipeline.preprocess()
+
+
+def _encoder_meta(s: SampleInputs):
+    """Host facts that must agree before two samples' encoder inputs are compared by content."""
+    if s.image_u8 is not None:
+        return ("u8", tuple(s.image_u8.shape), tuple(s.boxes.shape))
+    return ("px", tuple(s.grid_hw), tuple(s.pixel_values.shape), tuple(s.image_aux.shape), tuple(s.boxes.shape))
+
+
+def _same_tensor(a: torch.Tensor, b: torch.Tensor) -> bool:
+    return a is b or (a.device == b.device and a.dtype == b.dtype and torch.equal(a, b))
+
+
+def encoder_groups(samples: Sequence[SampleInputs]) -> List[int]:
+    """rep[b]: the first sample whose encoder inputs (image and boxes) equal sample b's by content.  Host metadata first, then the boxes
+    of the remaining candidates in one host copy, then their pixels: distinct images with distinct boxes cost at most that one copy."""
+    B = len(samples)
+    meta = [_encoder_meta(s) for s in samples]
+    count: Dict[tuple, int] = {}
+    for m in meta:
+        count[m] = count.get(m, 0) + 1
+    cand = [b for b in range(B) if count[meta[b]] > 1]
+    rep = list(range(B))
+    if not cand:
+        return rep
+    flat = [samples[b].boxes.reshape(-1).to(torch.float32) for b in cand]     # encode() reads the boxes as fp32
+    on_dev = [i for i, x in enumerate(flat) if x.is_cuda]
+    if on_dev:
+        for i, h in zip(on_dev, torch.cat([flat[i] for i in on_dev]).cpu().split([flat[i].numel() for i in on_dev])):
+            flat[i] = h
+    boxes = dict(zip(cand, flat))
+    for i, b in enumerate(cand):
+        s = samples[b]
+        for c in cand[:i]:
+            if rep[c] != c or meta[c] != meta[b] or not torch.equal(boxes[c], boxes[b]):
+                continue
+            o = samples[c]
+            pix = [(o.image_u8, s.image_u8)] if s.image_u8 is not None else [(o.pixel_values, s.pixel_values), (o.image_aux, s.image_aux)]
+            if all(_same_tensor(x, y) for x, y in pix):
+                rep[b] = c
+                break
+    return rep
+
+
+def shared_prefix_groups(prompts: Sequence[Sequence[int]], rep: Sequence[int], image_rows: Sequence[int], lens: Sequence[int],
+                         image_placeholder: int = -200) -> List[Tuple[List[int], int]]:
+    """-> [(members, P)] for every set of >= 2 samples with equal encoder inputs (``rep``): P is the longest common prefix of their ids,
+    placeholders included, counted in spliced rows (an image placeholder is ``image_rows[b]`` rows) and capped at min L_b - 1, so each
+    member keeps one row of its own.  Sets with P == 0 are left out (they still share the towers)."""
+    sets: Dict[int, List[int]] = {}
+    for b, r in enumerate(rep):
+        sets.setdefault(r, []).append(b)
+    out = []
+    for r, mem in sets.items():
+        if len(mem) < 2:
+            continue
+        first = prompts[mem[0]]
+        n = min(len(prompts[b]) for b in mem)
+        k = 0
+        while k < n and all(prompts[b][k] == first[k] for b in mem):
+            k += 1
+        rows = sum(image_rows[r] if t == image_placeholder else 1 for t in first[:k])
+        P = min(rows, min(lens[b] for b in mem) - 1)
+        if P >= 1:
+            out.append((mem, P))
+    return out
 
 
 class Fo1Pipeline:
@@ -41,6 +107,7 @@ class Fo1Pipeline:
         self._keep_stages = None
         self._pre = None
         self.check_plan = True
+        self._share_inputs = True            # tests clear it to get the unshared path as the reference of the shared one
 
     def _mark(self, name: str) -> None:
         if self.profile_stages:
@@ -189,6 +256,13 @@ class Fo1Pipeline:
         ``want_logits`` / ``raw_rows``: per-token scores, as Engine.generate.  ``on_tokens``: the streaming callback of
         Engine.generate (columns of the whole batch, in sample order)."""
         eng, dev = self.eng, self.eng.device
+        kw = dict(max_new_tokens=max_new_tokens, stop_ids=stop_ids, pad_id=pad_id, early_exit_interval=early_exit_interval,
+                  want_prefill_logits=want_prefill_logits, sampling=sampling, want_logprobs=want_logprobs, want_scores=want_scores,
+                  want_logits=want_logits, raw_rows=raw_rows, on_tokens=on_tokens)
+        if self._share_inputs and len(samples) > 1:
+            rep = encoder_groups(samples)
+            if any(r != b for b, r in enumerate(rep)):
+                return self._generate_shared(samples, rep, **kw)
         samples = self.preprocess(samples)           # uint8 images -> the towers' input tensors, on the device
         feats, img_off, region_tokens, _ = self.encode(samples)
         # splice + M-RoPE bookkeeping of the whole batch in one launch on the device (fo1_splice_plan_batch); the per-sample host
@@ -208,6 +282,54 @@ class Fo1Pipeline:
         out = eng.generate(embeds, pos, lens, deltas, max_new_tokens, stop_ids, pad_id, want_prefill_logits=want_prefill_logits,
                            early_exit_interval=early_exit_interval, sampling=sampling, want_logprobs=want_logprobs, want_scores=want_scores,
                            want_logits=want_logits, raw_rows=raw_rows, on_tokens=on_tokens)
+        self._mark("llm_prefill_decode")
+        out["prompt_lens"] = lens
+        return out
+
+    def _generate_shared(self, samples, rep, max_new_tokens, stop_ids, pad_id, early_exit_interval, want_prefill_logits, sampling,
+                         want_logprobs, want_scores, want_logits, raw_rows, on_tokens):
+        """generate() of a batch in which some samples have equal encoder inputs: the towers run once per unique image, and each set's
+        common prompt prefix is prefilled once (Engine.generate's ``prefix``).  Bit-identical to the unshared path."""
+        eng, dev = self.eng, self.eng.device
+        B = len(samples)
+        own = [b for b in range(B) if rep[b] == b]
+        slot = {b: i for i, b in enumerate(own)}
+        uniq = self.preprocess([samples[b] for b in own])
+        feats, _, region_tokens, _ = self.encode(uniq)
+        merge = eng.cfg.vit["spatial_merge_size"]
+        grids = [uniq[slot[rep[b]]].grid_hw for b in range(B)]
+        prompts = [samples[b].input_ids for b in range(B)]
+        plan = splice_plan_batch(prompts, [[g] for g in grids], [region_tokens[slot[rep[b]]].shape[0] for b in range(B)], dev, merge=merge,
+                                 row_src=rep, **self.ids)
+        lens = plan["lens"]
+        if self.check_plan:
+            st = plan["status"].cpu().tolist()
+            if any(st):
+                raise ValueError(f"fo1_splice_plan_batch: per-sample status {st} (placeholders and features disagree)")
+        regions = torch.cat(region_tokens, 0)
+        groups = shared_prefix_groups(prompts, rep, [gh * gw // (merge * merge) for gh, gw in grids], lens)
+        prefix = None
+        if not groups:
+            embeds, pos = eng.build_embeds(plan["kind"], plan["index"], feats, regions), plan["position_ids"]
+        else:
+            start = np.cumsum([0] + list(lens))
+            seq_group, pre = [-1] * B, [0] * B
+            sel = []
+            for g, (mem, P) in enumerate(groups):
+                sel.append(np.arange(start[mem[0]], start[mem[0]] + P))
+                for b in mem:
+                    seq_group[b], pre[b] = g, P
+            sel += [np.arange(start[b] + pre[b], start[b + 1]) for b in range(B)]
+            idx = torch.from_numpy(np.concatenate(sel).astype(np.int64)).to(dev, non_blocking=True)
+            n_pre = sum(P for _, P in groups)
+            emb = eng.build_embeds(plan["kind"][idx].contiguous(), plan["index"][idx].contiguous(), feats, regions)
+            pos_all = plan["position_ids"][:, idx]
+            prefix = Prefix([P for _, P in groups], emb[:n_pre], pos_all[:, :n_pre], seq_group)
+            embeds, pos = emb[n_pre:], pos_all[:, n_pre:]
+        self._mark("splice")
+        out = eng.generate(embeds, pos, lens, plan["rope_delta"], max_new_tokens, stop_ids, pad_id, want_prefill_logits=want_prefill_logits,
+                           early_exit_interval=early_exit_interval, sampling=sampling, want_logprobs=want_logprobs, want_scores=want_scores,
+                           want_logits=want_logits, raw_rows=raw_rows, on_tokens=on_tokens, prefix=prefix)
         self._mark("llm_prefill_decode")
         out["prompt_lens"] = lens
         return out

@@ -16,7 +16,7 @@ import torch
 # generation_config.json fields of logits processors the engine does not implement, with HF GenerationConfig's neutral defaults.
 # On the sampled path a non-neutral value is refused (honour or refuse, never ignore); greedy decoding does not read them.
 _UNSUPPORTED_PROCESSORS = (("repetition_penalty", 1.0), ("min_p", None), ("typical_p", 1.0), ("epsilon_cutoff", 0.0),
-                           ("eta_cutoff", 0.0), ("no_repeat_ngram_size", 0), ("num_beams", 1), ("num_return_sequences", 1))
+                           ("eta_cutoff", 0.0), ("no_repeat_ngram_size", 0), ("num_beams", 1))
 
 
 class Fo1ForCausalLM:
@@ -148,13 +148,48 @@ class Fo1ForCausalLM:
             T.append(t); P.append(p); K.append(k)
         return E.Sampling(T, P, K, seeds)
 
+    def _num_return_sequences(self, kwargs):
+        n = kwargs.get("num_return_sequences")
+        n = self.generation_config.get("num_return_sequences", 1) if n is None else n
+        n = 1 if n is None else int(n)
+        if n < 1:
+            raise ValueError(f"`num_return_sequences` has to be a positive integer, but is {n}")
+        return n
+
+    def _results(self, out, inputs, want):
+        """The n rows of an engine output as HF returns num_return_sequences: LongTensor [n, P + T_max] padded with the pad id, or the
+        output dict with scores / logits as tuples of [n, V] (rows past a sequence's stop are unspecified)."""
+        lens = [int(x) for x in out["lens"].cpu().tolist()]
+        n, T = len(lens), max(lens)
+        new = out["tokens"][:, :T].to(torch.long)                 # pad past each sequence's stop (the engine's pad_id)
+        full = torch.cat([inputs.to(new.device).expand(n, -1), new], 1)
+        if want is None:
+            return full
+        from transformers.generation.utils import GenerateDecoderOnlyOutput
+        rows = lambda key: tuple(out[key][t] for t in range(T))
+        return GenerateDecoderOnlyOutput(sequences=full, scores=rows("scores") if want[0] else None,
+                                         logits=rows("logits") if want[1] else None, past_key_values=None)
+
     @torch.no_grad()
     def generate(self, inputs=None, images=None, images_aux=None, image_grid_thws=None, bbox_list=None, do_sample=False, temperature=0.0,
                  max_new_tokens=512, streamer=None, top_p=1.0, use_cache=True, stopping_criteria=None, pad_token_id=None, top_k=None, **kwargs):
         want = self._outputs(kwargs)
+        n = self._num_return_sequences(kwargs)
+        kwargs.pop("num_return_sequences", None)
+        if n > 1 and not do_sample:
+            raise ValueError("Greedy methods without beam search do not support `num_return_sequences` different than 1 "
+                             f"(got {n}).")
+        if n > 1 and streamer is not None:
+            raise ValueError("`streamer` cannot be used with `num_return_sequences` > 1: streamers accept one sequence")
         sample, stop, samp = self._sample(inputs, images, images_aux, image_grid_thws, bbox_list, do_sample, temperature, stopping_criteria,
                                           top_p, top_k, **kwargs)
         pad = pad_token_id if pad_token_id is not None else (stop[0] if stop else 0)
+        if n > 1:
+            # n copies of the sample share the whole prompt but its last row (the pipeline prefills it once); one seed each
+            out = self.pipeline.generate([sample] * n, int(max_new_tokens), sorted(set(stop)), pad_id=int(pad), early_exit_interval=8,
+                                         sampling=self._sampling([samp] * n), want_scores=bool(want and want[0]),
+                                         want_logits=bool(want and want[1]))
+            return self._results(out, inputs[0], want)
         on_tokens = None
         if streamer is not None:
             # HF's order: the prompt once, then each generated token (the stop token included, pad not) as the device publishes
@@ -183,6 +218,8 @@ class Fo1ForCausalLM:
         if not batch:
             return []
         wants = [self._outputs(kw) for kw in batch]
+        if any(self._num_return_sequences(kw) != 1 for kw in batch):
+            raise NotImplementedError("num_return_sequences > 1 in generate_batch: call generate for such a sample, or repeat it in the batch")
         keys = ("inputs", "images", "images_aux", "image_grid_thws", "bbox_list", "do_sample", "temperature", "stopping_criteria", "top_p",
                 "top_k") + tuple(n for n, _ in _UNSUPPORTED_PROCESSORS)
         samples, stops, samps = zip(*(self._sample(**{k: v for k, v in kw.items() if k in keys}) for kw in batch))
