@@ -502,6 +502,39 @@ int fo1_llm_generate_prefixed(fo1_model* m, fo1_generate_desc* d, const fo1_pref
                               const fo1_score_desc* sc /* NULL: unscored */, const fo1_stream_desc* st /* NULL: not streamed */,
                               void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Beam search (HF generate with num_beams > 1 and do_sample=False: transformers' GenerationMixin._beam_search and its helpers).
+ * Each of the n_seqs prompts runs as if it were alone in the call, with num_beams = N decode rows and cache slots.  Per step,
+ * over log_softmax(logits) of the running beams: accumulated = log-prob + running score (initially [0, -1e9, ...]); the best
+ * n_keep = K of the N * V continuations (score descending, then beam * V + token ascending); a continuation hits the stop test
+ * if its token is a stop id or it reaches max_new_tokens; the running set is the best N of (score + hit * -1e9); hits among the
+ * best N enter the finished set with score / (float)pow(len, length_penalty) unless the prompt is full (early_stopping True) or
+ * cannot improve (the early-stop heuristic); the finished set keeps the best N (old entries before new on equal scores).  The
+ * prompt stops when HF's _beam_search_has_unfinished_sequences would for it alone.  Every fp32 operation is HF's, in its order,
+ * so the selection is bit-identical to HF's fed the same log-prob rows.  The prompt is prefilled once; its K/V is written into
+ * its N slots, and after each step the generated rows of each new beam are copied from its parent's slot.
+ * In d: out_tokens [n_seqs * num_return][max_new_tokens] (pad_id past each length) and out_lens [n_seqs * num_return] receive the
+ * best num_return hypotheses of each prompt, best first; all_logits is refused, prefill_logits is allowed; steps_run is the number
+ * of decode iterations the loop ran.  Always the per-kernel decode path (fo1_last_decode_path() == 0).
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct {
+  int32_t num_beams;         /* N: 2 .. 16 */
+  int32_t n_keep;            /* K: HF's max(2, 1 + number of eos ids) * N; 2N <= K <= 128 and K <= vocab */
+  double length_penalty;     /* finite; double, as HF's Python float: the divisors are (float)pow(len, length_penalty) */
+  int32_t early_stopping;    /* 0 = False, 1 = True, 2 = "never" */
+  int32_t num_return;        /* 1 .. N hypotheses per prompt */
+  float* sequence_scores;    /* DEVICE fp32 [n_seqs * num_return]: the hypotheses' length-penalised scores */
+  int32_t* beam_indices;     /* DEVICE int32 [n_seqs * num_return][max_new_tokens]: prompt * N + parent beam per token, -1 past the length */
+  int32_t* steps_run;        /* DEVICE int32 [n_seqs]: steps the prompt ran (rows of scores / logits it wrote) */
+  float* scores;             /* optional DEVICE fp32 [max_new_tokens][n_seqs * N][vocab]: log_softmax of each beam row (HF output_scores) */
+  float* logits;             /* optional DEVICE fp32 [max_new_tokens][n_seqs * N][vocab]: the raw rows (HF output_logits) */
+  float* logprobs;           /* optional DEVICE fp32 [n_seqs * num_return][max_new_tokens]: each returned token's log-probability
+                                under its parent beam's row (HF's compute_transition_scores with beam_indices); 0 past the length */
+} fo1_beam_desc;
+/* Checked on the host before any CUDA call: 2 <= N <= 16, 1 <= num_return <= N, 2N <= n_keep <= min(128, vocab), a finite
+ * length_penalty, early_stopping in {0, 1, 2}, max_new_tokens >= 1, the outputs non-NULL and no all_logits. */
+int fo1_llm_generate_beam(fo1_model* m, fo1_generate_desc* d, const fo1_beam_desc* bm, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -93,6 +93,14 @@ class PrefixAttnDesc(C.Structure):
                 ("kv_heads", C.c_int32), ("head_dim", C.c_int32), ("scale", C.c_float), ("out", C.c_void_p), ("ldo", C.c_int64)]
 
 
+class BeamDesc(C.Structure):
+    """fo1_beam_desc: HOST parameters; DEVICE outputs sequence_scores [n * num_return], beam_indices [n * num_return][max_new],
+    steps_run [n], optional scores / logits [max_new][n * num_beams][V] and logprobs [n * num_return][max_new]."""
+    _fields_ = [("num_beams", C.c_int32), ("n_keep", C.c_int32), ("length_penalty", C.c_double), ("early_stopping", C.c_int32),
+                ("num_return", C.c_int32), ("sequence_scores", C.c_void_p), ("beam_indices", C.c_void_p), ("steps_run", C.c_void_p),
+                ("scores", C.c_void_p), ("logits", C.c_void_p), ("logprobs", C.c_void_p)]
+
+
 FO1_STREAM_DONE = 1 << 30
 
 _lib = None
@@ -141,6 +149,8 @@ def lib() -> C.CDLL:
     L.fo1_llm_generate_prefixed.restype = C.c_int
     L.fo1_llm_generate_prefixed.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(PrefixDesc), C.POINTER(SamplingDesc), C.POINTER(ScoreDesc),
                                             C.POINTER(StreamDesc), C.c_void_p]
+    L.fo1_llm_generate_beam.restype = C.c_int
+    L.fo1_llm_generate_beam.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(BeamDesc), C.c_void_p]
     L.fo1_prefix_attention.restype = C.c_int
     L.fo1_prefix_attention.argtypes = [C.POINTER(PrefixAttnDesc), C.c_void_p]
     L.fo1_stream_progress.restype = C.c_int32

@@ -4,8 +4,9 @@
 
 namespace fo1 {
 
-// how a column's tokens are chosen (a scored greedy call samples with top_k 1 on raw rows: the arg-max, bit for bit)
-enum DecodeMode { DEC_GREEDY, DEC_SAMPLED, DEC_SCORED };
+// how a column's tokens are chosen (a scored greedy call samples with top_k 1 on raw rows: the arg-max, bit for bit); DEC_BEAM: beam
+// search (beam.cuh), per-kernel path only
+enum DecodeMode { DEC_GREEDY, DEC_SAMPLED, DEC_SCORED, DEC_BEAM };
 
 struct DecodeState {
   int* cache_len;  // [B] K/V entries in the cache

@@ -11,7 +11,9 @@
 // state stay on the device, the host only enqueues kernels (no per-token sync); lm_head runs on the last
 // prompt position only.
 #include <algorithm>
+#include <cmath>
 
+#include "beam.cuh"
 #include "decode_loop.cuh"
 #include "decode_mega.cuh"
 
@@ -473,7 +475,8 @@ struct PrefixTables {
 // one decoder layer over `rows` packed rows.  x_in -> x_out (x_mid scratch).  prefill: varlen causal attention
 // + cache fill (px: the shared-prefix split of it); decode: cache append + single-query attention.
 struct LayerBuf { bf16 *xn, *qkv, *att, *x_mid, *h; float* dec_part; int* rowseg = nullptr; double attn_flops = 0.0; const int* tiles = nullptr; int n_tiles = 0;
-                  const PrefixTables* px = nullptr; };
+                  const PrefixTables* px = nullptr;
+                  const int *fan_gt = nullptr, *fan_off = nullptr, *fan_mem = nullptr; };   // beam search: each prompt row into its N slots
 
 // the prefill attention of a shared-prefix layer: prefix K/V into every member's slot, own K/V into the own slot, then the prefix rows
 // as causal segments and the own rows against the cache
@@ -522,7 +525,10 @@ static int llm_layer(Model* m, int li, const bf16* x_in, bf16* x_out, const Laye
     FO1_TRY(prefix_layer_attention(m, B_, rows, kc, vc, s, dry));
   } else if (prefill) {
     FO1_RUN(rope_apply(B_.qkv, ldq, cs, rows, c.llm_heads + c.llm_kv_heads, hd, s));   // q|k heads are contiguous in the packed row
-    if (!dry) {
+    if (!dry && B_.fan_gt != nullptr) {
+      kv_fanout_kernel<<<rows, 64, 0, s>>>(B_.qkv, ldq, QD, KD, reinterpret_cast<const int2*>(B_.fan_gt), B_.fan_off, B_.fan_mem, kc, vc, m->kv_cap);
+      FO1_LAUNCH_CHECK();
+    } else if (!dry) {
       kv_store_kernel<<<rows, 128, 0, s>>>(B_.qkv, ldq, QD, KD, d_row_seq, d_row_t, kc, vc, m->kv_cap);
       FO1_LAUNCH_CHECK();
     }
@@ -553,6 +559,13 @@ struct DecodeBufs {
   float *cs_dec, *logits, *mg_ssq, *mg_amax_v;
   int *mg_amax_i, *mg_sync, *samp_tok;
   SampleRowParams* samp;
+  BeamArgs* beam = nullptr;       // DEC_BEAM
+};
+
+// a beam-search call: the device state (beam.cuh) and the host table of length-penalty divisors
+struct BeamRun {
+  BeamArgs a;
+  std::vector<float> lp_div;
 };
 
 // the tokens of the current output column into new_tok (scored: also the column's scores), then their recording; every kernel reads
@@ -560,6 +573,7 @@ struct DecodeBufs {
 static int decode_column(DecodeMode mode, const DecodeBufs& g, const ColumnSink& k, const fo1_score_desc* sc, int B, int V, int advance,
                          cudaStream_t s) {
   const DecodeState& st = k.st;
+  if (mode == DEC_BEAM) return beam_column(*g.beam, g.logits, st, advance, s);
   if (mode == DEC_SCORED) {
     FO1_TRY(score_rows(g.logits, V, B, V, g.samp, st.step, st.new_tok, true, st.finished, k.max_new, sc->logprobs, k.max_new, sc->scores,
                        sc->logits, V, s));
@@ -614,7 +628,7 @@ static int prefix_tables(Model* m, const fo1_generate_desc* d, const fo1_prefix_
 }
 
 static int llm_prefill(Model* m, fo1_generate_desc* d, const fo1_prefix_desc* px, const fo1_sampling_desc* sp, const fo1_score_desc* sc,
-                       DecodeMode mode, const ColumnSink& k, cudaStream_t s, bool dry, DecodeBufs& g) {
+                       DecodeMode mode, const ColumnSink& k, cudaStream_t s, bool dry, DecodeBufs& g, BeamRun* bm = nullptr) {
   const fo1_model_config& c = m->cfg;
   Arena& A = m->arena;
   const int B = d->n_seqs, H = c.llm_hidden, hd = c.llm_head_dim, V = c.llm_vocab;
@@ -625,7 +639,8 @@ static int llm_prefill(Model* m, fo1_generate_desc* d, const fo1_prefix_desc* px
   for (int b = 0; b < B; ++b) { T += d->seq_lens[b] - prefix_of(px, b); max_len = std::max(max_len, d->seq_lens[b]); }
   for (int gi = 0; px && gi < px->n_groups; ++gi) n_pre += px->prefix_lens[gi];
   T += n_pre;
-  const int R = (int)std::max<long long>(T, B);
+  const int RD = bm ? B * bm->a.N : B;      // rows of a decode step: one per sequence, or one per beam
+  const int R = (int)std::max<long long>(T, RD);
 
   g = DecodeBufs();
   LayerBuf& buf = g.layer;
@@ -637,13 +652,13 @@ static int llm_prefill(Model* m, fo1_generate_desc* d, const fo1_prefix_desc* px
   buf.x_mid = A.alloc<bf16>((size_t)R * H);
   buf.h = A.alloc<bf16>((size_t)R * Ip);
   float* cs_pre = A.alloc<float>((size_t)R * hd);
-  g.cs_dec = A.alloc<float>((size_t)B * hd);
-  buf.dec_part = A.alloc<float>((size_t)B * c.llm_heads * kDecSplits * (128 + 4));
+  g.cs_dec = A.alloc<float>((size_t)RD * hd);
+  buf.dec_part = A.alloc<float>((size_t)RD * c.llm_heads * kDecSplits * (128 + 4));
   buf.rowseg = A.alloc<int>((size_t)R * 2);
   for (int b = 0; b < B; ++b) buf.attn_flops += 2.0 * (double)d->seq_lens[b] * d->seq_lens[b] * QD;   // causal: half of 4 L^2 d
   bf16* last = A.alloc<bf16>((size_t)B * H);
-  g.lastn = A.alloc<bf16>((size_t)B * H);
-  g.logits = A.alloc<float>((size_t)B * V);
+  g.lastn = A.alloc<bf16>((size_t)RD * H);
+  g.logits = A.alloc<float>((size_t)RD * V);
   bf16* alln = d->all_logits ? A.alloc<bf16>((size_t)T * H) : nullptr;
   int* d_lens = A.alloc<int>(B);
   int* d_deltas = A.alloc<int>(B);
@@ -653,14 +668,18 @@ static int llm_prefill(Model* m, fo1_generate_desc* d, const fo1_prefix_desc* px
   // FO1_MEGA_MAX_B lowers the threshold, FO1_NO_MEGA disables the kernel.
   int mega_max_b = 32;
   if (const char* e = getenv("FO1_MEGA_MAX_B")) mega_max_b = std::max(0, std::min(32, atoi(e)));
-  g.mega_grid = (m->llm.mega_ok && B <= mega_max_b && getenv("FO1_NO_MEGA") == nullptr) ? decode_mega_grid() : 0;
+  g.mega_grid = (m->llm.mega_ok && !bm && B <= mega_max_b && getenv("FO1_NO_MEGA") == nullptr) ? decode_mega_grid() : 0;
   g.mg_ssq = A.alloc<float>((size_t)2 * std::max(g.mega_grid, 1) * 32);
   g.mg_amax_v = A.alloc<float>((size_t)std::max(g.mega_grid, 1) * 32);
   g.mg_amax_i = A.alloc<int>((size_t)std::max(g.mega_grid, 1) * 32);
   g.mg_sync = A.alloc<int>((size_t)B * c.llm_kv_heads + 8);
   // sampled or scored decoding: the per-sequence parameters and the tokens the persistent kernel's CTA b drew
-  g.samp = mode != DEC_GREEDY ? A.alloc<SampleRowParams>(B) : nullptr;
-  g.samp_tok = mode != DEC_GREEDY ? A.alloc<int>(B) : nullptr;
+  g.samp = mode == DEC_SAMPLED || mode == DEC_SCORED ? A.alloc<SampleRowParams>(B) : nullptr;
+  g.samp_tok = mode == DEC_SAMPLED || mode == DEC_SCORED ? A.alloc<int>(B) : nullptr;
+  if (bm) {   // beam search: its state and scratch (sized by the dry run like everything else)
+    beam_alloc(A, bm->a);
+    g.beam = &bm->a;
+  }
 
   // ---- integer tables of the packed batch ----
   const int *d_cu = nullptr, *d_row_seq = nullptr, *d_row_t = nullptr, *d_last = nullptr;
@@ -683,6 +702,17 @@ static int llm_prefill(Model* m, fo1_generate_desc* d, const fo1_prefix_desc* px
       lastrow.push_back(cu.back() - 1);
       key += ":" + std::to_string(d->seq_lens[b]);
     }
+    if (!px && bm) {     // prompt b's rows go to its N cache slots b * N .. b * N + N - 1 (kv_fanout_kernel)
+      const int N = bm->a.N;
+      std::vector<int> gt, off, mem;
+      for (int r = 0; r < (int)row_seq.size(); ++r) { gt.push_back(row_seq[r]); gt.push_back(row_t[r]); }
+      for (int b = 0; b <= B; ++b) off.push_back(b * N);
+      for (int r = 0; r < B * N; ++r) mem.push_back(r);
+      const std::string bk = key + ":beam" + std::to_string(N);
+      FO1_TRY(cached_ints(m, bk + ":gt", gt, &buf.fan_gt, s));
+      FO1_TRY(cached_ints(m, bk + ":off", off, &buf.fan_off, s));
+      FO1_TRY(cached_ints(m, bk + ":mem", mem, &buf.fan_mem, s));
+    }
     if (!px) {
       FO1_TRY(cached_ints(m, key + ":cu", cu, &d_cu, s));
       FO1_TRY(cached_ints(m, key + ":rs", row_seq, &d_row_seq, s));
@@ -697,7 +727,11 @@ static int llm_prefill(Model* m, fo1_generate_desc* d, const fo1_prefix_desc* px
     if (d->rope_deltas_device != nullptr) FO1_CUDA(cudaMemcpyAsync(d_deltas, d->rope_deltas_device, B * sizeof(int), cudaMemcpyDeviceToDevice, s));
     else FO1_CUDA(cudaMemcpyAsync(d_deltas, d->rope_deltas, B * sizeof(int), cudaMemcpyHostToDevice, s));
     if (d->n_stop_ids > 0) FO1_CUDA(cudaMemcpyAsync(k.st.stop_ids, d->stop_ids, d->n_stop_ids * sizeof(int), cudaMemcpyHostToDevice, s));
-    if (mode != DEC_GREEDY) {
+    if (bm) {
+      FO1_CUDA(cudaMemcpyAsync(const_cast<int*>(bm->a.prompt_len), d->seq_lens, B * sizeof(int), cudaMemcpyHostToDevice, s));
+      FO1_CUDA(cudaMemcpyAsync(const_cast<float*>(bm->a.lp_div), bm->lp_div.data(), bm->lp_div.size() * sizeof(float), cudaMemcpyHostToDevice, s));
+    }
+    if (mode == DEC_SAMPLED || mode == DEC_SCORED) {
       // a scored greedy call samples with top_k 1 (bit-identical to greedy) so that both paths score in the sampler's per-row pass
       std::vector<SampleRowParams> h(B);
       for (int b = 0; b < B; ++b) h[b] = score_row_params(sp, sc ? sc->raw_rows : nullptr, b);
@@ -746,8 +780,12 @@ static int llm_prefill(Model* m, fo1_generate_desc* d, const fo1_prefix_desc* px
   }
   if (dry) return FO1_OK;
   if (d->prefill_logits) FO1_CUDA(cudaMemcpyAsync(d->prefill_logits, g.logits, (size_t)B * V * sizeof(float), cudaMemcpyDeviceToDevice, s));
-  decode_init_kernel<<<ceil_div(B, 128), 128, 0, s>>>(k.st, d_lens, d_deltas, B);
-  FO1_LAUNCH_CHECK();
+  if (bm) {
+    FO1_TRY(beam_init(bm->a, k.st, d_lens, d_deltas, s));
+  } else {
+    decode_init_kernel<<<ceil_div(B, 128), 128, 0, s>>>(k.st, d_lens, d_deltas, B);
+    FO1_LAUNCH_CHECK();
+  }
   if (d->max_new_tokens <= 0) return FO1_OK;
   return decode_column(mode, g, k, sc, B, V, 0, s);
 }
@@ -785,7 +823,7 @@ static int decode_persistent(Model* m, fo1_generate_desc* d, const fo1_score_des
 static int decode_per_kernel(Model* m, fo1_generate_desc* d, const fo1_score_desc* sc, DecodeMode mode, const ColumnSink& k,
                              const DecodeBufs& g, const int32_t* h_progress, cudaStream_t s) {
   const fo1_model_config& c = m->cfg;
-  const int B = d->n_seqs, H = c.llm_hidden, hd = c.llm_head_dim, V = c.llm_vocab;
+  const int B = g.beam ? g.beam->S * g.beam->N : d->n_seqs, H = c.llm_hidden, hd = c.llm_head_dim, V = c.llm_vocab;
   LlmState* ls = static_cast<LlmState*>(m->llm_state);
   // programmatic dependent launch: each kernel of the step starts (prologue, weight prefetch) while its predecessor drains
   const bool use_pdl = getenv("FO1_NO_PDL") == nullptr;
@@ -894,7 +932,7 @@ static int prefix_check(const fo1_generate_desc* d, const fo1_prefix_desc* px) {
 }
 
 int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, const fo1_score_desc* sc, const fo1_stream_desc* stm,
-                 cudaStream_t s, const fo1_prefix_desc* px = nullptr) {
+                 cudaStream_t s, const fo1_prefix_desc* px = nullptr, const fo1_beam_desc* bmd = nullptr) {
   if (sc != nullptr && sc->logprobs == nullptr && sc->scores == nullptr && sc->logits == nullptr) sc = nullptr;   // nothing to score
   // the per-sequence host arrays first: they are the caller's, and need neither the model nor the device
   if (sp) FO1_TRY(sampling_check(sp, d->n_seqs, sc ? "fo1_llm_generate_scored" : "fo1_llm_generate_sampled"));
@@ -915,30 +953,49 @@ int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, co
     FO1_TRY(stream_resolve(stm, &k.stream));
     __atomic_store_n(stm->progress, d->max_new_tokens > 0 ? 0 : FO1_STREAM_DONE, __ATOMIC_RELEASE);   // before anything is enqueued
   }
-  FO1_TRY(ensure_state(m, d->n_seqs, d->n_stop_ids, &k.st));
+  const int rows = bmd ? d->n_seqs * bmd->num_beams : d->n_seqs;     // decode rows / cache slots
+  FO1_TRY(ensure_state(m, rows, d->n_stop_ids, &k.st));
   k.n_stop = d->n_stop_ids; k.pad_id = d->pad_id; k.max_new = d->max_new_tokens;
   k.out_tokens = d->out_tokens; k.out_lens = d->out_lens;
-  const DecodeMode mode = sc ? DEC_SCORED : sp ? DEC_SAMPLED : DEC_GREEDY;
+  const DecodeMode mode = bmd ? DEC_BEAM : sc ? DEC_SCORED : sp ? DEC_SAMPLED : DEC_GREEDY;
   // a shared-prefix call rounds the slot up to 64 rows: the cache-reading attention's last key tile stays inside the slot
   const int cap = max_len + std::max(d->max_new_tokens, 1);
-  FO1_TRY(ensure_kv(m, d->n_seqs, px ? (cap + 63) / 64 * 64 : cap));
+  FO1_TRY(ensure_kv(m, rows, px ? (cap + 63) / 64 * 64 : cap));
   FO1_TRY(int_cache_trim(m));
+  BeamRun brun;
+  BeamRun* bm = nullptr;
+  if (bmd) {
+    BeamArgs& a = brun.a;
+    memset(&a, 0, sizeof(a));
+    a.S = d->n_seqs; a.N = bmd->num_beams; a.K = bmd->n_keep; a.V = c.llm_vocab; a.max_new = d->max_new_tokens;
+    a.num_return = bmd->num_return; a.early_stopping = bmd->early_stopping; a.lp_positive = bmd->length_penalty > 0.0 ? 1 : 0;
+    a.n_stop = d->n_stop_ids; a.pad_id = d->pad_id; a.stop_ids = k.st.stop_ids;
+    const size_t layer_stride = (size_t)m->kv_batch * m->kv_cap * c.llm_kv_heads * c.llm_head_dim;
+    a.kc = static_cast<bf16*>(m->kv_cache); a.vc = a.kc + (size_t)c.llm_layers * layer_stride; a.layer_stride = (long long)layer_stride;
+    a.layers = c.llm_layers; a.cap = m->kv_cap; a.kv_dim = c.llm_kv_heads * c.llm_head_dim;
+    a.steps_run = bmd->steps_run; a.out_tokens = d->out_tokens; a.out_lens = d->out_lens; a.beam_indices = bmd->beam_indices;
+    a.seq_scores = bmd->sequence_scores; a.out_logprobs = bmd->logprobs; a.scores = bmd->scores; a.logits = bmd->logits;
+    // HF divides by (len ** length_penalty), a Python float that torch rounds to fp32
+    for (int i = 0; i <= a.max_new; ++i) brun.lp_div.push_back((float)std::pow((double)i, bmd->length_penalty));
+    bm = &brun;
+  }
   m->arena.reset(true);
   DecodeBufs g;
-  FO1_TRY(llm_prefill(m, d, px, sp, sc, mode, k, s, true, g));
+  FO1_TRY(llm_prefill(m, d, px, sp, sc, mode, k, s, true, g, bm));
   FO1_TRY(arena_ensure(m, m->arena.peak));
   m->arena.reset(false);
-  if (d->max_new_tokens > 0) {  // out_tokens pre-filled with pad so an early exit leaves a clean tail
+  if (d->max_new_tokens > 0 && !bm) {  // out_tokens pre-filled with pad so an early exit leaves a clean tail
     const long long n = (long long)d->n_seqs * d->max_new_tokens;
     fill_int_kernel<<<(int)std::min<long long>((n + 255) / 256, 1024), 256, 0, s>>>(d->out_tokens, d->pad_id, n);
     FO1_LAUNCH_CHECK();
     FO1_CUDA(cudaMemsetAsync(d->out_lens, 0, d->n_seqs * sizeof(int), s));
     if (sc && sc->logprobs) FO1_CUDA(cudaMemsetAsync(sc->logprobs, 0, (size_t)n * sizeof(float), s));      // 0 past out_lens
   }
-  FO1_TRY(llm_prefill(m, d, px, sp, sc, mode, k, s, false, g));
+  FO1_TRY(llm_prefill(m, d, px, sp, sc, mode, k, s, false, g, bm));
   if (d->max_new_tokens <= 0) return FO1_OK;
   if (g.mega_grid > 0 && d->max_new_tokens > 1) return decode_persistent(m, d, sc, mode, k, g, s);
-  return decode_per_kernel(m, d, sc, mode, k, g, stm ? stm->progress : nullptr, s);
+  FO1_TRY(decode_per_kernel(m, d, sc, mode, k, g, stm ? stm->progress : nullptr, s));
+  return bm ? beam_finalize(bm->a, s) : FO1_OK;
 }
 
 // -------------------------------------------------------------------------------- splice plan (host, integer)
@@ -1081,6 +1138,12 @@ extern "C" int fo1_llm_generate_prefixed(fo1_model* m, fo1_generate_desc* d, con
                 "progress are required; cancel may be NULL)");
   if (px) FO1_TRY(prefix_check(d, px));
   return llm_generate(m, d, sp, sc, st, static_cast<cudaStream_t>(stream), px);
+}
+
+extern "C" int fo1_llm_generate_beam(fo1_model* m, fo1_generate_desc* d, const fo1_beam_desc* bm, void* stream) {
+  FO1_CHECK_ARG(m && d && bm, "fo1_llm_generate_beam: null argument");
+  FO1_TRY(beam_check(d, bm, m->cfg.llm_vocab));
+  return llm_generate(m, d, nullptr, nullptr, nullptr, static_cast<cudaStream_t>(stream), nullptr, bm);
 }
 
 extern "C" int32_t fo1_stream_progress(const int32_t* progress) { return __atomic_load_n(progress, __ATOMIC_ACQUIRE); }

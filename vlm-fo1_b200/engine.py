@@ -268,13 +268,32 @@ class Prefix:
     seq_group: Sequence[int]
 
 
+@dataclass
+class Beams:
+    """Beam search of a generate call (fo1_beam_desc), one setting for every prompt: ``num_beams`` N in [2, 16]; ``n_keep`` the
+    candidates kept per step, HF's max(2, 1 + number of eos ids) * N; ``length_penalty``; ``early_stopping`` True, False or
+    "never"; ``num_return`` hypotheses per prompt (<= N)."""
+    num_beams: int
+    n_keep: int
+    length_penalty: float = 1.0
+    early_stopping: object = False
+    num_return: int = 1
+
+    def code(self) -> int:
+        if self.early_stopping == "never":
+            return 2
+        if isinstance(self.early_stopping, bool):
+            return int(self.early_stopping)
+        raise ValueError(f"early_stopping must be True, False or 'never', not {self.early_stopping!r}")
+
+
 def _engine_generate(self, inputs_embeds: torch.Tensor, position_ids: torch.Tensor, seq_lens: Sequence[int],
                      rope_deltas: Sequence[int], max_new_tokens: int, stop_ids: Sequence[int], pad_id: int,
                      want_prefill_logits: bool = False, want_all_logits: bool = False, early_exit_interval: int = 8,
                      sampling: Optional[Sampling] = None, want_logprobs: bool = False, want_scores: bool = False,
                      want_logits: bool = False, raw_rows: Optional[Sequence[int]] = None,
                      on_tokens: Optional[Callable[[int, int, "np.ndarray", "np.ndarray"], Optional[bool]]] = None,
-                     prefix: Optional[Prefix] = None):
+                     prefix: Optional[Prefix] = None, beams: Optional[Beams] = None):
     """Prefill + decode of a packed batch: greedy, or sampled per sequence when ``sampling`` is given.  position_ids int32
     [3, sum L].  Returns a dict of device tensors.
 
@@ -291,7 +310,18 @@ def _engine_generate(self, inputs_embeds: torch.Tensor, position_ids: torch.Tens
 
     Shared prefixes (include/fo1.h, fo1_prefix_desc): with ``prefix``, ``seq_lens`` stay the full lengths and ``inputs_embeds`` /
     ``position_ids`` hold only each sequence's rows after its group's prefix.  Every output is bit-identical to the call on the
-    full sequences; ``want_all_logits`` is refused."""
+    full sequences; ``want_all_logits`` is refused.
+
+    Beam search (include/fo1.h, fo1_beam_desc): with ``beams``, every prompt runs HF's beam search on its own N rows.  ``tokens``
+    int32 [B * num_return, max_new] / ``lens`` [B * num_return] hold each prompt's best hypotheses, best first; added are
+    ``sequence_scores`` fp32 [B * num_return], ``beam_indices`` int32 [B * num_return, max_new] (prompt * N + beam, -1 past the
+    length) and ``beam_steps`` int32 [B] (the steps each prompt ran).  ``want_scores`` / ``want_logits`` give [max_new, B * N, V]
+    log-prob / raw rows; ``want_logprobs`` [B * num_return, max_new] the returned tokens' log-probabilities.  Sampling, streaming,
+    prefixes, ``raw_rows`` and ``want_all_logits`` are refused."""
+    if beams is not None:
+        return self._generate_beam(inputs_embeds, position_ids, seq_lens, rope_deltas, max_new_tokens, stop_ids, pad_id, beams,
+                                   want_prefill_logits, early_exit_interval, want_logprobs, want_scores, want_logits, sampling, raw_rows,
+                                   on_tokens, prefix, want_all_logits)
     B = len(seq_lens)
     V = self.cfg.llm["vocab_size"]
     pre = [0] * B
@@ -361,6 +391,60 @@ def _engine_generate(self, inputs_embeds: torch.Tensor, position_ids: torch.Tens
     else:
         self._run_streamed(launch, B, max_new_tokens, on_tokens)
     out = dict(tokens=toks, lens=lens, prefill_logits=pl, all_logits=al, steps_run=d.steps_run)
+    if want_logprobs:
+        out["logprobs"] = lp
+    if want_scores:
+        out["scores"] = sc
+    if want_logits:
+        out["logits"] = lg
+    return out
+
+
+def _engine_generate_beam(self, inputs_embeds, position_ids, seq_lens, rope_deltas, max_new_tokens, stop_ids, pad_id, beams: Beams,
+                          want_prefill_logits, early_exit_interval, want_logprobs, want_scores, want_logits, sampling, raw_rows, on_tokens, prefix,
+                          want_all_logits):
+    """Engine.generate with ``beams`` (fo1_llm_generate_beam)."""
+    for name, v in (("sampling", sampling), ("raw_rows", raw_rows), ("on_tokens", on_tokens), ("prefix", prefix)):
+        if v is not None:
+            raise ValueError(f"beam search does not take `{name}`")
+    if want_all_logits:
+        raise ValueError("beam search does not take `want_all_logits`")
+    B, N, nr = len(seq_lens), int(beams.num_beams), int(beams.num_return)
+    V, T = self.cfg.llm["vocab_size"], max(int(max_new_tokens), 1)
+    assert inputs_embeds.shape == (int(sum(seq_lens)), self.cfg.llm["hidden_size"]) and inputs_embeds.dtype == torch.bfloat16
+    inputs_embeds = inputs_embeds.contiguous()
+    position_ids = position_ids.to(self.device, torch.int32).contiguous()
+    dev = self.device
+    toks = torch.empty((B * nr, T), dtype=torch.int32, device=dev)
+    lens = torch.zeros((B * nr,), dtype=torch.int32, device=dev)
+    seq_scores = torch.empty((B * nr,), dtype=torch.float32, device=dev)
+    bidx = torch.empty((B * nr, T), dtype=torch.int32, device=dev)
+    steps = torch.zeros((B,), dtype=torch.int32, device=dev)
+    pl = torch.empty((B, V), dtype=torch.float32, device=dev) if want_prefill_logits else None
+    sc = torch.empty((T, B * N, V), dtype=torch.float32, device=dev) if want_scores else None
+    lg = torch.empty((T, B * N, V), dtype=torch.float32, device=dev) if want_logits else None
+    lp = torch.empty((B * nr, T), dtype=torch.float32, device=dev) if want_logprobs else None
+    d = GenerateDescC()
+    d.n_seqs = B
+    sl = (C.c_int32 * B)(*[int(x) for x in seq_lens])
+    dev_deltas = rope_deltas if isinstance(rope_deltas, torch.Tensor) else None
+    rd = (C.c_int32 * B)(*([0] * B if dev_deltas is not None else [int(x) for x in rope_deltas]))
+    if dev_deltas is not None:
+        assert dev_deltas.is_cuda and dev_deltas.dtype == torch.int32 and dev_deltas.numel() == B
+        d.rope_deltas_device = dev_deltas.data_ptr()
+    st = (C.c_int32 * max(len(stop_ids), 1))(*[int(x) for x in stop_ids])
+    d.seq_lens, d.rope_deltas, d.stop_ids, d.n_stop_ids = sl, rd, st, len(stop_ids)
+    d.inputs_embeds, d.position_ids = inputs_embeds.data_ptr(), position_ids.data_ptr()
+    d.max_new_tokens, d.pad_id = max_new_tokens, pad_id
+    d.out_tokens, d.out_lens = toks.data_ptr(), lens.data_ptr()
+    d.prefill_logits = pl.data_ptr() if pl is not None else None
+    d.early_exit_interval = early_exit_interval
+    ptr = lambda t: t.data_ptr() if t is not None else None
+    bd = _lib.BeamDesc(N, int(beams.n_keep), float(beams.length_penalty), beams.code(), nr, seq_scores.data_ptr(), bidx.data_ptr(),
+                       steps.data_ptr(), ptr(sc), ptr(lg), ptr(lp))
+    check(lib().fo1_llm_generate_beam(self._h, C.byref(d), C.byref(bd), _stream()), "fo1_llm_generate_beam")
+    out = dict(tokens=toks, lens=lens, prefill_logits=pl, all_logits=None, steps_run=d.steps_run, sequence_scores=seq_scores,
+               beam_indices=bidx, beam_steps=steps)
     if want_logprobs:
         out["logprobs"] = lp
     if want_scores:
@@ -496,6 +580,7 @@ def _engine_run_streamed(self, launch, B: int, T: int, on_tokens) -> None:
 
 Engine.build_embeds = _engine_build_embeds
 Engine.generate = _engine_generate
+Engine._generate_beam = _engine_generate_beam
 Engine._stream_buffers = _engine_stream_buffers
 Engine._run_streamed = _engine_run_streamed
 Engine.sample_tokens = staticmethod(sample_tokens)

@@ -148,6 +148,54 @@ class Fo1ForCausalLM:
             T.append(t); P.append(p); K.append(k)
         return E.Sampling(T, P, K, seeds)
 
+    def _beams(self, do_sample, kwargs):
+        """None (num_beams 1) or the engine.Beams of a beam-search call, from the call's kwargs, else generation_config.json, else
+        HF's defaults.  Beam sampling is refused by _sampling_params; group, diverse and constrained beam search here."""
+        gc = self.generation_config
+        get = lambda name, default: kwargs[name] if kwargs.get(name) is not None else gc.get(name, default)
+        N = get("num_beams", 1)
+        N = 1 if N is None else int(N)
+        if N <= 1 or do_sample:
+            return None
+        if (get("num_beam_groups", 1) or 1) > 1 or (get("diversity_penalty", 0.0) or 0.0) != 0.0:
+            raise NotImplementedError("group / diverse beam search (num_beam_groups, diversity_penalty) is not supported by the fo1-b200 "
+                                      "engine (it implements beam search)")
+        if get("constraints", None) is not None or get("force_words_ids", None) is not None:
+            raise NotImplementedError("constrained beam search (constraints, force_words_ids) is not supported by the fo1-b200 engine")
+        n = self._num_return_sequences(kwargs)
+        if n > N:
+            raise ValueError(f"`num_return_sequences` ({n}) has to be smaller or equal to `num_beams` ({N}).")
+        lp = get("length_penalty", 1.0)
+        es = get("early_stopping", False)
+        if es not in (True, False, "never"):
+            raise ValueError(f"`early_stopping` must be a boolean or 'never', but is {es}.")
+        E = import_module("vlm-fo1_b200.engine")
+        eos = gc.get("eos_token_id", self.default_stop_ids)
+        n_eos = len(eos) if isinstance(eos, (list, tuple)) else int(eos is not None)
+        return E.Beams(num_beams=N, n_keep=max(2, 1 + n_eos) * N, length_penalty=float(1.0 if lp is None else lp), early_stopping=es,
+                       num_return=n)
+
+    def _beam_result(self, out, b, inputs, want, beams, b_local=0):
+        """Prompt b of a beam-search engine output -> what HF's generate returns: LongTensor [num_return, P + T] (T: the longest
+        returned hypothesis, pad after each one's end) or GenerateBeamDecoderOnlyOutput.  Beam indices are made relative to prompt
+        b_local, as a call with that prompt alone returns them."""
+        N, nr = beams.num_beams, beams.num_return
+        rows = slice(b * nr, (b + 1) * nr)
+        lens = out["lens"][rows]
+        T = max(int(x) for x in lens)
+        new = out["tokens"][rows, :T].to(torch.long)
+        full = torch.cat([inputs[0].to(new.device).expand(nr, -1), new], 1)
+        if want is None:
+            return full
+        from transformers.generation.utils import GenerateBeamDecoderOnlyOutput
+        steps = int(out["beam_steps"][b])
+        block = lambda key: tuple(out[key][t, b * N:(b + 1) * N] for t in range(steps))
+        bi = out["beam_indices"][rows, :T]
+        bi = torch.where(bi >= 0, bi - (b - b_local) * N, bi)
+        return GenerateBeamDecoderOnlyOutput(sequences=full, sequences_scores=out["sequence_scores"][rows] if want[0] else None,
+                                             scores=block("scores") if want[0] else None, logits=block("logits") if want[1] else None,
+                                             beam_indices=bi, past_key_values=None)
+
     def _num_return_sequences(self, kwargs):
         n = kwargs.get("num_return_sequences")
         n = self.generation_config.get("num_return_sequences", 1) if n is None else n
@@ -174,8 +222,18 @@ class Fo1ForCausalLM:
     def generate(self, inputs=None, images=None, images_aux=None, image_grid_thws=None, bbox_list=None, do_sample=False, temperature=0.0,
                  max_new_tokens=512, streamer=None, top_p=1.0, use_cache=True, stopping_criteria=None, pad_token_id=None, top_k=None, **kwargs):
         want = self._outputs(kwargs)
+        beams = self._beams(do_sample, kwargs)
         n = self._num_return_sequences(kwargs)
         kwargs.pop("num_return_sequences", None)
+        if beams is not None:
+            if streamer is not None:
+                raise ValueError("`streamer` cannot be used with beam search (yet!). Make sure that `num_beams` is set to 1.")
+            sample, stop, _ = self._sample(inputs, images, images_aux, image_grid_thws, bbox_list, do_sample, temperature, stopping_criteria,
+                                           top_p, top_k, **kwargs)
+            out = self.pipeline.generate([sample], int(max_new_tokens), sorted(set(stop)), pad_id=int(self._beam_pad(pad_token_id, stop)),
+                                         early_exit_interval=8, want_scores=bool(want and want[0]), want_logits=bool(want and want[1]),
+                                         beams=beams)
+            return self._beam_result(out, 0, inputs, want, beams)
         if n > 1 and not do_sample:
             raise ValueError("Greedy methods without beam search do not support `num_return_sequences` different than 1 "
                              f"(got {n}).")
@@ -208,6 +266,12 @@ class Fo1ForCausalLM:
             streamer.end()
         return res
 
+    def _beam_pad(self, pad_token_id, stop):
+        """HF's beam-search fill value: ``pad_token_id or eos_token_id[0]``."""
+        eos = self.generation_config.get("eos_token_id", self.default_stop_ids)
+        eos = list(eos) if isinstance(eos, (list, tuple)) else ([eos] if eos is not None else list(stop))
+        return pad_token_id or (eos[0] if eos else 0)
+
     @torch.no_grad()
     def generate_batch(self, batch, max_new_tokens=None, output_logprobs=False):
         """``batch``: a list of the dicts ``prepare_inputs`` returns (one sample each, mm_utils.py:640-654).  All samples run as ONE
@@ -218,6 +282,9 @@ class Fo1ForCausalLM:
         if not batch:
             return []
         wants = [self._outputs(kw) for kw in batch]
+        beams = [self._beams(kw.get("do_sample", False), kw) for kw in batch]
+        if any(b is not None for b in beams):
+            return self._generate_batch_beams(batch, beams, wants, max_new_tokens, output_logprobs)
         if any(self._num_return_sequences(kw) != 1 for kw in batch):
             raise NotImplementedError("num_return_sequences > 1 in generate_batch: call generate for such a sample, or repeat it in the batch")
         keys = ("inputs", "images", "images_aux", "image_grid_thws", "bbox_list", "do_sample", "temperature", "stopping_criteria", "top_p",
@@ -238,4 +305,30 @@ class Fo1ForCausalLM:
         for b, kw in enumerate(batch):
             r = self._result(out, b, kw["inputs"], wants[b])
             res.append((r, out["logprobs"][b:b + 1, :out["lens"][b]]) if output_logprobs else r)
+        return res
+
+    def _generate_batch_beams(self, batch, beams, wants, max_new_tokens, output_logprobs):
+        """generate_batch of beam-search samples: one packed engine call when every sample asks for the same beam setting.  With
+        ``output_logprobs`` each element carries fp32 [num_return, T], the returned tokens' log-probabilities gathered along their
+        beam paths on the device (HF's compute_transition_scores(sequences, scores, beam_indices), 0 past each hypothesis' end)."""
+        if any(b != beams[0] for b in beams):
+            raise NotImplementedError("generate_batch runs beam search as one call: every sample must use the same num_beams, "
+                                      "length_penalty, early_stopping and num_return_sequences (call generate for the others)")
+        keys = ("inputs", "images", "images_aux", "image_grid_thws", "bbox_list", "do_sample", "temperature", "stopping_criteria", "top_p",
+                "top_k") + tuple(n for n, _ in _UNSUPPORTED_PROCESSORS)
+        samples, stops, _ = zip(*(self._sample(**{k: v for k, v in kw.items() if k in keys}) for kw in batch))
+        stop = sorted(set(x for s in stops for x in s))
+        T = int(max_new_tokens if max_new_tokens is not None else max(int(kw.get("max_new_tokens", 512)) for kw in batch))
+        pad = self._beam_pad(batch[0].get("pad_token_id"), stop)
+        out = self.pipeline.generate(list(samples), T, stop, pad_id=int(pad), early_exit_interval=8, want_logprobs=bool(output_logprobs),
+                                     want_scores=any(w is not None and w[0] for w in wants),
+                                     want_logits=any(w is not None and w[1] for w in wants), beams=beams[0])
+        nr = beams[0].num_return
+        res = []
+        for b, kw in enumerate(batch):
+            r = self._beam_result(out, b, kw["inputs"], wants[b], beams[0])
+            if output_logprobs:
+                width = int(out["lens"][b * nr:(b + 1) * nr].max())
+                r = (r, out["logprobs"][b * nr:(b + 1) * nr, :width])
+            res.append(r)
         return res
