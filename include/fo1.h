@@ -535,6 +535,39 @@ typedef struct {
  * length_penalty, early_stopping in {0, 1, 2}, max_new_tokens >= 1, the outputs non-NULL and no all_logits. */
 int fo1_llm_generate_beam(fo1_model* m, fo1_generate_desc* d, const fo1_beam_desc* bm, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Prompt-lookup decoding (HF generate's prompt_lookup_num_tokens / max_matching_ngram_size).  Each sequence's corpus is its
+ * prompt ids as the caller passes them (placeholders included), followed by every token it has emitted.  Per step, the drafts are
+ * HF's PromptLookupCandidateGenerator.get_candidates: for n = min(max_ngram, len - 1) down to 1, the leftmost occurrence of the
+ * last n ids with a non-empty continuation gives up to K following ids, cut at the first stop id.  The engine also cuts them at
+ * the first negative id, caps them at max_new_tokens - emitted - 1 and K at 16.  One verify step runs B * (K + 1) rows, each
+ * bit-identical to the plain per-kernel step's row for that position; the longest draft prefix equal to the rows' tokens is
+ * accepted and n_matches + 1 tokens are emitted (stopping at a stop id or max_new_tokens).  So tokens, lengths and the score
+ * outputs (rows up to each length) equal those of the plain per-kernel call (FO1_NO_MEGA=1), greedy, sampled or scored.  Always
+ * the per-kernel decode path; the K/V cache slot grows by K rows.  steps_run is the number of verify steps the loop ran: with
+ * early_exit_interval > 0 the loop polls after every verify step, one step behind (at most one step runs after the last sequence
+ * ends); with 0 it never polls and runs max_new_tokens - 1 steps.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct {
+  int32_t num_tokens;               /* K >= 1 (drafts per step; more than 16 proposes 16) */
+  int32_t max_ngram;                /* >= 1 */
+  const int32_t* corpus;            /* HOST int32, the n_seqs corpora packed */
+  const int32_t* corpus_offsets;    /* HOST int32 [n_seqs + 1]: corpus b is corpus[offsets[b] .. offsets[b + 1]) */
+  int32_t* steps;                   /* optional DEVICE int32 [n_seqs]: verify steps the sequence took part in */
+  int32_t* accepted;                /* optional DEVICE int32 [n_seqs]: drafts accepted */
+} fo1_lookup_desc;
+/* Checked on the host before any CUDA call: num_tokens >= 1, max_ngram >= 1, corpus offsets present, starting at 0 and
+ * non-decreasing, corpus present when non-empty; with px, the checks of fo1_llm_generate_prefixed.  sp / sc as in
+ * fo1_llm_generate_scored; px as in fo1_llm_generate_prefixed (the prefill is unchanged). */
+int fo1_llm_generate_lookup(fo1_model* m, fo1_generate_desc* d, const fo1_lookup_desc* lk, const fo1_prefix_desc* px /* NULL */,
+                            const fo1_sampling_desc* sp /* NULL: greedy */, const fo1_score_desc* sc /* NULL: unscored */, void* stream);
+/* The draft rule alone: corpora DEVICE int32 [n_seqs][ld] with lengths lens [n_seqs] -> drafts DEVICE int32 [n_seqs][num_tokens]
+ * and n_draft [n_seqs].  stop_ids DEVICE [n_stop]; emitted (DEVICE [n_seqs], optional) with max_new_tokens caps the drafts at
+ * max_new_tokens - emitted - 1.  1 <= num_tokens <= 16, max_ngram >= 1. */
+int fo1_lookup_drafts(const int32_t* corpus, int64_t ld, const int32_t* lens, int32_t n_seqs, int32_t num_tokens, int32_t max_ngram,
+                      const int32_t* stop_ids, int32_t n_stop, const int32_t* emitted, int32_t max_new_tokens, int32_t* drafts,
+                      int32_t* n_draft, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -101,6 +101,13 @@ class BeamDesc(C.Structure):
                 ("scores", C.c_void_p), ("logits", C.c_void_p), ("logprobs", C.c_void_p)]
 
 
+class LookupDesc(C.Structure):
+    """fo1_lookup_desc: HOST num_tokens, max_ngram, packed corpus int32 and offsets [n + 1]; optional DEVICE int32 [n] outputs steps /
+    accepted."""
+    _fields_ = [("num_tokens", C.c_int32), ("max_ngram", C.c_int32), ("corpus", C.POINTER(C.c_int32)),
+                ("corpus_offsets", C.POINTER(C.c_int32)), ("steps", C.c_void_p), ("accepted", C.c_void_p)]
+
+
 FO1_STREAM_DONE = 1 << 30
 
 _lib = None
@@ -151,6 +158,12 @@ def lib() -> C.CDLL:
                                             C.POINTER(StreamDesc), C.c_void_p]
     L.fo1_llm_generate_beam.restype = C.c_int
     L.fo1_llm_generate_beam.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(BeamDesc), C.c_void_p]
+    L.fo1_llm_generate_lookup.restype = C.c_int
+    L.fo1_llm_generate_lookup.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(LookupDesc), C.POINTER(PrefixDesc), C.POINTER(SamplingDesc),
+                                          C.POINTER(ScoreDesc), C.c_void_p]
+    L.fo1_lookup_drafts.restype = C.c_int
+    L.fo1_lookup_drafts.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p,
+                                    C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     L.fo1_prefix_attention.restype = C.c_int
     L.fo1_prefix_attention.argtypes = [C.POINTER(PrefixAttnDesc), C.c_void_p]
     L.fo1_stream_progress.restype = C.c_int32

@@ -82,6 +82,16 @@ struct SplitKScope {
   explicit SplitKScope(bool on) : prev(t_splitk_ok) { t_splitk_ok = on; }
   ~SplitKScope() { t_splitk_ok = prev; }
 };
+// Inside a GemmChoiceScope(m) the automatic tile-width and split-K choice of gemm_bf16 is the one it makes for M = m, whatever the
+// launch's own M.  The prompt-lookup verify step runs B * (K + 1) rows through GEMMs that must sum every row in the order the plain
+// decode step (M = B) uses; the choice depends on M only through ceil(M / 128), so without the scope a verify step above 128 rows
+// would take another split.  0: the launch's own M.
+extern thread_local int t_gemm_choice_m;
+struct GemmChoiceScope {
+  int prev;
+  explicit GemmChoiceScope(int m) : prev(t_gemm_choice_m) { t_gemm_choice_m = m; }
+  ~GemmChoiceScope() { t_gemm_choice_m = prev; }
+};
 #ifdef __CUDACC__
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args&&... args) {

@@ -730,7 +730,7 @@ int gemm_bf16(const fo1_gemm_desc* d, cudaStream_t stream) {
   }
   // tile-width choice: widest tile that still yields >= 1 wave of CTAs, else narrower for occupancy
   const int sms = device_sm_count();
-  const long long tm = ceil_div(d->M, BM);
+  const long long tm = ceil_div(t_gemm_choice_m > 0 ? t_gemm_choice_m : d->M, BM);   // (GemmChoiceScope: see common.cuh)
   if (d->N >= 256 && tm * ceil_div(d->N, 256) >= sms) return launch_gemm<256>(d, stream);
   // weight-streaming problems whose 128-wide tiles need a second, mostly empty wave (decode gate/up: 172 tiles on 132 SMs)
   // run as ONE wave of 192-wide tiles instead

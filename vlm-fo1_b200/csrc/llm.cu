@@ -16,6 +16,7 @@
 #include "beam.cuh"
 #include "decode_loop.cuh"
 #include "decode_mega.cuh"
+#include "lookup.cuh"
 
 namespace fo1 {
 
@@ -247,6 +248,144 @@ __global__ void __launch_bounds__(kDecWarps * 32) decode_attn_kernel(const bf16*
   }
 }
 
+// The prompt-lookup verify step's decode attention: decode_attn_kernel with query row b = blockIdx.x reading cache slot row_slot[b]
+// up to its own index idx[b].  A separate copy, so that decode_attn_kernel keeps its code; the arithmetic of each (row, split) is
+// decode_attn_kernel's, and the launch takes the plain step's split count, so a row's bits are those of the plain step at its position.
+__global__ void __launch_bounds__(kDecWarps * 32) decode_attn_rows_kernel(const bf16* __restrict__ q, long long ldq, const bf16* __restrict__ kc,
+                                                                          const bf16* __restrict__ vc, const int* __restrict__ row_slot,
+                                                                          const int* __restrict__ idx, int cap, int kv_heads, int G,
+                                                                          float* __restrict__ part, float scale) {
+  constexpr int HD = 128;
+  extern __shared__ __align__(128) uint8_t dec_smem[];
+  const int b = blockIdx.x, kvh = blockIdx.y, sp = blockIdx.z;
+  griddep_launch();
+  griddep_wait();
+  const int slot = row_slot[b];
+  const int n = idx[b] + 1;        // the row's own K/V was appended at index idx[b]
+  const int n_splits = gridDim.z;
+  const int chunk = ((n + n_splits - 1) / n_splits + 15) & ~15;
+  const int t_begin = sp * chunk, t_end = min(n, t_begin + chunk);
+  const int kv_dim = kv_heads * HD;
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int g = lane >> 2, t = lane & 3;
+  // Q fragments (A operand, rows = heads): a0 = dims (16 ks + 2t, +1), a2 = dims (16 ks + 8 + 2t, +1) of head g
+  uint32_t qa[8][2];
+#pragma unroll
+  for (int ks = 0; ks < 8; ++ks) { qa[ks][0] = 0u; qa[ks][1] = 0u; }
+  if (g < G) {
+    const bf16* qp = q + (long long)b * ldq + (long long)(kvh * G + g) * HD + 2 * t;
+#pragma unroll
+    for (int ks = 0; ks < 8; ++ks) {
+      qa[ks][0] = *reinterpret_cast<const uint32_t*>(qp + ks * 16);
+      qa[ks][1] = *reinterpret_cast<const uint32_t*>(qp + ks * 16 + 8);
+    }
+  }
+  const float sc = scale * 1.4426950408889634f;
+  float m = -INFINITY, l = 0.f, o[16][4];
+#pragma unroll
+  for (int j = 0; j < 16; ++j) { o[j][0] = o[j][1] = o[j][2] = o[j][3] = 0.f; }
+
+  const uint32_t ring = (uint32_t)__cvta_generic_to_shared(dec_smem) + w * kDecStages * kDecTileBytes;
+  // copy plan: instruction i moves chunk (key = 2i + lane/16, 16-byte chunk lane%16) of the K half and of the V half
+  const int cp_key = lane >> 4, cp_chunk = lane & 15;
+  const bf16* kbase = kc + (long long)slot * cap * kv_dim + kvh * HD + cp_chunk * 8;
+  const bf16* vbase = vc + (long long)slot * cap * kv_dim + kvh * HD + cp_chunk * 8;
+  int t_issue = t_begin + w * 16;
+  uint32_t st_issue = 0, st_done = 0;
+  auto issue_tile = [&]() {
+    if (t_issue < t_end) {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int key = 2 * i + cp_key, tok = t_issue + key;
+        const bool ok = tok < t_end;                          // keys beyond the split: zero rows (their scores are masked)
+        const long long off = (long long)(ok ? tok : t_begin) * kv_dim;
+        const uint32_t dst = ring + st_issue + key * 256 + ((cp_chunk ^ (key & 7)) << 4);
+        dec_cp16(dst, kbase + off, ok);
+        dec_cp16(dst + 16 * 256, vbase + off, ok);
+      }
+      t_issue += kDecWarps * 16;
+      st_issue = (st_issue == (kDecStages - 1) * kDecTileBytes) ? 0u : st_issue + kDecTileBytes;
+    }
+    asm volatile("cp.async.commit_group;" ::: "memory");
+  };
+  issue_tile();
+  issue_tile();
+  // ldmatrix lane roles: S: matrix m = lane/8 -> (keys (m/2)*8 + r, chunk 2 ks + (m&1)); PV (trans): (keys (m&1)*8 + r, chunk c + m/2)
+  const int lr = lane & 7, lm = lane >> 3;
+  for (int t0 = t_begin + w * 16; t0 < t_end; t0 += kDecWarps * 16) {
+    issue_tile();
+    asm volatile("cp.async.wait_group 2;" ::: "memory");
+    __syncwarp();
+    const uint32_t kt = ring + st_done, vt = kt + 16 * 256;
+    float s[2][4];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) { s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f; }
+#pragma unroll
+    for (int ks = 0; ks < 8; ++ks) {
+      uint32_t bk[4];
+      const int key = (lm >> 1) * 8 + lr;
+      dec_ldsm(bk, kt + key * 256 + (((2 * ks + (lm & 1)) ^ (key & 7)) << 4));
+      mma_m16n8k16(s[0], qa[ks][0], qa[ks][1], bk[0], bk[1]);
+      mma_m16n8k16(s[1], qa[ks][0], qa[ks][1], bk[2], bk[3]);
+    }
+    float tmax = -INFINITY;
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        s[i][e] = (t0 + i * 8 + 2 * t + e < t_end) ? s[i][e] * sc : -INFINITY;
+        tmax = fmaxf(tmax, s[i][e]);
+      }
+    tmax = fmaxf(tmax, __shfl_xor_sync(0xffffffffu, tmax, 1));
+    tmax = fmaxf(tmax, __shfl_xor_sync(0xffffffffu, tmax, 2));
+    const float mn = fmaxf(m, tmax);            // key t0 is always valid: mn is finite
+    const float alpha = exp2f(m - mn);          // m = -inf on the first tile -> 0
+    const float p00 = exp2f(s[0][0] - mn), p01 = exp2f(s[0][1] - mn), p10 = exp2f(s[1][0] - mn), p11 = exp2f(s[1][1] - mn);
+    l = l * alpha + (p00 + p01) + (p10 + p11);
+    m = mn;
+    const uint32_t pa0 = pack2_bf16(p00, p01), pa2 = pack2_bf16(p10, p11);
+#pragma unroll
+    for (int c = 0; c < 16; c += 2) {
+      uint32_t bv[4];
+      const int key = (lm & 1) * 8 + lr;
+      dec_ldsm_t(bv, vt + key * 256 + (((c + (lm >> 1)) ^ (key & 7)) << 4));
+      o[c][0] *= alpha; o[c][1] *= alpha; o[c + 1][0] *= alpha; o[c + 1][1] *= alpha;
+      mma_m16n8k16(o[c], pa0, pa2, bv[0], bv[1]);
+      mma_m16n8k16(o[c + 1], pa0, pa2, bv[2], bv[3]);
+    }
+    __syncwarp();                               // the stage may be refilled by the next issue_tile()
+    st_done = (st_done == (kDecStages - 1) * kDecTileBytes) ? 0u : st_done + kDecTileBytes;
+  }
+  asm volatile("cp.async.wait_group 0;" ::: "memory");
+  l += __shfl_xor_sync(0xffffffffu, l, 1);
+  l += __shfl_xor_sync(0xffffffffu, l, 2);
+  __syncthreads();                              // every warp is done with its ring: reuse it for the merge
+  float* sm_o = reinterpret_cast<float*>(dec_smem);                    // [kDecWarps][8][HD]
+  float* sm_m = sm_o + kDecWarps * 8 * HD;                             // [kDecWarps][8]
+  float* sm_l = sm_m + kDecWarps * 8;
+  if (t == 0) { sm_m[w * 8 + g] = m; sm_l[w * 8 + g] = l; }
+#pragma unroll
+  for (int j = 0; j < 16; ++j)
+    *reinterpret_cast<float2*>(&sm_o[(w * 8 + g) * HD + j * 8 + 2 * t]) = make_float2(o[j][0], o[j][1]);
+  __syncthreads();
+  const int d = threadIdx.x;   // kDecWarps * 32 == HD
+  for (int r = 0; r < G; ++r) {
+    float mm = -INFINITY;
+#pragma unroll
+    for (int ww = 0; ww < kDecWarps; ++ww) mm = fmaxf(mm, sm_m[ww * 8 + r]);
+    float num = 0.f, den = 0.f;
+#pragma unroll
+    for (int ww = 0; ww < kDecWarps; ++ww) {
+      const float f = (sm_m[ww * 8 + r] == -INFINITY) ? 0.f : exp2f(sm_m[ww * 8 + r] - mm);
+      num += sm_o[(ww * 8 + r) * HD + d] * f;
+      den += sm_l[ww * 8 + r] * f;
+    }
+    // partial record per (b, head, split): [m, l, pad, pad, acc[128]]
+    float* rec = part + (((long long)b * kv_heads * G + kvh * G + r) * kDecSplits + sp) * (HD + 4);
+    if (d == 0) { rec[0] = mm; rec[1] = den; }
+    rec[4 + d] = num;
+  }
+}
 // merge the kDecSplits partials of one (sequence, q head): out = sum_s acc_s * 2^(m_s - m) / sum_s l_s * 2^(m_s - m)
 __global__ void __launch_bounds__(128) decode_attn_combine_kernel(const float* __restrict__ part, bf16* __restrict__ out, long long ldo,
                                                                   int q_heads, int n_splits) {
@@ -269,9 +408,12 @@ __global__ void __launch_bounds__(128) decode_attn_combine_kernel(const float* _
   out[(long long)b * ldo + (long long)h * HD + d] = __float2bfloat16_rn(num / den);
 }
 
-// host side of the decode attention: split count = one wave of blocks (2 per SM: 96 KB of shared memory each)
+// host side of the decode attention: split count = one wave of blocks (2 per SM: 96 KB of shared memory each).  row_slot (the
+// prompt-lookup verify step): row r reads slot row_slot[r] up to index cache_len[r] (then a per-row index), and the split count is
+// the one of the plain step over n_seqs sequences, so each row's key chunks are those the plain step at its position would use
 static int decode_attention(const bf16* q, long long ldq, const bf16* kc, const bf16* vc, const int* cache_len, int rows, int cap,
-                            int q_heads, int kv_heads, int hd, float scale, bf16* out, long long ldo, float* part, cudaStream_t s) {
+                            int q_heads, int kv_heads, int hd, float scale, bf16* out, long long ldo, float* part, cudaStream_t s,
+                            const int* row_slot = nullptr, int n_seqs = 0) {
   const int G = kv_heads > 0 ? q_heads / kv_heads : 0;
   if (kv_heads <= 0 || q_heads % kv_heads != 0 || G > 8 || hd != 128) {
     set_error("decode attention: %d/%d heads, head_dim %d unsupported (GQA group <= 8, head_dim 128)", q_heads, kv_heads, hd);
@@ -279,12 +421,22 @@ static int decode_attention(const bf16* q, long long ldq, const bf16* kc, const 
   }
   if (rows == 0) return FO1_OK;
   static bool attr_set = false;
-  if (!attr_set) { FO1_CUDA(cudaFuncSetAttribute(decode_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kDecSmemBytes)); attr_set = true; }
+  if (!attr_set) {
+    FO1_CUDA(cudaFuncSetAttribute(decode_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kDecSmemBytes));
+    FO1_CUDA(cudaFuncSetAttribute(decode_attn_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kDecSmemBytes));
+    attr_set = true;
+  }
   const int slots = 2 * device_sm_count();
-  const int n_splits = std::max(1, std::min(kDecSplits, slots / std::max(1, rows * kv_heads)));
+  const int n_splits = std::max(1, std::min(kDecSplits, slots / std::max(1, (row_slot ? n_seqs : rows) * kv_heads)));
   dim3 grid(rows, kv_heads, n_splits);
-  ProfScope prof("decode_attn", 0.0, 0.0, s);
-  launch_k(decode_attn_kernel, grid, dim3(kDecWarps * 32), kDecSmemBytes, s, q, ldq, kc, vc, cache_len, cap, kv_heads, G, part, scale);
+  if (row_slot != nullptr) {
+    ProfScope prof("decode_attn_rows", 0.0, 0.0, s);
+    launch_k(decode_attn_rows_kernel, grid, dim3(kDecWarps * 32), kDecSmemBytes, s, q, ldq, kc, vc, row_slot, cache_len, cap, kv_heads, G,
+             part, scale);
+  } else {
+    ProfScope prof("decode_attn", 0.0, 0.0, s);
+    launch_k(decode_attn_kernel, grid, dim3(kDecWarps * 32), kDecSmemBytes, s, q, ldq, kc, vc, cache_len, cap, kv_heads, G, part, scale);
+  }
   FO1_LAUNCH_CHECK();
   launch_k(decode_attn_combine_kernel, dim3(rows, q_heads), dim3(128), 0, s, (const float*)part, out, ldo, q_heads, n_splits);
   FO1_LAUNCH_CHECK();
@@ -476,7 +628,8 @@ struct PrefixTables {
 // + cache fill (px: the shared-prefix split of it); decode: cache append + single-query attention.
 struct LayerBuf { bf16 *xn, *qkv, *att, *x_mid, *h; float* dec_part; int* rowseg = nullptr; double attn_flops = 0.0; const int* tiles = nullptr; int n_tiles = 0;
                   const PrefixTables* px = nullptr;
-                  const int *fan_gt = nullptr, *fan_off = nullptr, *fan_mem = nullptr; };   // beam search: each prompt row into its N slots
+                  const int *fan_gt = nullptr, *fan_off = nullptr, *fan_mem = nullptr;    // beam search: each prompt row into its N slots
+                  const int *row_slot = nullptr, *row_idx = nullptr; int n_seqs = 0; };   // prompt-lookup verify: rows of n_seqs slots
 
 // the prefill attention of a shared-prefix layer: prefix K/V into every member's slot, own K/V into the own slot, then the prefix rows
 // as causal segments and the own rows against the cache
@@ -540,9 +693,10 @@ static int llm_layer(Model* m, int li, const bf16* x_in, bf16* x_out, const Laye
     a.scale = 1.0f / sqrtf((float)hd); a.causal = 1;
     FO1_RUN(attention_varlen(a, s));
   } else if (!dry) {
-    FO1_RUN(rope_kv_append(B_.qkv, ldq, cs, rows, c.llm_heads, c.llm_kv_heads, hd, st->cache_len, kc, vc, m->kv_cap, s));
-    FO1_RUN(decode_attention(B_.qkv, ldq, kc, vc, st->cache_len, rows, m->kv_cap, c.llm_heads, c.llm_kv_heads, hd,
-                             1.0f / sqrtf((float)hd), B_.att, QD, B_.dec_part, s));
+    const int* idx = B_.row_slot ? B_.row_idx : st->cache_len;
+    FO1_RUN(rope_kv_append(B_.qkv, ldq, cs, rows, c.llm_heads, c.llm_kv_heads, hd, idx, kc, vc, m->kv_cap, s, B_.row_slot));
+    FO1_RUN(decode_attention(B_.qkv, ldq, kc, vc, idx, rows, m->kv_cap, c.llm_heads, c.llm_kv_heads, hd,
+                             1.0f / sqrtf((float)hd), B_.att, QD, B_.dec_part, s, B_.row_slot, B_.n_seqs));
   }
   FO1_RUN(linear(B_.att, QD, L.o_w, QD, B_.x_mid, H, FO1_BF16, rows, H, QD, nullptr, 0, FO1_EPI_NONE, x_in, H, 0, s));
   FO1_RUN(rmsnorm(B_.x_mid, H, L.ln2, B_.xn, H, rows, H, c.rms_eps, nk, s));
@@ -560,12 +714,19 @@ struct DecodeBufs {
   int *mg_amax_i, *mg_sync, *samp_tok;
   SampleRowParams* samp;
   BeamArgs* beam = nullptr;       // DEC_BEAM
+  LookupArgs* lk = nullptr;       // prompt lookup (lookup.cuh)
 };
 
 // a beam-search call: the device state (beam.cuh) and the host table of length-penalty divisors
 struct BeamRun {
   BeamArgs a;
   std::vector<float> lp_div;
+};
+
+// a prompt-lookup call: the device state (lookup.cuh) and the caller's descriptor
+struct LookupRun {
+  LookupArgs a;
+  const fo1_lookup_desc* desc;
 };
 
 // the tokens of the current output column into new_tok (scored: also the column's scores), then their recording; every kernel reads
@@ -628,7 +789,8 @@ static int prefix_tables(Model* m, const fo1_generate_desc* d, const fo1_prefix_
 }
 
 static int llm_prefill(Model* m, fo1_generate_desc* d, const fo1_prefix_desc* px, const fo1_sampling_desc* sp, const fo1_score_desc* sc,
-                       DecodeMode mode, const ColumnSink& k, cudaStream_t s, bool dry, DecodeBufs& g, BeamRun* bm = nullptr) {
+                       DecodeMode mode, const ColumnSink& k, cudaStream_t s, bool dry, DecodeBufs& g, BeamRun* bm = nullptr,
+                       LookupRun* lk = nullptr) {
   const fo1_model_config& c = m->cfg;
   Arena& A = m->arena;
   const int B = d->n_seqs, H = c.llm_hidden, hd = c.llm_head_dim, V = c.llm_vocab;
@@ -639,7 +801,7 @@ static int llm_prefill(Model* m, fo1_generate_desc* d, const fo1_prefix_desc* px
   for (int b = 0; b < B; ++b) { T += d->seq_lens[b] - prefix_of(px, b); max_len = std::max(max_len, d->seq_lens[b]); }
   for (int gi = 0; px && gi < px->n_groups; ++gi) n_pre += px->prefix_lens[gi];
   T += n_pre;
-  const int RD = bm ? B * bm->a.N : B;      // rows of a decode step: one per sequence, or one per beam
+  const int RD = bm ? B * bm->a.N : lk ? B * (lk->a.K + 1) : B;   // rows of a decode step: one per sequence, beam or verify row
   const int R = (int)std::max<long long>(T, RD);
 
   g = DecodeBufs();
@@ -668,7 +830,7 @@ static int llm_prefill(Model* m, fo1_generate_desc* d, const fo1_prefix_desc* px
   // FO1_MEGA_MAX_B lowers the threshold, FO1_NO_MEGA disables the kernel.
   int mega_max_b = 32;
   if (const char* e = getenv("FO1_MEGA_MAX_B")) mega_max_b = std::max(0, std::min(32, atoi(e)));
-  g.mega_grid = (m->llm.mega_ok && !bm && B <= mega_max_b && getenv("FO1_NO_MEGA") == nullptr) ? decode_mega_grid() : 0;
+  g.mega_grid = (m->llm.mega_ok && !bm && !lk && B <= mega_max_b && getenv("FO1_NO_MEGA") == nullptr) ? decode_mega_grid() : 0;
   g.mg_ssq = A.alloc<float>((size_t)2 * std::max(g.mega_grid, 1) * 32);
   g.mg_amax_v = A.alloc<float>((size_t)std::max(g.mega_grid, 1) * 32);
   g.mg_amax_i = A.alloc<int>((size_t)std::max(g.mega_grid, 1) * 32);
@@ -679,6 +841,10 @@ static int llm_prefill(Model* m, fo1_generate_desc* d, const fo1_prefix_desc* px
   if (bm) {   // beam search: its state and scratch (sized by the dry run like everything else)
     beam_alloc(A, bm->a);
     g.beam = &bm->a;
+  }
+  if (lk) {
+    lookup_alloc(A, lk->a, lk->desc);
+    g.lk = &lk->a;
   }
 
   // ---- integer tables of the packed batch ----
@@ -731,6 +897,7 @@ static int llm_prefill(Model* m, fo1_generate_desc* d, const fo1_prefix_desc* px
       FO1_CUDA(cudaMemcpyAsync(const_cast<int*>(bm->a.prompt_len), d->seq_lens, B * sizeof(int), cudaMemcpyHostToDevice, s));
       FO1_CUDA(cudaMemcpyAsync(const_cast<float*>(bm->a.lp_div), bm->lp_div.data(), bm->lp_div.size() * sizeof(float), cudaMemcpyHostToDevice, s));
     }
+    if (lk) FO1_TRY(lookup_upload(lk->a, lk->desc, s));
     if (mode == DEC_SAMPLED || mode == DEC_SCORED) {
       // a scored greedy call samples with top_k 1 (bit-identical to greedy) so that both paths score in the sampler's per-row pass
       std::vector<SampleRowParams> h(B);
@@ -825,6 +992,7 @@ static int decode_per_kernel(Model* m, fo1_generate_desc* d, const fo1_score_des
   const fo1_model_config& c = m->cfg;
   const int B = g.beam ? g.beam->S * g.beam->N : d->n_seqs, H = c.llm_hidden, hd = c.llm_head_dim, V = c.llm_vocab;
   LlmState* ls = static_cast<LlmState*>(m->llm_state);
+  const int R = g.lk ? B * (g.lk->K + 1) : B;     // rows of a step
   // programmatic dependent launch: each kernel of the step starts (prologue, weight prefetch) while its predecessor drains
   const bool use_pdl = getenv("FO1_NO_PDL") == nullptr;
   auto enqueue_step = [&]() -> int {
@@ -843,19 +1011,56 @@ static int decode_per_kernel(Model* m, fo1_generate_desc* d, const fo1_score_des
     FO1_TRY(linear(g.lastn, H, m->llm.lm_head, H, g.logits, V, FO1_F32, B, V, H, nullptr, 0, FO1_EPI_NONE, nullptr, 0, 0, s));
     return decode_column(mode, g, k, sc, B, V, 1, s);
   };
+  // prompt lookup: drafts, then ONE verify step over R = B * (K + 1) rows, each computing the plain step's bits for its position
+  // (block norms, GEMMs with the M = B choice, the K/V append and attention through the row map), then the acceptance
+  auto enqueue_verify = [&]() -> int {
+    const LookupArgs& a = *g.lk;
+    PdlScope pdl(use_pdl);
+    SplitKScope sk(true);
+    GemmChoiceScope gc(B);
+    FO1_TRY(lookup_drafts(a.corpus, a.ld, a.corpus_len, B, a.K, a.max_ngram, k.st.stop_ids, k.n_stop, a.col, k.max_new, a.drafts, a.n_draft, s));
+    FO1_TRY(lookup_rows(a, k.st, s));
+    launch_k(embed_tokens_kernel, dim3(R), dim3(256), 0, s, (const int*)a.row_tok, m->llm.embed, g.xa, H);
+    FO1_LAUNCH_CHECK();
+    FO1_TRY(mrope_table(a.row_pos, g.cs_dec, R, hd, c.mrope_section[0], c.mrope_section[1], c.mrope_section[2], c.rope_theta, s));
+    LayerBuf lb = g.layer;
+    lb.row_slot = a.row_slot; lb.row_idx = a.row_idx; lb.n_seqs = B;
+    const bf16* xin = g.xa;
+    for (int li = 0; li < c.llm_layers; ++li) {
+      bf16* xo = (li & 1) ? g.xa : g.xb;
+      FO1_TRY(llm_layer(m, li, xin, xo, lb, R, g.cs_dec, false, nullptr, B, 0, nullptr, nullptr, &k.st, s, false));
+      xin = xo;
+    }
+    FO1_TRY(rmsnorm(xin, H, m->llm.norm, g.lastn, H, R, H, c.rms_eps, seq_norm_kernel(H), s));
+    FO1_TRY(linear(g.lastn, H, m->llm.lm_head, H, g.logits, V, FO1_F32, R, V, H, nullptr, 0, FO1_EPI_NONE, nullptr, 0, 0, s));
+    if (mode == DEC_SCORED) {
+      FO1_TRY(score_rows_lookup(g.logits, V, R, a.K + 1, V, g.samp, a.row_col, a.row_out, a.row_lp, k.st.finished, k.max_new, B, sc->scores,
+                                sc->logits, s));
+    } else if (mode == DEC_SAMPLED) {
+      FO1_TRY(sample_rows(g.logits, V, R, V, a.row_prm, a.row_col, 1, a.row_out, s));   // each row's Philox step is its own column
+    } else {
+      launch_k(argmax_kernel, dim3(R), dim3(1024), 0, s, (const float*)g.logits, V, a.row_out);
+      FO1_LAUNCH_CHECK();
+    }
+    return lookup_accept(a, k, s);
+  };
+  auto enqueue = [&]() -> int { return g.lk ? enqueue_verify() : enqueue_step(); };
   cudaGraphExec_t gexec = nullptr;
   m->last_decode_path = 0;
   const bool want_graph = !g_prof_on && d->max_new_tokens > 3 && getenv("FO1_NO_GRAPH") == nullptr;
   d->steps_run = 0;
   int rc = FO1_OK;
+  cudaEvent_t poll_ev[2] = {nullptr, nullptr};
+  if (g.lk != nullptr && d->early_exit_interval > 0)
+    for (cudaEvent_t& e : poll_ev) FO1_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
   for (int step = 1; step < d->max_new_tokens; ++step) {
     if (gexec != nullptr) {
       if (cudaGraphLaunch(gexec, s) != cudaSuccess) { set_error("cudaGraphLaunch failed: %s", cudaGetErrorString(cudaGetLastError())); rc = FO1_ERR_CUDA; break; }
-      count_launch((uint64_t)c.llm_layers * 9 + 6);
+      count_launch((uint64_t)c.llm_layers * 9 + (g.lk ? 8 : 6));
     } else if (want_graph && step == 2) {
       cudaGraph_t graph = nullptr;
       if (cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
-        const int erc = enqueue_step();
+        const int erc = enqueue();
         const cudaError_t ce = cudaStreamEndCapture(s, &graph);
         if (erc == FO1_OK && ce == cudaSuccess && graph != nullptr && cudaGraphInstantiate(&gexec, graph, 0) == cudaSuccess) {
           cudaGraphDestroy(graph);
@@ -864,19 +1069,32 @@ static int decode_per_kernel(Model* m, fo1_generate_desc* d, const fo1_score_des
           if (graph) cudaGraphDestroy(graph);
           cudaGetLastError();
           gexec = nullptr;
-          if ((rc = enqueue_step()) != FO1_OK) break;
+          if ((rc = enqueue()) != FO1_OK) break;
         }
       } else {
         cudaGetLastError();
-        if ((rc = enqueue_step()) != FO1_OK) break;
+        if ((rc = enqueue()) != FO1_OK) break;
       }
     } else {
-      if ((rc = enqueue_step()) != FO1_OK) break;
+      if ((rc = enqueue()) != FO1_OK) break;
     }
     d->steps_run = step;
     // streamed: `done` is in host memory, so the host loop stops enqueueing without a sync once the device has published it
     if (h_progress != nullptr && (__atomic_load_n(h_progress, __ATOMIC_ACQUIRE) & FO1_STREAM_DONE)) break;
-    if (d->early_exit_interval > 0 && step % d->early_exit_interval == 0) {
+    // prompt lookup: sequences end after a varying number of steps, so the loop polls after every step, one step behind: it waits for
+    // the previous step's n_active while this step runs, so the device never waits for the host and at most one step runs past the
+    // end of the last sequence
+    if (g.lk != nullptr && d->early_exit_interval > 0) {
+      const int slot = step & 1;
+      if (cudaMemcpyAsync(ls->h_flag + slot, k.st.n_active, sizeof(int), cudaMemcpyDeviceToHost, s) != cudaSuccess ||
+          cudaEventRecord(poll_ev[slot], s) != cudaSuccess) {
+        set_error("early-exit poll failed"); rc = FO1_ERR_CUDA; break;
+      }
+      if (step > 1) {
+        if (cudaEventSynchronize(poll_ev[slot ^ 1]) != cudaSuccess) { set_error("early-exit poll failed"); rc = FO1_ERR_CUDA; break; }
+        if (ls->h_flag[slot ^ 1] <= 0) break;
+      }
+    } else if (d->early_exit_interval > 0 && step % d->early_exit_interval == 0) {
       if (cudaMemcpyAsync(ls->h_flag, k.st.n_active, sizeof(int), cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess) {
         set_error("early-exit poll failed"); rc = FO1_ERR_CUDA; break;
       }
@@ -887,6 +1105,8 @@ static int decode_per_kernel(Model* m, fo1_generate_desc* d, const fo1_score_des
     cudaStreamSynchronize(s);   // the exec must outlive its in-flight launches
     cudaGraphExecDestroy(gexec);
   }
+  for (cudaEvent_t e : poll_ev)
+    if (e != nullptr) cudaEventDestroy(e);
   return rc;
 }
 
@@ -932,7 +1152,8 @@ static int prefix_check(const fo1_generate_desc* d, const fo1_prefix_desc* px) {
 }
 
 int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, const fo1_score_desc* sc, const fo1_stream_desc* stm,
-                 cudaStream_t s, const fo1_prefix_desc* px = nullptr, const fo1_beam_desc* bmd = nullptr) {
+                 cudaStream_t s, const fo1_prefix_desc* px = nullptr, const fo1_beam_desc* bmd = nullptr,
+                 const fo1_lookup_desc* lkd = nullptr) {
   if (sc != nullptr && sc->logprobs == nullptr && sc->scores == nullptr && sc->logits == nullptr) sc = nullptr;   // nothing to score
   // the per-sequence host arrays first: they are the caller's, and need neither the model nor the device
   if (sp) FO1_TRY(sampling_check(sp, d->n_seqs, sc ? "fo1_llm_generate_scored" : "fo1_llm_generate_sampled"));
@@ -958,8 +1179,10 @@ int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, co
   k.n_stop = d->n_stop_ids; k.pad_id = d->pad_id; k.max_new = d->max_new_tokens;
   k.out_tokens = d->out_tokens; k.out_lens = d->out_lens;
   const DecodeMode mode = bmd ? DEC_BEAM : sc ? DEC_SCORED : sp ? DEC_SAMPLED : DEC_GREEDY;
-  // a shared-prefix call rounds the slot up to 64 rows: the cache-reading attention's last key tile stays inside the slot
-  const int cap = max_len + std::max(d->max_new_tokens, 1);
+  // a shared-prefix call rounds the slot up to 64 rows: the cache-reading attention's last key tile stays inside the slot; a lookup
+  // call's verify rows write up to K rows past the sequence's last position
+  const int n_drafts = lkd ? std::min(lkd->num_tokens, kLookupMaxDrafts) : 0;
+  const int cap = max_len + std::max(d->max_new_tokens, 1) + n_drafts;
   FO1_TRY(ensure_kv(m, rows, px ? (cap + 63) / 64 * 64 : cap));
   FO1_TRY(int_cache_trim(m));
   BeamRun brun;
@@ -979,9 +1202,22 @@ int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, co
     for (int i = 0; i <= a.max_new; ++i) brun.lp_div.push_back((float)std::pow((double)i, bmd->length_penalty));
     bm = &brun;
   }
+  LookupRun lrun;
+  LookupRun* lk = nullptr;
+  if (lkd) {
+    LookupArgs& a = lrun.a;
+    memset(&a, 0, sizeof(a));
+    a.B = d->n_seqs; a.K = n_drafts; a.max_ngram = lkd->max_ngram; a.max_new = d->max_new_tokens;
+    int longest = 0;
+    for (int b = 0; b < d->n_seqs; ++b) longest = std::max(longest, lkd->corpus_offsets[b + 1] - lkd->corpus_offsets[b]);
+    a.ld = (long long)longest + std::max(d->max_new_tokens, 1);
+    a.logprobs = sc ? sc->logprobs : nullptr;
+    lrun.desc = lkd;
+    lk = &lrun;
+  }
   m->arena.reset(true);
   DecodeBufs g;
-  FO1_TRY(llm_prefill(m, d, px, sp, sc, mode, k, s, true, g, bm));
+  FO1_TRY(llm_prefill(m, d, px, sp, sc, mode, k, s, true, g, bm, lk));
   FO1_TRY(arena_ensure(m, m->arena.peak));
   m->arena.reset(false);
   if (d->max_new_tokens > 0 && !bm) {  // out_tokens pre-filled with pad so an early exit leaves a clean tail
@@ -991,8 +1227,9 @@ int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, co
     FO1_CUDA(cudaMemsetAsync(d->out_lens, 0, d->n_seqs * sizeof(int), s));
     if (sc && sc->logprobs) FO1_CUDA(cudaMemsetAsync(sc->logprobs, 0, (size_t)n * sizeof(float), s));      // 0 past out_lens
   }
-  FO1_TRY(llm_prefill(m, d, px, sp, sc, mode, k, s, false, g, bm));
+  FO1_TRY(llm_prefill(m, d, px, sp, sc, mode, k, s, false, g, bm, lk));
   if (d->max_new_tokens <= 0) return FO1_OK;
+  if (lk) FO1_TRY(lookup_init(lk->a, k.st, g.samp, s));
   if (g.mega_grid > 0 && d->max_new_tokens > 1) return decode_persistent(m, d, sc, mode, k, g, s);
   FO1_TRY(decode_per_kernel(m, d, sc, mode, k, g, stm ? stm->progress : nullptr, s));
   return bm ? beam_finalize(bm->a, s) : FO1_OK;
@@ -1144,6 +1381,15 @@ extern "C" int fo1_llm_generate_beam(fo1_model* m, fo1_generate_desc* d, const f
   FO1_CHECK_ARG(m && d && bm, "fo1_llm_generate_beam: null argument");
   FO1_TRY(beam_check(d, bm, m->cfg.llm_vocab));
   return llm_generate(m, d, nullptr, nullptr, nullptr, static_cast<cudaStream_t>(stream), nullptr, bm);
+}
+
+extern "C" int fo1_llm_generate_lookup(fo1_model* m, fo1_generate_desc* d, const fo1_lookup_desc* lk, const fo1_prefix_desc* px,
+                                       const fo1_sampling_desc* sp, const fo1_score_desc* sc, void* stream) {
+  if (px != nullptr && px->n_groups == 0) px = nullptr;
+  FO1_CHECK_ARG(m && d && lk, "fo1_llm_generate_lookup: null argument");
+  FO1_TRY(lookup_check(d, lk));
+  if (px) FO1_TRY(prefix_check(d, px));
+  return llm_generate(m, d, sp, sc, nullptr, static_cast<cudaStream_t>(stream), px, nullptr, lk);
 }
 
 extern "C" int32_t fo1_stream_progress(const int32_t* progress) { return __atomic_load_n(progress, __ATOMIC_ACQUIRE); }

@@ -51,11 +51,10 @@ __global__ void __launch_bounds__(256) rope_apply_kernel(bf16* __restrict__ x, l
 
 // decode step: the same rotation over the q and k heads of row b, with the rotated K head and the V row appended to
 // the cache at index cache_len[b] in the same pass (one launch instead of rope + append)
-__global__ void __launch_bounds__(256) rope_kv_append_kernel(bf16* __restrict__ x, long long ld, const float* __restrict__ cs, int T,
-                                                             int q_heads, int kv_heads, int hd, const int* __restrict__ cache_len,
-                                                             bf16* __restrict__ kc, bf16* __restrict__ vc, int cap) {
-  griddep_launch();
-  griddep_wait();
+// row t's K/V goes to index idx[t] of cache slot slot[t] (slot == nullptr: slot t)
+__device__ __forceinline__ void rope_kv_append_rows(bf16* __restrict__ x, long long ld, const float* __restrict__ cs, int T, int q_heads,
+                                                    int kv_heads, int hd, const int* __restrict__ slot, const int* __restrict__ idx,
+                                                    bf16* __restrict__ kc, bf16* __restrict__ vc, int cap) {
   const int half = hd / 2, chunks = half / 8, n_heads = q_heads + kv_heads, kv_dim = kv_heads * hd;
   const long long n_rot = (long long)T * n_heads * chunks, n_v = (long long)T * (kv_dim / 8);
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n_rot + n_v; i += (long long)gridDim.x * blockDim.x) {
@@ -63,7 +62,7 @@ __global__ void __launch_bounds__(256) rope_kv_append_kernel(bf16* __restrict__ 
       const long long j = i - n_rot;
       const int t = (int)(j / (kv_dim / 8)), c = (int)(j % (kv_dim / 8));
       const bf16* src = x + (long long)t * ld + (long long)n_heads * hd + c * 8;
-      *reinterpret_cast<uint4*>(vc + ((long long)t * cap + cache_len[t]) * kv_dim + c * 8) = *reinterpret_cast<const uint4*>(src);
+      *reinterpret_cast<uint4*>(vc + ((long long)(slot ? slot[t] : t) * cap + idx[t]) * kv_dim + c * 8) = *reinterpret_cast<const uint4*>(src);
       continue;
     }
     const int c = (int)(i % chunks);
@@ -89,20 +88,40 @@ __global__ void __launch_bounds__(256) rope_kv_append_kernel(bf16* __restrict__ 
       *reinterpret_cast<uint4*>(p) = va;
       *reinterpret_cast<uint4*>(p + half) = vb;
     } else {   // K heads are only consumed from the cache
-      bf16* kp = kc + ((long long)t * cap + cache_len[t]) * kv_dim + (long long)(h - q_heads) * hd + c * 8;
+      bf16* kp = kc + ((long long)(slot ? slot[t] : t) * cap + idx[t]) * kv_dim + (long long)(h - q_heads) * hd + c * 8;
       *reinterpret_cast<uint4*>(kp) = va;
       *reinterpret_cast<uint4*>(kp + half) = vb;
     }
   }
 }
+__global__ void __launch_bounds__(256) rope_kv_append_kernel(bf16* __restrict__ x, long long ld, const float* __restrict__ cs, int T,
+                                                             int q_heads, int kv_heads, int hd, const int* __restrict__ cache_len,
+                                                             bf16* __restrict__ kc, bf16* __restrict__ vc, int cap) {
+  griddep_launch();
+  griddep_wait();
+  rope_kv_append_rows(x, ld, cs, T, q_heads, kv_heads, hd, nullptr, cache_len, kc, vc, cap);
+}
+// the prompt-lookup verify step: row t into (slot row_slot[t], index row_idx[t])
+__global__ void __launch_bounds__(256) rope_kv_append_map_kernel(bf16* __restrict__ x, long long ld, const float* __restrict__ cs, int T,
+                                                                 int q_heads, int kv_heads, int hd, const int* __restrict__ row_slot,
+                                                                 const int* __restrict__ row_idx, bf16* __restrict__ kc, bf16* __restrict__ vc,
+                                                                 int cap) {
+  griddep_launch();
+  griddep_wait();
+  rope_kv_append_rows(x, ld, cs, T, q_heads, kv_heads, hd, row_slot, row_idx, kc, vc, cap);
+}
 
 int rope_kv_append(bf16* qkv, long long ld, const float* cos_sin, int T, int q_heads, int kv_heads, int head_dim, const int* cache_len,
-                   bf16* kc, bf16* vc, int cap, cudaStream_t s) {
+                   bf16* kc, bf16* vc, int cap, cudaStream_t s, const int* row_slot) {
   FO1_CHECK_ARG(head_dim % 16 == 0 && ld % 8 == 0, "rope_kv_append: head_dim %d must be a multiple of 16 and the pitch of 8", head_dim);
   if (T == 0) return FO1_OK;
   const long long n = (long long)T * (q_heads + kv_heads) * (head_dim / 16) + (long long)T * kv_heads * head_dim / 8;
   const int blocks = (int)((n + 255) / 256 < device_sm_count() * 16 ? (n + 255) / 256 : device_sm_count() * 16);
-  launch_k(rope_kv_append_kernel, dim3(blocks), dim3(256), 0, s, qkv, ld, cos_sin, T, q_heads, kv_heads, head_dim, cache_len, kc, vc, cap);
+  if (row_slot != nullptr)
+    launch_k(rope_kv_append_map_kernel, dim3(blocks), dim3(256), 0, s, qkv, ld, cos_sin, T, q_heads, kv_heads, head_dim, row_slot, cache_len,
+             kc, vc, cap);
+  else
+    launch_k(rope_kv_append_kernel, dim3(blocks), dim3(256), 0, s, qkv, ld, cos_sin, T, q_heads, kv_heads, head_dim, cache_len, kc, vc, cap);
   FO1_LAUNCH_CHECK();
   return FO1_OK;
 }

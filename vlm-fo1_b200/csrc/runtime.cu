@@ -24,6 +24,7 @@ void set_error(const char* fmt, ...) {
 bool g_prof_on = false;
 thread_local bool t_pdl = false;
 thread_local bool t_splitk_ok = false;
+thread_local int t_gemm_choice_m = 0;
 struct ProfRec { cudaEvent_t a, b; std::string tag; double flops, bytes; };
 static std::vector<ProfRec> g_recs;
 static std::mutex g_prof_mu;

@@ -3,7 +3,7 @@
 #include <cmath>
 #include <vector>
 
-#include "sampling.cuh"
+#include "lookup.cuh"
 
 namespace fo1 {
 
@@ -49,6 +49,37 @@ __global__ void __launch_bounds__(kSampleThreads) score_rows_kernel(const float*
   const float lp = score_row<kSampleThreads>(row, V, p.temperature, t, sm, scores ? scores + o : nullptr,
                                              logits_out ? logits_out + o : nullptr);
   if (threadIdx.x == 0 && logprobs != nullptr) logprobs[(long long)r * lp_stride + col] = lp;
+}
+
+// scored prompt-lookup verify rows (one CTA per row): score_rows_kernel<true>'s draw and scoring with row r's own column
+// row_col[r] and sequence b = r / K1's parameters; the scores / logits rows go to (column, b), the log-probability to row_lp[r]
+__global__ void __launch_bounds__(kSampleThreads) score_rows_lookup_kernel(const float* __restrict__ logits, long long ld, int V, int K1,
+                                                                           const SampleRowParams* __restrict__ prm, const int* __restrict__ row_col,
+                                                                           int* __restrict__ tok, float* __restrict__ row_lp,
+                                                                           const int* __restrict__ finished, int max_new, int n_seqs,
+                                                                           float* __restrict__ scores, float* __restrict__ logits_out) {
+  griddep_launch();
+  griddep_wait();
+  __shared__ SampleSmem<kSampleThreads> sm;
+  const int r = blockIdx.x, b = r / K1;
+  const SampleRowParams p = prm[b];
+  const float* row = logits + (long long)r * ld;
+  const int col = __ldcg(row_col + r);
+  const int t = sample_row<kSampleThreads, SMP_DRAW_KEPT>(row, V, p, col, sm);
+  if (threadIdx.x == 0) tok[r] = t;
+  if (col >= max_new || __ldcg(finished + b)) return;     // past the sequence's end: nothing is recorded
+  const long long o = ((long long)col * n_seqs + b) * V;
+  const float lp = score_row<kSampleThreads>(row, V, p.temperature, t, sm, scores ? scores + o : nullptr, logits_out ? logits_out + o : nullptr);
+  if (threadIdx.x == 0) row_lp[r] = lp;
+}
+
+int score_rows_lookup(const float* logits, long long ld, int n_rows, int K1, int V, const SampleRowParams* prm, const int* row_col,
+                      int* tok, float* row_lp, const int* finished, int max_new, int n_seqs, float* scores, float* logits_out, cudaStream_t s) {
+  FO1_CHECK_ARG(n_rows <= 65535, "score_rows_lookup: %d rows exceed the grid limit", n_rows);
+  launch_k(score_rows_lookup_kernel, dim3(n_rows), dim3(kSampleThreads), 0, s, logits, ld, V, K1, prm, row_col, tok, row_lp, finished, max_new,
+           n_seqs, scores, logits_out);
+  FO1_LAUNCH_CHECK();
+  return FO1_OK;
 }
 
 int sampling_check(const fo1_sampling_desc* sp, int n, const char* fn) {

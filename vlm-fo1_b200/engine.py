@@ -287,13 +287,57 @@ class Beams:
         raise ValueError(f"early_stopping must be True, False or 'never', not {self.early_stopping!r}")
 
 
+@dataclass
+class Lookup:
+    """Prompt-lookup decoding of a generate call (fo1_lookup_desc): ``num_tokens`` drafts per step (HF's prompt_lookup_num_tokens; the
+    device proposes at most 16), ``max_ngram`` (HF's max_matching_ngram_size) and ``corpus``, one id list per sequence (HF's prompt
+    ``input_ids``; None: empty corpora, only the emitted tokens are searched)."""
+    num_tokens: int
+    max_ngram: int = 2
+    corpus: Optional[Sequence[Sequence[int]]] = None
+
+
+def _lookup_desc(lookup: Lookup, B: int, dev):
+    """(LookupDesc, keep-alive, steps, accepted) of a call with B sequences."""
+    corpus = lookup.corpus if lookup.corpus is not None else [[] for _ in range(B)]
+    if len(corpus) != B:
+        raise ValueError(f"lookup corpus: {len(corpus)} id lists for {B} sequences")
+    flat = [int(t) for c in corpus for t in c]
+    offs = [0]
+    for c in corpus:
+        offs.append(offs[-1] + len(c))
+    ids = (C.c_int32 * max(len(flat), 1))(*flat)
+    off = (C.c_int32 * (B + 1))(*offs)
+    steps = torch.zeros((B,), dtype=torch.int32, device=dev)
+    acc = torch.zeros((B,), dtype=torch.int32, device=dev)
+    desc = _lib.LookupDesc(int(lookup.num_tokens), int(lookup.max_ngram), ids, off, steps.data_ptr(), acc.data_ptr())
+    return desc, (ids, off), steps, acc
+
+
+def lookup_drafts(corpus: torch.Tensor, lens: torch.Tensor, num_tokens: int, max_ngram: int, stop_ids: Sequence[int],
+                  emitted: Optional[torch.Tensor] = None, max_new_tokens: int = 0):
+    """fo1_lookup_drafts: the draft rule alone.  ``corpus`` int32 [B, ld] on the device, ``lens`` int32 [B] -> (drafts int32
+    [B, num_tokens], n_draft int32 [B]).  ``emitted`` (int32 [B]) with ``max_new_tokens`` caps the drafts at max_new - emitted - 1."""
+    B = corpus.shape[0]
+    dev = corpus.device
+    corpus, lens = corpus.to(torch.int32).contiguous(), lens.to(dev, torch.int32).contiguous()
+    st = torch.tensor([int(x) for x in stop_ids] or [0], dtype=torch.int32, device=dev)
+    drafts = torch.zeros((B, num_tokens), dtype=torch.int32, device=dev)
+    nd = torch.zeros((B,), dtype=torch.int32, device=dev)
+    em = emitted.to(dev, torch.int32).contiguous() if emitted is not None else None
+    check(lib().fo1_lookup_drafts(corpus.data_ptr(), corpus.stride(0), lens.data_ptr(), B, int(num_tokens), int(max_ngram), st.data_ptr(),
+                                  len(stop_ids), em.data_ptr() if em is not None else None, int(max_new_tokens), drafts.data_ptr(),
+                                  nd.data_ptr(), _stream()), "fo1_lookup_drafts")
+    return drafts, nd
+
+
 def _engine_generate(self, inputs_embeds: torch.Tensor, position_ids: torch.Tensor, seq_lens: Sequence[int],
                      rope_deltas: Sequence[int], max_new_tokens: int, stop_ids: Sequence[int], pad_id: int,
                      want_prefill_logits: bool = False, want_all_logits: bool = False, early_exit_interval: int = 8,
                      sampling: Optional[Sampling] = None, want_logprobs: bool = False, want_scores: bool = False,
                      want_logits: bool = False, raw_rows: Optional[Sequence[int]] = None,
                      on_tokens: Optional[Callable[[int, int, "np.ndarray", "np.ndarray"], Optional[bool]]] = None,
-                     prefix: Optional[Prefix] = None, beams: Optional[Beams] = None):
+                     prefix: Optional[Prefix] = None, beams: Optional[Beams] = None, lookup: Optional[Lookup] = None):
     """Prefill + decode of a packed batch: greedy, or sampled per sequence when ``sampling`` is given.  position_ids int32
     [3, sum L].  Returns a dict of device tensors.
 
@@ -317,7 +361,16 @@ def _engine_generate(self, inputs_embeds: torch.Tensor, position_ids: torch.Tens
     ``sequence_scores`` fp32 [B * num_return], ``beam_indices`` int32 [B * num_return, max_new] (prompt * N + beam, -1 past the
     length) and ``beam_steps`` int32 [B] (the steps each prompt ran).  ``want_scores`` / ``want_logits`` give [max_new, B * N, V]
     log-prob / raw rows; ``want_logprobs`` [B * num_return, max_new] the returned tokens' log-probabilities.  Sampling, streaming,
-    prefixes, ``raw_rows`` and ``want_all_logits`` are refused."""
+    prefixes, ``raw_rows`` and ``want_all_logits`` are refused.
+
+    Prompt lookup (include/fo1.h, fo1_lookup_desc): with ``lookup``, each step drafts tokens from the sequence's corpus and verifies
+    them in one step of B * (K + 1) rows on the per-kernel decode path.  Tokens, lengths, logprobs and the score rows up to each
+    length are bit-identical to the same call on the per-kernel path without lookup (FO1_NO_MEGA=1); against the persistent
+    kernel (B <= 32 by default) they agree as any two decode paths do (DESIGN.md §2).  ``steps_run`` counts verify steps; added
+    are ``lookup_steps`` / ``lookup_accepted`` int32 [B] (verify steps each sequence took part in, drafts it accepted).
+    Streaming and beams are refused."""
+    if lookup is not None and (beams is not None or on_tokens is not None):
+        raise ValueError("prompt lookup does not take `beams` or `on_tokens`")
     if beams is not None:
         return self._generate_beam(inputs_embeds, position_ids, seq_lens, rope_deltas, max_new_tokens, stop_ids, pad_id, beams,
                                    want_prefill_logits, early_exit_interval, want_logprobs, want_scores, want_logits, sampling, raw_rows,
@@ -380,9 +433,16 @@ def _engine_generate(self, inputs_embeds: torch.Tensor, position_ids: torch.Tens
                              (C.c_int32 * B)(*[int(g) for g in prefix.seq_group]))
         px_arg = C.byref(px)
 
+    lk_out = None
+    if lookup is not None:
+        lk, _lk_keep, lk_steps, lk_acc = _lookup_desc(lookup, B, self.device)
+        lk_out = (lk_steps, lk_acc)
+
     def launch(stream, st=None):
         sa = C.byref(st) if st is not None else None
-        if px_arg is None:
+        if lookup is not None:
+            check(L.fo1_llm_generate_lookup(self._h, C.byref(d), C.byref(lk), px_arg, sp_arg, sc_arg, stream), "fo1_llm_generate_lookup")
+        elif px_arg is None:
             check(L.fo1_llm_generate_streamed(self._h, C.byref(d), sp_arg, sc_arg, sa, stream), "fo1_llm_generate_streamed")
         else:
             check(L.fo1_llm_generate_prefixed(self._h, C.byref(d), px_arg, sp_arg, sc_arg, sa, stream), "fo1_llm_generate_prefixed")
@@ -391,6 +451,8 @@ def _engine_generate(self, inputs_embeds: torch.Tensor, position_ids: torch.Tens
     else:
         self._run_streamed(launch, B, max_new_tokens, on_tokens)
     out = dict(tokens=toks, lens=lens, prefill_logits=pl, all_logits=al, steps_run=d.steps_run)
+    if lk_out is not None:
+        out["lookup_steps"], out["lookup_accepted"] = lk_out
     if want_logprobs:
         out["logprobs"] = lp
     if want_scores:
@@ -584,6 +646,7 @@ Engine._generate_beam = _engine_generate_beam
 Engine._stream_buffers = _engine_stream_buffers
 Engine._run_streamed = _engine_run_streamed
 Engine.sample_tokens = staticmethod(sample_tokens)
+Engine.lookup_drafts = staticmethod(lookup_drafts)
 Engine.prefix_attention = staticmethod(prefix_attention)
 Engine.score_rows = staticmethod(score_rows)
 

@@ -251,15 +251,19 @@ class Fo1Pipeline:
     # ---- language side -----------------------------------------------------------------------------------
     def generate(self, samples: Sequence[SampleInputs], max_new_tokens: int, stop_ids: Sequence[int], pad_id: int = 151643,
                  early_exit_interval: int = 8, want_prefill_logits: bool = False, sampling=None, want_logprobs: bool = False,
-                 want_scores: bool = False, want_logits: bool = False, raw_rows=None, on_tokens=None, beams=None):
+                 want_scores: bool = False, want_logits: bool = False, raw_rows=None, on_tokens=None, beams=None, lookup=None):
         """``sampling``: None (greedy) or an engine.Sampling with one parameter set per sample.  ``want_logprobs`` / ``want_scores`` /
         ``want_logits`` / ``raw_rows``: per-token scores, as Engine.generate.  ``on_tokens``: the streaming callback of
         Engine.generate (columns of the whole batch, in sample order).  ``beams``: an engine.Beams, beam search for every sample
-        (Engine.generate's outputs); the towers still run once per unique image, but each prompt is prefilled in full."""
+        (Engine.generate's outputs); the towers still run once per unique image, but each prompt is prefilled in full.  ``lookup``: an
+        engine.Lookup, prompt-lookup decoding; without a corpus of its own, each sample's ``input_ids`` is its corpus (HF's)."""
+        if lookup is not None and lookup.corpus is None:
+            from dataclasses import replace
+            lookup = replace(lookup, corpus=[list(s.input_ids) for s in samples])
         eng, dev = self.eng, self.eng.device
         kw = dict(max_new_tokens=max_new_tokens, stop_ids=stop_ids, pad_id=pad_id, early_exit_interval=early_exit_interval,
                   want_prefill_logits=want_prefill_logits, sampling=sampling, want_logprobs=want_logprobs, want_scores=want_scores,
-                  want_logits=want_logits, raw_rows=raw_rows, on_tokens=on_tokens, beams=beams)
+                  want_logits=want_logits, raw_rows=raw_rows, on_tokens=on_tokens, beams=beams, lookup=lookup)
         if self._share_inputs and len(samples) > 1:
             rep = encoder_groups(samples)
             if any(r != b for b, r in enumerate(rep)):
@@ -282,13 +286,13 @@ class Fo1Pipeline:
         self._mark("splice")
         out = eng.generate(embeds, pos, lens, deltas, max_new_tokens, stop_ids, pad_id, want_prefill_logits=want_prefill_logits,
                            early_exit_interval=early_exit_interval, sampling=sampling, want_logprobs=want_logprobs, want_scores=want_scores,
-                           want_logits=want_logits, raw_rows=raw_rows, on_tokens=on_tokens, beams=beams)
+                           want_logits=want_logits, raw_rows=raw_rows, on_tokens=on_tokens, beams=beams, lookup=lookup)
         self._mark("llm_prefill_decode")
         out["prompt_lens"] = lens
         return out
 
     def _generate_shared(self, samples, rep, max_new_tokens, stop_ids, pad_id, early_exit_interval, want_prefill_logits, sampling,
-                         want_logprobs, want_scores, want_logits, raw_rows, on_tokens, beams):
+                         want_logprobs, want_scores, want_logits, raw_rows, on_tokens, beams, lookup):
         """generate() of a batch in which some samples have equal encoder inputs: the towers run once per unique image, and each set's
         common prompt prefix is prefilled once (Engine.generate's ``prefix``).  Bit-identical to the unshared path."""
         eng, dev = self.eng, self.eng.device
@@ -331,7 +335,7 @@ class Fo1Pipeline:
         self._mark("splice")
         out = eng.generate(embeds, pos, lens, plan["rope_delta"], max_new_tokens, stop_ids, pad_id, want_prefill_logits=want_prefill_logits,
                            early_exit_interval=early_exit_interval, sampling=sampling, want_logprobs=want_logprobs, want_scores=want_scores,
-                           want_logits=want_logits, raw_rows=raw_rows, on_tokens=on_tokens, prefix=prefix, beams=beams)
+                           want_logits=want_logits, raw_rows=raw_rows, on_tokens=on_tokens, prefix=prefix, beams=beams, lookup=lookup)
         self._mark("llm_prefill_decode")
         out["prompt_lens"] = lens
         return out

@@ -196,6 +196,25 @@ class Fo1ForCausalLM:
                                              scores=block("scores") if want[0] else None, logits=block("logits") if want[1] else None,
                                              beam_indices=bi, past_key_values=None)
 
+    def _lookup(self, kwargs):
+        """None or the engine.Lookup of a prompt-lookup call: ``prompt_lookup_num_tokens`` and ``max_matching_ngram_size`` from the
+        call's kwargs, else generation_config.json, as HF reads them; a non-positive value raises HF's ValueError.  The corpus is the
+        prompt's ids (the pipeline fills it in).  As in HF, ``num_return_sequences > 1`` with lookup raises ValueError, and with
+        ``num_beams > 1`` the kwargs have no effect; a call with a ``streamer`` runs without lookup (same outputs).  Lookup runs on the per-kernel decode path: its tokens are bit-identical to the plain
+        per-kernel call (FO1_NO_MEGA=1), and agree with the default persistent-kernel call wherever any two decode paths agree
+        (DESIGN.md §2)."""
+        gc = self.generation_config
+        get = lambda name: kwargs[name] if kwargs.get(name) is not None else gc.get(name)
+        K = get("prompt_lookup_num_tokens")
+        if K is None:
+            return None
+        ng = get("max_matching_ngram_size")
+        ng = 2 if ng is None else ng
+        if int(K) <= 0 or int(ng) <= 0:
+            raise ValueError("Invalid max_matching_ngram_size or num_output_tokens")
+        E = import_module("vlm-fo1_b200.engine")
+        return E.Lookup(num_tokens=int(K), max_ngram=int(ng))
+
     def _num_return_sequences(self, kwargs):
         n = kwargs.get("num_return_sequences")
         n = self.generation_config.get("num_return_sequences", 1) if n is None else n
@@ -223,6 +242,7 @@ class Fo1ForCausalLM:
                  max_new_tokens=512, streamer=None, top_p=1.0, use_cache=True, stopping_criteria=None, pad_token_id=None, top_k=None, **kwargs):
         want = self._outputs(kwargs)
         beams = self._beams(do_sample, kwargs)
+        lookup = self._lookup(kwargs)       # (with beams HF only warns and runs beam search; a streamed call runs without lookup)
         n = self._num_return_sequences(kwargs)
         kwargs.pop("num_return_sequences", None)
         if beams is not None:
@@ -234,6 +254,8 @@ class Fo1ForCausalLM:
                                          early_exit_interval=8, want_scores=bool(want and want[0]), want_logits=bool(want and want[1]),
                                          beams=beams)
             return self._beam_result(out, 0, inputs, want, beams)
+        if n > 1 and lookup is not None:
+            raise ValueError(f"num_return_sequences has to be 1 when doing assisted generate, but is {n}.")
         if n > 1 and not do_sample:
             raise ValueError("Greedy methods without beam search do not support `num_return_sequences` different than 1 "
                              f"(got {n}).")
@@ -260,7 +282,7 @@ class Fo1ForCausalLM:
                     streamer.put(torch.tensor([int(toks[0, t - lo])], dtype=torch.long))
         out = self.pipeline.generate([sample], int(max_new_tokens), sorted(set(stop)), pad_id=int(pad), early_exit_interval=8,
                                      sampling=self._sampling([samp]), want_scores=bool(want and want[0]), want_logits=bool(want and want[1]),
-                                     on_tokens=on_tokens)
+                                     on_tokens=on_tokens, **({"lookup": lookup} if lookup is not None and streamer is None else {}))
         res = self._result(out, 0, inputs, want)
         if streamer is not None:
             streamer.end()
@@ -295,11 +317,16 @@ class Fo1ForCausalLM:
         pads = [kw.get("pad_token_id") for kw in batch]
         pad = pads[0] if pads[0] is not None else (stop[0] if stop else 0)
         sampling = self._sampling(samps)
+        lookups = [self._lookup(kw) for kw in batch]
+        if any(lk != lookups[0] for lk in lookups):
+            raise NotImplementedError("generate_batch runs prompt lookup as one call: every sample must use the same "
+                                      "prompt_lookup_num_tokens and max_matching_ngram_size (call generate for the others)")
         # a greedy sample in a sampled batch is scored on its raw logits, as HF's greedy search reports them
         raw = [int(s is None) for s in samps] if sampling is not None else None
         out = self.pipeline.generate(list(samples), T, stop, pad_id=int(pad), early_exit_interval=8, sampling=sampling,
                                      want_logprobs=bool(output_logprobs), want_scores=any(w is not None and w[0] for w in wants),
-                                     want_logits=any(w is not None and w[1] for w in wants), raw_rows=raw)
+                                     want_logits=any(w is not None and w[1] for w in wants), raw_rows=raw,
+                                     **({"lookup": lookups[0]} if lookups[0] is not None else {}))
         out["lens"] = out["lens"].cpu().tolist()
         res = []
         for b, kw in enumerate(batch):
