@@ -93,15 +93,29 @@ struct GemmChoiceScope {
   ~GemmChoiceScope() { t_gemm_choice_m = prev; }
 };
 #ifdef __CUDACC__
+// `cluster` > 1: thread-block clusters of that many CTAs along x (grid.x must be a multiple of it)
 template <typename... KArgs, typename... Args>
-inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args&&... args) {
+inline cudaError_t launch_k_cluster(int cluster, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args&&... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = s;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at; cfg.numAttrs = t_pdl ? 1 : 0;
+  cudaLaunchAttribute at[2];
+  unsigned n = 0;
+  if (t_pdl) {
+    at[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[n].val.programmaticStreamSerializationAllowed = 1;
+    ++n;
+  }
+  if (cluster > 1) {
+    at[n].id = cudaLaunchAttributeClusterDimension;
+    at[n].val.clusterDim.x = cluster; at[n].val.clusterDim.y = 1; at[n].val.clusterDim.z = 1;
+    ++n;
+  }
+  cfg.attrs = at; cfg.numAttrs = n;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+}
+template <typename... KArgs, typename... Args>
+inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args&&... args) {
+  return launch_k_cluster(1, kernel, grid, block, smem, s, static_cast<Args&&>(args)...);
 }
 #endif
 

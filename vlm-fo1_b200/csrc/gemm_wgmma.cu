@@ -362,9 +362,58 @@ __device__ __forceinline__ void load_a_tile(const GemmArgs& g, const CUtensorMap
   }
 }
 
-template <int BN>
+// Paired launches (CL = 2) deal out pair-tiles -- m-tiles 2 mp and 2 mp + 1 of one n-tile -- in groups of kGroupPairs m-pairs, m-pairs
+// varying fastest inside a group, so the clusters running at the same time share a few W tiles through L2 instead of each streaming its
+// own.  A wave of 66 clusters over a group of G m-pairs touches G pair-rows of A and 66 / G n-tiles of W; G = 8 keeps that smallest for
+// the gate/up GEMM (86 n-tiles of 2048-deep W, 90 MB, more than L2 holds).  Measured on H100 (G = 4 / 8 / 16): gate/up 7.99 / 7.97 /
+// 8.09 ms, down 2.72 / 2.72 / 2.83 ms, ViT gated fc1 6.70 / 6.81 / 6.65 ms.
+constexpr int kGroupPairs = 8;
+// automatic choice: weights of at least this many bytes take the paired launch (see launch_gemm).  An empirical cutoff, tuned on this
+// engine's shapes: it falls between the LLM qkv weight (10.5 MB, 18 % slower paired) and the ViT gated fc1 weight (17.5 MB, faster).
+constexpr long long kPairMinWeightBytes = 16LL << 20;
+
+struct WorkTile { int tile, split, m0, n0; };
+__device__ __forceinline__ int num_work_units(const GemmArgs& g, int cl) {
+  return cl == 1 ? g.tiles_m * g.tiles_n * g.ksplit : ((g.tiles_m + 1) >> 1) * g.tiles_n;
+}
+// work unit -> output tile of CTA `rank` of its cluster; the producer and the consumers of both CTAs of a pair walk the same sequence
+template <int BN, int CL>
+__device__ __forceinline__ WorkTile work_tile(const GemmArgs& g, int work, int rank) {
+  if constexpr (CL == 1) {
+    const int tile = work / g.ksplit;
+    return {tile, work - tile * g.ksplit, (tile / g.tiles_n) * BM, (tile % g.tiles_n) * BN};
+  } else {
+    const int pairs_m = (g.tiles_m + 1) >> 1;
+    const int per_group = kGroupPairs * g.tiles_n;
+    const int group = work / per_group, first = group * kGroupPairs;
+    const int rows = min(kGroupPairs, pairs_m - first);
+    const int local = work - group * per_group;
+    const int mt = 2 * (first + local % rows) + rank, nt = local / rows;
+    return {mt * g.tiles_n + nt, 0, mt * BM, nt * BN};
+  }
+}
+
+// the W tile of k-block kb into a ring stage.  Paired: CTA r loads W rows [r BN / 2, (r + 1) BN / 2) of the tile into both CTAs.
+template <int BN, int CL>
+__device__ __forceinline__ void load_w_tile(const CUtensorMap* tmW, uint32_t dst, uint32_t bar, int kb, int n0, uint32_t rank) {
+  if constexpr (CL == 1) {
+    ptx::tma_load_2d(dst, tmW, bar, kb * BK, n0);
+  } else {
+    ptx::tma_load_2d_multicast(dst + rank * (BN / 2) * BK * 2, tmW, bar, kb * BK, n0 + (int)rank * (BN / 2), (uint16_t)0x3);
+  }
+}
+// a consumer warp is done with a ring stage.  Paired: the slot is refilled only when the consumers of both CTAs have released it.
+template <int CL>
+__device__ __forceinline__ void release_stage(uint32_t empty_bar, uint32_t rank) {
+  ptx::mbar_arrive(empty_bar);
+  if constexpr (CL == 2) ptx::mbar_arrive_cluster(empty_bar, rank ^ 1u);
+}
+
+// CL = 1: one CTA per work item.  CL = 2: clusters of two CTAs along M sharing (multicasting) the W tile; split-K is never paired.
+template <int BN, int CL>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW, const __grid_constant__ GemmArgs g) {
+  static_assert(CL == 1 || CL == 2, "CTA pairs only");
   const int S = g.stages;
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment: required by the 128B swizzle atoms the wgmma descriptors assume
@@ -380,19 +429,22 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int num_tiles = g.tiles_m * g.tiles_n * g.ksplit;   // work items
+  const int num_units = num_work_units(g, CL);
   const int num_kb_total = (g.K + BK - 1) / BK;
+  const uint32_t rank = CL == 1 ? 0u : ptx::cluster_ctarank();
 
   if (threadIdx.x == 0) {
     ptx::prefetch_tmap(&tmA);
     ptx::prefetch_tmap(&tmW);
     for (int s = 0; s < S; ++s) {
       ptx::mbar_init(ptx::smem_u32(full_bar + s), 1);
-      ptx::mbar_init(ptx::smem_u32(empty_bar + s), kEpiThreads / 32);   // one arrive per consumer warp
+      ptx::mbar_init(ptx::smem_u32(empty_bar + s), CL * kEpiThreads / 32);   // one arrive per consumer warp of the cluster
     }
     ptx::mbar_fence_init();
   }
-  __syncthreads();
+  // paired: the peer's barriers must be initialised before the first multicast lands in its shared memory
+  if constexpr (CL == 2) ptx::cluster_sync();
+  else __syncthreads();
   griddep_launch();   // programmatic dependent launch: the next kernel of the stream may begin its own prologue now
 
   if (warp == kEpiThreads / 32) {
@@ -400,11 +452,9 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
     if (ptx::elect_one()) {
       uint32_t it = 0;
       bool first = true;
-      for (int work = blockIdx.x; work < num_tiles; work += gridDim.x) {
-        const int tile = work / g.ksplit, split = work - tile * g.ksplit;
-        const int m0 = (tile / g.tiles_n) * BM;
-        const int n0 = (tile % g.tiles_n) * BN;
-        const int kb0 = split * g.kb_per_split, kb1 = min(num_kb_total, kb0 + g.kb_per_split);
+      for (int work = blockIdx.x / CL; work < num_units; work += gridDim.x / CL) {
+        const WorkTile wt = work_tile<BN, CL>(g, work, (int)rank);
+        const int kb0 = wt.split * g.kb_per_split, kb1 = min(num_kb_total, kb0 + g.kb_per_split);
         int kb = kb0;
         if (first) {
           // W never depends on the previous kernel of the stream: fill the ring with weight tiles BEFORE waiting for
@@ -414,11 +464,11 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
           for (int i = 0; i < pre; ++i) {
             const uint32_t fb = ptx::smem_u32(full_bar + i);
             ptx::mbar_expect_tx(fb, (uint32_t)g.stage_tx);
-            ptx::tma_load_2d(ptx::smem_u32(smem_b + i * g.b_stage_bytes), &tmW, fb, (kb0 + i) * BK, n0);
+            load_w_tile<BN, CL>(&tmW, ptx::smem_u32(smem_b + i * g.b_stage_bytes), fb, kb0 + i, wt.n0, rank);
           }
           griddep_wait();
           for (int i = 0; i < pre; ++i)
-            load_a_tile(g, &tmA, ptx::smem_u32(smem_a + i * g.a_stage_bytes), ptx::smem_u32(full_bar + i), kb0 + i, m0);
+            load_a_tile(g, &tmA, ptx::smem_u32(smem_a + i * g.a_stage_bytes), ptx::smem_u32(full_bar + i), kb0 + i, wt.m0);
           it = pre; kb = kb0 + pre;
         }
         for (; kb < kb1; ++kb, ++it) {
@@ -426,8 +476,8 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
           ptx::mbar_wait(ptx::smem_u32(empty_bar + s), ph ^ 1);
           const uint32_t fb = ptx::smem_u32(full_bar + s);
           ptx::mbar_expect_tx(fb, (uint32_t)g.stage_tx);
-          load_a_tile(g, &tmA, ptx::smem_u32(smem_a + s * g.a_stage_bytes), fb, kb, m0);
-          ptx::tma_load_2d(ptx::smem_u32(smem_b + s * g.b_stage_bytes), &tmW, fb, kb * BK, n0);
+          load_a_tile(g, &tmA, ptx::smem_u32(smem_a + s * g.a_stage_bytes), fb, kb, wt.m0);
+          load_w_tile<BN, CL>(&tmW, ptx::smem_u32(smem_b + s * g.b_stage_bytes), fb, kb, wt.n0, rank);
         }
       }
     }
@@ -438,13 +488,12 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
     uint8_t* stg = staging + warp * kFragStageBytes;
     uint32_t it = 0;
     griddep_wait();   // residual reads / output writes are ordered after the previous kernel
-    for (int work = blockIdx.x; work < num_tiles; work += gridDim.x) {
-      const int tile = work / g.ksplit, split = work - tile * g.ksplit;
-      const int m0 = (tile / g.tiles_n) * BM;
-      const int n0 = (tile % g.tiles_n) * BN;
+    for (int work = blockIdx.x / CL; work < num_units; work += gridDim.x / CL) {
+      const WorkTile wt = work_tile<BN, CL>(g, work, (int)rank);
+      const int tile = wt.tile, split = wt.split, m0 = wt.m0, n0 = wt.n0;
       const int kb0 = split * g.kb_per_split, kb1 = min(num_kb_total, kb0 + g.kb_per_split);
-      // a warpgroup whose 64 rows lie beyond M (decode: M = batch) still multiplies them (whatever the slot holds: a wgmma in a
-      // divergent path is serialised by the compiler) and skips the epilogue
+      // a warpgroup whose 64 rows lie beyond M (decode: M = batch; the second CTA of the last pair when tiles_m is odd) still multiplies
+      // them (whatever the slot holds: a wgmma in a divergent path is serialised by the compiler) and skips the epilogue
       const bool live = m0 + wg * 64 < g.M;
       float acc[BN / 2];
 #pragma unroll
@@ -465,13 +514,13 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
           ptx::wgmma_commit();
           ptx::wgmma_wait<1>();          // the previous k-block's group has retired: its slot is free
         }
-        if (prev_s >= 0 && lane == 0) ptx::mbar_arrive(ptx::smem_u32(empty_bar + prev_s));
+        if (prev_s >= 0 && lane == 0) release_stage<CL>(ptx::smem_u32(empty_bar + prev_s), rank);
         prev_s = (int)s;
       }
       ptx::wgmma_wait<0>();
       ptx::wgmma_fence_regs(acc);
-      if (lane == 0) ptx::mbar_arrive(ptx::smem_u32(empty_bar + prev_s));
-      if (g.ksplit > 1) {
+      if (lane == 0) release_stage<CL>(ptx::smem_u32(empty_bar + prev_s), rank);
+      if (CL == 1 && g.ksplit > 1) {
         // ---- split-K: park the fp32 partial, the last split to arrive reduces + finishes the tile ----
         float* part = g.ws + (long long)(tile * g.ksplit + split) * BM * BN;
         if (live) {
@@ -499,6 +548,8 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       if (live) epilogue_frag<BN>(g, acc, stg, lane, m0 + wrow, n0);
     }
   }
+  // paired: no CTA leaves while its peer may still multicast into its shared memory or arrive on its barriers
+  if constexpr (CL == 2) ptx::cluster_sync();
 }
 
 // ---------------------------------------------------------------------------------------------- host
@@ -626,14 +677,46 @@ static int splitk_scratch(cudaStream_t stream, size_t need_bytes, int need_count
 
 struct ConvInfo { int B, H, W, C, Wt; };   // implicit 3x3 conv: d->A is the NHWC map, d->M = B*H*W, d->K = 9*C
 
+// how many 2-CTA clusters of gemm_bf16_wgmma_kernel<BN, 2> the device runs at once (one CTA per SM; a cluster's CTAs share a GPC)
+template <int BN>
+static int pair_clusters() {
+  static int n = 0;
+  if (n == 0) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(2 * ((device_sm_count() + 1) / 2)); cfg.blockDim = dim3(kGemmThreads); cfg.dynamicSmemBytes = GemmCfg<BN>::kSmemBytes;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeClusterDimension;
+    at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+    cfg.attrs = at; cfg.numAttrs = 1;
+    int c = 0;
+    if (cudaOccupancyMaxActiveClusters(&c, gemm_bf16_wgmma_kernel<BN, 2>, &cfg) != cudaSuccess || c < 1) {
+      set_error("cudaOccupancyMaxActiveClusters failed for the paired GEMM (BN = %d)", BN);
+      return 0;
+    }
+    n = c;
+  }
+  return n;
+}
+
 template <int BN>
 static int launch_gemm(const fo1_gemm_desc* d, cudaStream_t stream, int ksplit = 1, const ConvInfo* conv = nullptr) {
   using Cfg = GemmCfg<BN>;
   static bool attr_set = false;
   if (!attr_set) {
-    FO1_CUDA(cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+    FO1_CUDA(cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<BN, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+    FO1_CUDA(cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<BN, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
     attr_set = true;
   }
+  // CTA pairs: each CTA of a pair loads its own A tile and half of the W tile, multicast into both, which halves the W bytes a CTA pulls
+  // per k-block.  Measured on H100, that pays on the large weights (LLM down 2.85 -> 2.55 ms, ViT gated fc1 7.09 -> 6.79 ms with pairs
+  // alone) and costs on the small ones, whose pair lockstep outweighs the saved traffic (LLM qkv 18 % slower), hence the cutoff
+  // kPairMinWeightBytes.  Skinny problems (one m-tile: decode, LM head) and split-K keep one CTA per tile, and so does the implicit
+  // 3x3 conv, whose weights in this engine (9 x 512 x 512) are far below the cutoff.  A pinned tile width pairs whenever it can.
+  const int tiles_m = ceil_div(d->M, BM);
+  const int num_kb = ceil_div(d->K, BK);
+  const int kb_per_split = ceil_div(num_kb, ksplit);
+  const bool paired = tiles_m >= 2 && ceil_div(num_kb, kb_per_split) == 1 && conv == nullptr &&
+                      (d->tile_n != 0 || 2LL * d->N * d->K >= kPairMinWeightBytes);
   CUtensorMap tmA, tmW;
   // one m-tile only (decode: M = batch): fetch just the live rows of A, rounded to the 8-row swizzle atom; a live
   // warpgroup still multiplies all 64 of its smem rows, rows >= M hold stale data whose results are never stored
@@ -643,7 +726,7 @@ static int launch_gemm(const fo1_gemm_desc* d, cudaStream_t stream, int ksplit =
   } else {
     FO1_TRY(make_tmap_2d_bf16(&tmA, d->A, (uint64_t)d->K, (uint64_t)d->M, (uint64_t)d->lda, BK, a_rows));
   }
-  FO1_TRY(make_tmap_2d_bf16(&tmW, d->W, (uint64_t)d->K, (uint64_t)d->N, (uint64_t)d->ldw, BK, BN));
+  FO1_TRY(make_tmap_2d_bf16(&tmW, d->W, (uint64_t)d->K, (uint64_t)d->N, (uint64_t)d->ldw, BK, paired ? BN / 2 : BN));
   GemmArgs g;
   g.M = d->M; g.N = d->N; g.K = d->K;
   g.D = d->D; g.ldd = d->ldd; g.d_dtype = d->d_dtype;
@@ -652,7 +735,7 @@ static int launch_gemm(const fo1_gemm_desc* d, cudaStream_t stream, int ksplit =
   g.residual = static_cast<const __nv_bfloat16*>(d->residual); g.ldr = d->ldr;
   g.gated = d->gated;
   g.conv_cpb = conv ? conv->C / BK : 0; g.conv_H = conv ? conv->H : 0; g.conv_W = conv ? conv->W : 0; g.conv_Wt = conv ? conv->Wt : 0;
-  g.tiles_m = ceil_div(d->M, BM);
+  g.tiles_m = tiles_m;
   g.tiles_n = ceil_div(d->N, BN);
   g.stage_tx = (a_rows + BN) * BK * 2;
   // Skinny problems: the wgmma of a warpgroup reads whole 64-row halves of a stage, i.e. up to 16 KB from the slot's start -- past the
@@ -678,8 +761,7 @@ static int launch_gemm(const fo1_gemm_desc* d, cudaStream_t stream, int ksplit =
     static const bool direct_store = getenv("FO1_GEMM_DIRECT_STORE") != nullptr;   // A/B knob: per-row stores instead of the smem-staged lines
     g.coalesce = (d_ok && r_ok && !direct_store) ? 1 : 0;
   }
-  const int num_kb = ceil_div(d->K, BK);
-  g.kb_per_split = ceil_div(num_kb, ksplit);
+  g.kb_per_split = kb_per_split;
   g.ksplit = ceil_div(num_kb, g.kb_per_split);   // every split owns at least one k-block
   g.ws = nullptr; g.counters = nullptr;
   if (g.ksplit > 1) {
@@ -687,13 +769,21 @@ static int launch_gemm(const fo1_gemm_desc* d, cudaStream_t stream, int ksplit =
     FO1_TRY(splitk_scratch(stream, (size_t)g.tiles_m * g.tiles_n * g.ksplit * BM * BN * sizeof(float), g.tiles_m * g.tiles_n, &sc));
     g.ws = sc->ws; g.counters = sc->counters;
   }
-  const int tiles = g.tiles_m * g.tiles_n * g.ksplit;
-  const int grid = tiles < device_sm_count() ? tiles : device_sm_count();
+  int grid = 0;
+  if (paired) {
+    const int clusters = pair_clusters<BN>();
+    if (clusters == 0) return FO1_ERR_CUDA;
+    grid = 2 * std::min(clusters, ((g.tiles_m + 1) / 2) * g.tiles_n);
+  } else {
+    const int tiles = g.tiles_m * g.tiles_n * g.ksplit;
+    grid = tiles < device_sm_count() ? tiles : device_sm_count();
+  }
   char tag[96] = "gemm";
   if (g_prof_on) snprintf(tag, sizeof(tag), "%s:%dx%dx%d%s%s", d->M <= 128 ? "gemm_skinny" : "gemm", d->M, d->N, d->K, d->gated ? ":gated" : "", conv ? ":conv3x3" : "");
   ProfScope prof(tag, 2.0 * d->M * (double)d->N * d->K,
                  2.0 * ((double)d->M * d->K + (double)d->N * d->K + (double)d->M * (d->gated ? d->N / 2 : d->N)), stream);
-  launch_k(gemm_bf16_wgmma_kernel<BN>, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, tmA, tmW, g);
+  if (paired) launch_k_cluster(2, gemm_bf16_wgmma_kernel<BN, 2>, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, tmA, tmW, g);
+  else launch_k(gemm_bf16_wgmma_kernel<BN, 1>, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, tmA, tmW, g);
   FO1_LAUNCH_CHECK();
   return FO1_OK;
 }

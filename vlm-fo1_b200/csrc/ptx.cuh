@@ -44,6 +44,25 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   }
 }
 
+// ---- thread-block clusters ---------------------------------------------------------------------
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+// every thread of every CTA of the cluster; orders the shared-memory (and mbarrier) accesses before it against those after it
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release;\nbarrier.cluster.wait.acquire;" ::: "memory");
+}
+// arrive on the mbarrier at the same shared-memory offset in CTA `rank` of the cluster.  Default (CTA-scope) release: it only signals
+// that this warp's wgmma reads of a stage have retired (wgmma.wait_group), and a cluster-scope release would cost a GPU-wide fence
+// per k-block.
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t rank) {
+  uint32_t remote;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(bar), "r"(rank));
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
+}
+
 // ---- TMA (cp.async.bulk.tensor) ----------------------------------------------------------------
 __device__ __forceinline__ void prefetch_tmap(const void* tmap) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(tmap) : "memory");
@@ -52,6 +71,14 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const void* tmap, uint
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(dst), "l"(tmap), "r"(bar), "r"(c0), "r"(c1)
+      : "memory");
+}
+// the same box into the same shared-memory offset of every CTA in `cta_mask`, each completing the bytes on its own mbarrier at
+// `bar`'s offset
+__device__ __forceinline__ void tma_load_2d_multicast(uint32_t dst, const void* tmap, uint32_t bar, int c0, int c1, uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
+      ::"r"(dst), "l"(tmap), "r"(bar), "r"(c0), "r"(c1), "h"(cta_mask)
       : "memory");
 }
 __device__ __forceinline__ void tma_load_3d(uint32_t dst, const void* tmap, uint32_t bar, int c0, int c1, int c2) {
