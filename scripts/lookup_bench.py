@@ -26,8 +26,8 @@ import torch
 
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, REPO)
-KERNELS = ("lookup_drafts_kernel", "lookup_rows_kernel", "lookup_accept_kernel", "decode_attn_rows_kernel", "decode_attn_kernel",
-           "decode_attn_combine_kernel", "rope_kv_append_map_kernel", "rope_kv_append_kernel", "argmax_kernel")
+KERNELS = ("lookup_drafts_kernel", "lookup_rows_kernel", "lookup_accept_kernel", "decode_attn_kernel<true>", "decode_attn_kernel<false>",
+           "decode_attn_combine_kernel", "rope_kv_append_kernel<true>", "rope_kv_append_kernel<false>", "argmax_kernel")
 
 
 def card():

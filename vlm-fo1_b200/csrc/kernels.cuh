@@ -43,10 +43,10 @@ int vit_rope_apply(bf16* qkv, const float* cos_sin, int T, int heads, int head_d
 int mrope_table(const int* pos3 /*[3][T]*/, float* cos_sin, int T, int head_dim, int sec_t, int sec_h, int sec_w, float theta, cudaStream_t s);
 // rotate n_heads consecutive heads (q then k) of every row in place with a [T][hd/2] cos / sin table
 int rope_apply(bf16* x, long long ld, const float* cos_sin, int T, int n_heads, int head_dim, cudaStream_t s);
-// decode step: rotate q in place, append rotated K and V of row b to the cache at cache_len[b].  row_slot (the prompt-lookup
-// verify step): row b goes to slot row_slot[b] at index cache_len[b] (then a per-row index)
-int rope_kv_append(bf16* qkv, long long ld, const float* cos_sin, int T, int q_heads, int kv_heads, int head_dim, const int* cache_len,
-                   bf16* kc, bf16* vc, int cap, cudaStream_t s, const int* row_slot = nullptr);
+// decode step: rotate q in place, append rotated K and V of row b to the cache at index idx[b] of slot b, or of slot row_slot[b]
+// when the row map is given (the prompt-lookup verify step)
+int rope_kv_append(bf16* qkv, long long ld, const float* cos_sin, int T, int q_heads, int kv_heads, int head_dim, const int* idx,
+                   const int* row_slot, bf16* kc, bf16* vc, int cap, cudaStream_t s);
 
 // ---- attention_tc.cu ----
 // varlen flash attention over packed rows (wgmma / TMA); q/k/v may live in one packed buffer (pitches in elements)

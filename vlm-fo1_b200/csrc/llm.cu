@@ -12,6 +12,7 @@
 // prompt position only.
 #include <algorithm>
 #include <cmath>
+#include <type_traits>
 
 #include "beam.cuh"
 #include "decode_loop.cuh"
@@ -42,20 +43,8 @@ __global__ void __launch_bounds__(256) embed_tokens_kernel(const int* __restrict
   for (int c = threadIdx.x * 8; c < H; c += blockDim.x * 8) *reinterpret_cast<uint4*>(dst + c) = *reinterpret_cast<const uint4*>(src + c);
 }
 
-// prefill: copy the rotated K and V of packed row r into the cache slot (seq[r], t[r])
-__global__ void __launch_bounds__(128) kv_store_kernel(const bf16* __restrict__ qkv, long long ld, int q_dim, int kv_dim,
-                                                       const int* __restrict__ row_seq, const int* __restrict__ row_t,
-                                                       bf16* __restrict__ kc, bf16* __restrict__ vc, int cap) {
-  const int r = blockIdx.x;
-  const long long slot = ((long long)row_seq[r] * cap + row_t[r]) * kv_dim;
-  const bf16* kp = qkv + (long long)r * ld + q_dim;
-  for (int c = threadIdx.x * 8; c < kv_dim; c += blockDim.x * 8) {
-    *reinterpret_cast<uint4*>(kc + slot + c) = *reinterpret_cast<const uint4*>(kp + c);
-    *reinterpret_cast<uint4*>(vc + slot + c) = *reinterpret_cast<const uint4*>(kp + kv_dim + c);
-  }
-}
-// shared-prefix prefill: copy the rotated K and V of prefix row r (position row_gt[r].y of group row_gt[r].x) into the cache slot of
-// every member of the group (members[grp_off[g] .. grp_off[g + 1]))
+// prefill: copy the rotated K and V of packed row r (position row_gt[r].y of group row_gt[r].x) into the cache slot of every member of
+// the group (members[grp_off[g] .. grp_off[g + 1])).  prefill_plan() builds the groups of each kind of call.
 __global__ void __launch_bounds__(64) kv_fanout_kernel(const bf16* __restrict__ qkv, long long ld, int q_dim, int kv_dim,
                                                        const int2* __restrict__ row_gt, const int* __restrict__ grp_off,
                                                        const int* __restrict__ members, bf16* __restrict__ kc, bf16* __restrict__ vc, int cap) {
@@ -114,153 +103,19 @@ __device__ __forceinline__ void dec_ldsm(uint32_t (&r)[4], uint32_t addr) {
 __device__ __forceinline__ void dec_ldsm_t(uint32_t (&r)[4], uint32_t addr) {
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
 }
+// Query row b reads cache slot b, or (MAPPED: the prompt-lookup verify step) slot row_slot[b], up to its own index idx[b].  The verify
+// launch takes the plain step's split count, so a row's bits are those of the plain step at its position.
+template <bool MAPPED>
 __global__ void __launch_bounds__(kDecWarps * 32) decode_attn_kernel(const bf16* __restrict__ q, long long ldq, const bf16* __restrict__ kc,
-                                                                     const bf16* __restrict__ vc, const int* __restrict__ cache_len, int cap,
-                                                                     int kv_heads, int G, float* __restrict__ part, float scale) {
+                                                                     const bf16* __restrict__ vc, const int* __restrict__ row_slot,
+                                                                     const int* __restrict__ idx, int cap, int kv_heads, int G,
+                                                                     float* __restrict__ part, float scale) {
   constexpr int HD = 128;
   extern __shared__ __align__(128) uint8_t dec_smem[];
   const int b = blockIdx.x, kvh = blockIdx.y, sp = blockIdx.z;
   griddep_launch();
   griddep_wait();
-  const int n = cache_len[b] + 1;  // the step's own K/V was appended at index cache_len[b]
-  const int n_splits = gridDim.z;
-  const int chunk = ((n + n_splits - 1) / n_splits + 15) & ~15;
-  const int t_begin = sp * chunk, t_end = min(n, t_begin + chunk);
-  const int kv_dim = kv_heads * HD;
-  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int g = lane >> 2, t = lane & 3;
-  // Q fragments (A operand, rows = heads): a0 = dims (16 ks + 2t, +1), a2 = dims (16 ks + 8 + 2t, +1) of head g
-  uint32_t qa[8][2];
-#pragma unroll
-  for (int ks = 0; ks < 8; ++ks) { qa[ks][0] = 0u; qa[ks][1] = 0u; }
-  if (g < G) {
-    const bf16* qp = q + (long long)b * ldq + (long long)(kvh * G + g) * HD + 2 * t;
-#pragma unroll
-    for (int ks = 0; ks < 8; ++ks) {
-      qa[ks][0] = *reinterpret_cast<const uint32_t*>(qp + ks * 16);
-      qa[ks][1] = *reinterpret_cast<const uint32_t*>(qp + ks * 16 + 8);
-    }
-  }
-  const float sc = scale * 1.4426950408889634f;
-  float m = -INFINITY, l = 0.f, o[16][4];
-#pragma unroll
-  for (int j = 0; j < 16; ++j) { o[j][0] = o[j][1] = o[j][2] = o[j][3] = 0.f; }
-
-  const uint32_t ring = (uint32_t)__cvta_generic_to_shared(dec_smem) + w * kDecStages * kDecTileBytes;
-  // copy plan: instruction i moves chunk (key = 2i + lane/16, 16-byte chunk lane%16) of the K half and of the V half
-  const int cp_key = lane >> 4, cp_chunk = lane & 15;
-  const bf16* kbase = kc + (long long)b * cap * kv_dim + kvh * HD + cp_chunk * 8;
-  const bf16* vbase = vc + (long long)b * cap * kv_dim + kvh * HD + cp_chunk * 8;
-  int t_issue = t_begin + w * 16;
-  uint32_t st_issue = 0, st_done = 0;
-  auto issue_tile = [&]() {
-    if (t_issue < t_end) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int key = 2 * i + cp_key, tok = t_issue + key;
-        const bool ok = tok < t_end;                          // keys beyond the split: zero rows (their scores are masked)
-        const long long off = (long long)(ok ? tok : t_begin) * kv_dim;
-        const uint32_t dst = ring + st_issue + key * 256 + ((cp_chunk ^ (key & 7)) << 4);
-        dec_cp16(dst, kbase + off, ok);
-        dec_cp16(dst + 16 * 256, vbase + off, ok);
-      }
-      t_issue += kDecWarps * 16;
-      st_issue = (st_issue == (kDecStages - 1) * kDecTileBytes) ? 0u : st_issue + kDecTileBytes;
-    }
-    asm volatile("cp.async.commit_group;" ::: "memory");
-  };
-  issue_tile();
-  issue_tile();
-  // ldmatrix lane roles: S: matrix m = lane/8 -> (keys (m/2)*8 + r, chunk 2 ks + (m&1)); PV (trans): (keys (m&1)*8 + r, chunk c + m/2)
-  const int lr = lane & 7, lm = lane >> 3;
-  for (int t0 = t_begin + w * 16; t0 < t_end; t0 += kDecWarps * 16) {
-    issue_tile();
-    asm volatile("cp.async.wait_group 2;" ::: "memory");
-    __syncwarp();
-    const uint32_t kt = ring + st_done, vt = kt + 16 * 256;
-    float s[2][4];
-#pragma unroll
-    for (int i = 0; i < 2; ++i) { s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f; }
-#pragma unroll
-    for (int ks = 0; ks < 8; ++ks) {
-      uint32_t bk[4];
-      const int key = (lm >> 1) * 8 + lr;
-      dec_ldsm(bk, kt + key * 256 + (((2 * ks + (lm & 1)) ^ (key & 7)) << 4));
-      mma_m16n8k16(s[0], qa[ks][0], qa[ks][1], bk[0], bk[1]);
-      mma_m16n8k16(s[1], qa[ks][0], qa[ks][1], bk[2], bk[3]);
-    }
-    float tmax = -INFINITY;
-#pragma unroll
-    for (int i = 0; i < 2; ++i)
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        s[i][e] = (t0 + i * 8 + 2 * t + e < t_end) ? s[i][e] * sc : -INFINITY;
-        tmax = fmaxf(tmax, s[i][e]);
-      }
-    tmax = fmaxf(tmax, __shfl_xor_sync(0xffffffffu, tmax, 1));
-    tmax = fmaxf(tmax, __shfl_xor_sync(0xffffffffu, tmax, 2));
-    const float mn = fmaxf(m, tmax);            // key t0 is always valid: mn is finite
-    const float alpha = exp2f(m - mn);          // m = -inf on the first tile -> 0
-    const float p00 = exp2f(s[0][0] - mn), p01 = exp2f(s[0][1] - mn), p10 = exp2f(s[1][0] - mn), p11 = exp2f(s[1][1] - mn);
-    l = l * alpha + (p00 + p01) + (p10 + p11);
-    m = mn;
-    const uint32_t pa0 = pack2_bf16(p00, p01), pa2 = pack2_bf16(p10, p11);
-#pragma unroll
-    for (int c = 0; c < 16; c += 2) {
-      uint32_t bv[4];
-      const int key = (lm & 1) * 8 + lr;
-      dec_ldsm_t(bv, vt + key * 256 + (((c + (lm >> 1)) ^ (key & 7)) << 4));
-      o[c][0] *= alpha; o[c][1] *= alpha; o[c + 1][0] *= alpha; o[c + 1][1] *= alpha;
-      mma_m16n8k16(o[c], pa0, pa2, bv[0], bv[1]);
-      mma_m16n8k16(o[c + 1], pa0, pa2, bv[2], bv[3]);
-    }
-    __syncwarp();                               // the stage may be refilled by the next issue_tile()
-    st_done = (st_done == (kDecStages - 1) * kDecTileBytes) ? 0u : st_done + kDecTileBytes;
-  }
-  asm volatile("cp.async.wait_group 0;" ::: "memory");
-  l += __shfl_xor_sync(0xffffffffu, l, 1);
-  l += __shfl_xor_sync(0xffffffffu, l, 2);
-  __syncthreads();                              // every warp is done with its ring: reuse it for the merge
-  float* sm_o = reinterpret_cast<float*>(dec_smem);                    // [kDecWarps][8][HD]
-  float* sm_m = sm_o + kDecWarps * 8 * HD;                             // [kDecWarps][8]
-  float* sm_l = sm_m + kDecWarps * 8;
-  if (t == 0) { sm_m[w * 8 + g] = m; sm_l[w * 8 + g] = l; }
-#pragma unroll
-  for (int j = 0; j < 16; ++j)
-    *reinterpret_cast<float2*>(&sm_o[(w * 8 + g) * HD + j * 8 + 2 * t]) = make_float2(o[j][0], o[j][1]);
-  __syncthreads();
-  const int d = threadIdx.x;   // kDecWarps * 32 == HD
-  for (int r = 0; r < G; ++r) {
-    float mm = -INFINITY;
-#pragma unroll
-    for (int ww = 0; ww < kDecWarps; ++ww) mm = fmaxf(mm, sm_m[ww * 8 + r]);
-    float num = 0.f, den = 0.f;
-#pragma unroll
-    for (int ww = 0; ww < kDecWarps; ++ww) {
-      const float f = (sm_m[ww * 8 + r] == -INFINITY) ? 0.f : exp2f(sm_m[ww * 8 + r] - mm);
-      num += sm_o[(ww * 8 + r) * HD + d] * f;
-      den += sm_l[ww * 8 + r] * f;
-    }
-    // partial record per (b, head, split): [m, l, pad, pad, acc[128]]
-    float* rec = part + (((long long)b * kv_heads * G + kvh * G + r) * kDecSplits + sp) * (HD + 4);
-    if (d == 0) { rec[0] = mm; rec[1] = den; }
-    rec[4 + d] = num;
-  }
-}
-
-// The prompt-lookup verify step's decode attention: decode_attn_kernel with query row b = blockIdx.x reading cache slot row_slot[b]
-// up to its own index idx[b].  A separate copy, so that decode_attn_kernel keeps its code; the arithmetic of each (row, split) is
-// decode_attn_kernel's, and the launch takes the plain step's split count, so a row's bits are those of the plain step at its position.
-__global__ void __launch_bounds__(kDecWarps * 32) decode_attn_rows_kernel(const bf16* __restrict__ q, long long ldq, const bf16* __restrict__ kc,
-                                                                          const bf16* __restrict__ vc, const int* __restrict__ row_slot,
-                                                                          const int* __restrict__ idx, int cap, int kv_heads, int G,
-                                                                          float* __restrict__ part, float scale) {
-  constexpr int HD = 128;
-  extern __shared__ __align__(128) uint8_t dec_smem[];
-  const int b = blockIdx.x, kvh = blockIdx.y, sp = blockIdx.z;
-  griddep_launch();
-  griddep_wait();
-  const int slot = row_slot[b];
+  const int slot = MAPPED ? row_slot[b] : b;
   const int n = idx[b] + 1;        // the row's own K/V was appended at index idx[b]
   const int n_splits = gridDim.z;
   const int chunk = ((n + n_splits - 1) / n_splits + 15) & ~15;
@@ -386,6 +241,7 @@ __global__ void __launch_bounds__(kDecWarps * 32) decode_attn_rows_kernel(const 
     rec[4 + d] = num;
   }
 }
+
 // merge the kDecSplits partials of one (sequence, q head): out = sum_s acc_s * 2^(m_s - m) / sum_s l_s * 2^(m_s - m)
 __global__ void __launch_bounds__(128) decode_attn_combine_kernel(const float* __restrict__ part, bf16* __restrict__ out, long long ldo,
                                                                   int q_heads, int n_splits) {
@@ -408,12 +264,12 @@ __global__ void __launch_bounds__(128) decode_attn_combine_kernel(const float* _
   out[(long long)b * ldo + (long long)h * HD + d] = __float2bfloat16_rn(num / den);
 }
 
-// host side of the decode attention: split count = one wave of blocks (2 per SM: 96 KB of shared memory each).  row_slot (the
-// prompt-lookup verify step): row r reads slot row_slot[r] up to index cache_len[r] (then a per-row index), and the split count is
-// the one of the plain step over n_seqs sequences, so each row's key chunks are those the plain step at its position would use
-static int decode_attention(const bf16* q, long long ldq, const bf16* kc, const bf16* vc, const int* cache_len, int rows, int cap,
-                            int q_heads, int kv_heads, int hd, float scale, bf16* out, long long ldo, float* part, cudaStream_t s,
-                            const int* row_slot = nullptr, int n_seqs = 0) {
+// host side of the decode attention: split count = one wave of blocks (2 per SM: 96 KB of shared memory each) over n_seqs sequences.
+// Row r reads its cache slot up to index idx[r]; row_slot (the prompt-lookup verify step) maps the rows to n_seqs slots, and the split
+// count stays the plain step's, so each row's key chunks are those the plain step at its position would use.
+static int decode_attention(const bf16* q, long long ldq, const bf16* kc, const bf16* vc, const int* idx, const int* row_slot, int rows,
+                            int n_seqs, int cap, int q_heads, int kv_heads, int hd, float scale, bf16* out, long long ldo, float* part,
+                            cudaStream_t s) {
   const int G = kv_heads > 0 ? q_heads / kv_heads : 0;
   if (kv_heads <= 0 || q_heads % kv_heads != 0 || G > 8 || hd != 128) {
     set_error("decode attention: %d/%d heads, head_dim %d unsupported (GQA group <= 8, head_dim 128)", q_heads, kv_heads, hd);
@@ -422,22 +278,18 @@ static int decode_attention(const bf16* q, long long ldq, const bf16* kc, const 
   if (rows == 0) return FO1_OK;
   static bool attr_set = false;
   if (!attr_set) {
-    FO1_CUDA(cudaFuncSetAttribute(decode_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kDecSmemBytes));
-    FO1_CUDA(cudaFuncSetAttribute(decode_attn_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kDecSmemBytes));
+    FO1_CUDA(cudaFuncSetAttribute(decode_attn_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDecSmemBytes));
+    FO1_CUDA(cudaFuncSetAttribute(decode_attn_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDecSmemBytes));
     attr_set = true;
   }
   const int slots = 2 * device_sm_count();
-  const int n_splits = std::max(1, std::min(kDecSplits, slots / std::max(1, (row_slot ? n_seqs : rows) * kv_heads)));
-  dim3 grid(rows, kv_heads, n_splits);
-  if (row_slot != nullptr) {
-    ProfScope prof("decode_attn_rows", 0.0, 0.0, s);
-    launch_k(decode_attn_rows_kernel, grid, dim3(kDecWarps * 32), kDecSmemBytes, s, q, ldq, kc, vc, row_slot, cache_len, cap, kv_heads, G,
-             part, scale);
-  } else {
-    ProfScope prof("decode_attn", 0.0, 0.0, s);
-    launch_k(decode_attn_kernel, grid, dim3(kDecWarps * 32), kDecSmemBytes, s, q, ldq, kc, vc, cache_len, cap, kv_heads, G, part, scale);
+  const int n_splits = std::max(1, std::min(kDecSplits, slots / std::max(1, n_seqs * kv_heads)));
+  {
+    ProfScope prof(row_slot != nullptr ? "decode_attn_rows" : "decode_attn", 0.0, 0.0, s);
+    launch_k(row_slot != nullptr ? decode_attn_kernel<true> : decode_attn_kernel<false>, dim3(rows, kv_heads, n_splits), dim3(kDecWarps * 32),
+             kDecSmemBytes, s, q, ldq, kc, vc, row_slot, idx, cap, kv_heads, G, part, scale);
+    FO1_LAUNCH_CHECK();
   }
-  FO1_LAUNCH_CHECK();
   launch_k(decode_attn_combine_kernel, dim3(rows, q_heads), dim3(128), 0, s, (const float*)part, out, ldo, q_heads, n_splits);
   FO1_LAUNCH_CHECK();
   return FO1_OK;
@@ -612,56 +464,74 @@ static int ensure_state(Model* m, int B, int n_stop, DecodeState* st) {
 // size; the width alone decides for models wider than it serves
 static NormKernel seq_norm_kernel(int H) { return H <= kNormBlockMaxCols ? NORM_BLOCK : NORM_WARP; }
 
-// device tables of a shared-prefix prefill: the packed rows are the groups' prefix rows (one causal segment per group), then every
-// sequence's own rows
-struct PrefixTables {
-  int n_pre = 0, n_groups = 0;
-  const int *cu = nullptr, *tiles = nullptr;                  // prefix segments and their query tiles
-  int n_tiles = 0;
-  const int *row_gt = nullptr, *grp_off = nullptr, *members = nullptr;   // kv_fanout_kernel
-  const int *own_seq = nullptr, *own_t = nullptr;             // kv_store_kernel of the own rows
-  const int *own_rowseg = nullptr, *own_tiles = nullptr;      // the cache-reading attention of the own rows
-  int n_own_tiles = 0;
+// one generate call, described once by llm_generate: the caller's descriptors, the decode mode, the column sink, and the device state
+// of beam search (with its host table of length-penalty divisors) or of prompt lookup
+struct GenerateCall {
+  fo1_generate_desc* d;
+  const fo1_prefix_desc* px;        // shared prefix (null: none)
+  const fo1_sampling_desc* sp;
+  const fo1_score_desc* sc;
+  const fo1_stream_desc* stm;
+  DecodeMode mode;
+  ColumnSink k;
+  const fo1_beam_desc* bmd;         // beam search (null: none): `beam`, `lp_div`
+  BeamArgs beam;
+  std::vector<float> lp_div;
+  const fo1_lookup_desc* lkd;       // prompt lookup (null: none): `lookup`
+  LookupArgs lookup;
 };
 
-// one decoder layer over `rows` packed rows.  x_in -> x_out (x_mid scratch).  prefill: varlen causal attention
-// + cache fill (px: the shared-prefix split of it); decode: cache append + single-query attention.
-struct LayerBuf { bf16 *xn, *qkv, *att, *x_mid, *h; float* dec_part; int* rowseg = nullptr; double attn_flops = 0.0; const int* tiles = nullptr; int n_tiles = 0;
-                  const PrefixTables* px = nullptr;
-                  const int *fan_gt = nullptr, *fan_off = nullptr, *fan_mem = nullptr;    // beam search: each prompt row into its N slots
-                  const int *row_slot = nullptr, *row_idx = nullptr; int n_seqs = 0; };   // prompt-lookup verify: rows of n_seqs slots
+// the scratch buffers of a decoder layer over packed rows
+struct LayerBuf { bf16 *xn, *qkv, *att, *x_mid, *h; float* dec_part; int* rowseg; };
 
-// the prefill attention of a shared-prefix layer: prefix K/V into every member's slot, own K/V into the own slot, then the prefix rows
-// as causal segments and the own rows against the cache
-static int prefix_layer_attention(Model* m, const LayerBuf& B_, int rows, bf16* kc, bf16* vc, cudaStream_t s, bool dry) {
+// the attention of a prefill layer: the rotated K/V of every packed row into the cache through the write map (kv_fanout_kernel), the
+// causal attention over the packed segments, and with a shared prefix the own rows (the rows after the segments) against the cache
+// (own.k / own.v are the layer's cache, set per layer)
+struct PrefillAttn {
+  const int2* row_gt;
+  const int *grp_off, *members;
+  AttnArgs causal, own;             // own.total_rows == 0: no shared prefix
+};
+// the attention of a decode step: row r appends its K/V at index idx[r] of cache slot r, or of slot row_slot[r], and attends the slot up
+// to there; n_seqs sequences set the key split
+struct DecodeAttn {
+  const int* idx;
+  const int* row_slot;
+  int n_seqs;
+};
+
+static int layer_attention(Model* m, const PrefillAttn& p, const LayerBuf& b, int rows, const float* cs, bf16* kc, bf16* vc, cudaStream_t s,
+                           bool dry) {
   const fo1_model_config& c = m->cfg;
-  const PrefixTables& p = *B_.px;
   const int hd = c.llm_head_dim, QD = c.llm_heads * hd, KD = c.llm_kv_heads * hd, ldq = QD + 2 * KD;
-  const int np = p.n_pre, no = rows - np;
+  FO1_RUN(rope_apply(b.qkv, ldq, cs, rows, c.llm_heads + c.llm_kv_heads, hd, s));   // q|k heads are contiguous in the packed row
   if (!dry) {
-    kv_fanout_kernel<<<np, 64, 0, s>>>(B_.qkv, ldq, QD, KD, reinterpret_cast<const int2*>(p.row_gt), p.grp_off, p.members, kc, vc, m->kv_cap);
-    FO1_LAUNCH_CHECK();
-    kv_store_kernel<<<no, 128, 0, s>>>(B_.qkv + (size_t)np * ldq, ldq, QD, KD, p.own_seq, p.own_t, kc, vc, m->kv_cap);
+    kv_fanout_kernel<<<rows, 64, 0, s>>>(b.qkv, ldq, QD, KD, p.row_gt, p.grp_off, p.members, kc, vc, m->kv_cap);
     FO1_LAUNCH_CHECK();
   }
-  AttnArgs a;
-  a.q = B_.qkv; a.k = B_.qkv + QD; a.v = B_.qkv + QD + KD; a.o = B_.att;
-  a.ldq = a.ldk = a.ldv = ldq; a.ldo = QD;
-  a.cu_seqlens = p.cu; a.n_seqs = p.n_groups; a.max_seqlen = 0; a.total_rows = np; a.rowseg = B_.rowseg; a.tiles = p.tiles; a.n_tiles = p.n_tiles;
-  a.q_heads = c.llm_heads; a.kv_heads = c.llm_kv_heads; a.head_dim = hd;
-  a.scale = 1.0f / sqrtf((float)hd); a.causal = 1;
-  FO1_RUN(attention_varlen(a, s));
-  AttnArgs o = a;
-  o.q = B_.qkv + (size_t)np * ldq; o.k = kc; o.v = vc; o.o = B_.att + (size_t)np * QD;
-  o.ldk = o.ldv = KD;
-  o.cu_seqlens = nullptr; o.n_seqs = m->kv_batch; o.total_rows = no; o.rowseg = p.own_rowseg; o.tiles = p.own_tiles; o.n_tiles = p.n_own_tiles;
-  o.causal = 0; o.kv_rows = m->kv_batch * m->kv_cap;
-  FO1_RUN(attention_varlen(o, s));
+  FO1_RUN(attention_varlen(p.causal, s));
+  if (p.own.total_rows > 0) {
+    AttnArgs o = p.own;
+    o.k = kc; o.v = vc;
+    FO1_RUN(attention_varlen(o, s));
+  }
   return FO1_OK;
 }
 
-static int llm_layer(Model* m, int li, const bf16* x_in, bf16* x_out, const LayerBuf& B_, int rows, const float* cs, bool prefill,
-                     const int* d_cu, int n_seqs, int max_len, const int* d_row_seq, const int* d_row_t, const DecodeState* st,
+static int layer_attention(Model* m, const DecodeAttn& p, const LayerBuf& b, int rows, const float* cs, bf16* kc, bf16* vc, cudaStream_t s,
+                           bool dry) {
+  const fo1_model_config& c = m->cfg;
+  const int hd = c.llm_head_dim, QD = c.llm_heads * hd, KD = c.llm_kv_heads * hd, ldq = QD + 2 * KD;
+  FO1_RUN(rope_kv_append(b.qkv, ldq, cs, rows, c.llm_heads, c.llm_kv_heads, hd, p.idx, p.row_slot, kc, vc, m->kv_cap, s));
+  FO1_RUN(decode_attention(b.qkv, ldq, kc, vc, p.idx, p.row_slot, rows, p.n_seqs, m->kv_cap, c.llm_heads, c.llm_kv_heads, hd,
+                           1.0f / sqrtf((float)hd), b.att, QD, b.dec_part, s));
+  return FO1_OK;
+}
+
+// one decoder layer over `rows` packed rows, x_in -> x_out, with the attention of a prefill (PrefillAttn) or of a decode step
+// (DecodeAttn).  `dry` (the pass that sizes the arena) skips every launch.
+template <class Attn>
+static int llm_layer(Model* m, int li, const bf16* x_in, bf16* x_out, const LayerBuf& b, int rows, const float* cs, const Attn& at,
                      cudaStream_t s, bool dry) {
   const fo1_model_config& c = m->cfg;
   const LlmLayerW& L = m->llm.layer[li];
@@ -670,38 +540,14 @@ static int llm_layer(Model* m, int li, const bf16* x_in, bf16* x_out, const Laye
   const size_t layer_stride = (size_t)m->kv_batch * m->kv_cap * KD;
   bf16* kc = static_cast<bf16*>(m->kv_cache) + (size_t)li * layer_stride;
   bf16* vc = static_cast<bf16*>(m->kv_cache) + ((size_t)c.llm_layers + li) * layer_stride;
-  const NormKernel nk = prefill ? NORM_WARP : seq_norm_kernel(H);
-  FO1_RUN(rmsnorm(x_in, H, L.ln1, B_.xn, H, rows, H, c.rms_eps, nk, s));
-  FO1_RUN(linear(B_.xn, H, L.qkv_w, H, B_.qkv, ldq, FO1_BF16, rows, ldq, H, L.qkv_b, FO1_BF16, FO1_EPI_NONE, nullptr, 0, 0, s));
-  if (prefill && B_.px != nullptr) {
-    FO1_RUN(rope_apply(B_.qkv, ldq, cs, rows, c.llm_heads + c.llm_kv_heads, hd, s));
-    FO1_TRY(prefix_layer_attention(m, B_, rows, kc, vc, s, dry));
-  } else if (prefill) {
-    FO1_RUN(rope_apply(B_.qkv, ldq, cs, rows, c.llm_heads + c.llm_kv_heads, hd, s));   // q|k heads are contiguous in the packed row
-    if (!dry && B_.fan_gt != nullptr) {
-      kv_fanout_kernel<<<rows, 64, 0, s>>>(B_.qkv, ldq, QD, KD, reinterpret_cast<const int2*>(B_.fan_gt), B_.fan_off, B_.fan_mem, kc, vc, m->kv_cap);
-      FO1_LAUNCH_CHECK();
-    } else if (!dry) {
-      kv_store_kernel<<<rows, 128, 0, s>>>(B_.qkv, ldq, QD, KD, d_row_seq, d_row_t, kc, vc, m->kv_cap);
-      FO1_LAUNCH_CHECK();
-    }
-    AttnArgs a;
-    a.q = B_.qkv; a.k = B_.qkv + QD; a.v = B_.qkv + QD + KD; a.o = B_.att;
-    a.ldq = a.ldk = a.ldv = ldq; a.ldo = QD;
-    a.cu_seqlens = d_cu; a.n_seqs = n_seqs; a.max_seqlen = max_len; a.total_rows = rows; a.rowseg = B_.rowseg; a.flops = B_.attn_flops; a.tiles = B_.tiles; a.n_tiles = B_.n_tiles;
-    a.q_heads = c.llm_heads; a.kv_heads = c.llm_kv_heads; a.head_dim = hd;
-    a.scale = 1.0f / sqrtf((float)hd); a.causal = 1;
-    FO1_RUN(attention_varlen(a, s));
-  } else if (!dry) {
-    const int* idx = B_.row_slot ? B_.row_idx : st->cache_len;
-    FO1_RUN(rope_kv_append(B_.qkv, ldq, cs, rows, c.llm_heads, c.llm_kv_heads, hd, idx, kc, vc, m->kv_cap, s, B_.row_slot));
-    FO1_RUN(decode_attention(B_.qkv, ldq, kc, vc, idx, rows, m->kv_cap, c.llm_heads, c.llm_kv_heads, hd,
-                             1.0f / sqrtf((float)hd), B_.att, QD, B_.dec_part, s, B_.row_slot, B_.n_seqs));
-  }
-  FO1_RUN(linear(B_.att, QD, L.o_w, QD, B_.x_mid, H, FO1_BF16, rows, H, QD, nullptr, 0, FO1_EPI_NONE, x_in, H, 0, s));
-  FO1_RUN(rmsnorm(B_.x_mid, H, L.ln2, B_.xn, H, rows, H, c.rms_eps, nk, s));
-  FO1_RUN(linear(B_.xn, H, L.gateup_w, H, B_.h, Ip, FO1_BF16, rows, 2 * Ip, H, nullptr, 0, FO1_EPI_SILU, nullptr, 0, 1, s));
-  FO1_RUN(linear(B_.h, Ip, L.down_w, Ip, x_out, H, FO1_BF16, rows, H, Ip, nullptr, 0, FO1_EPI_NONE, B_.x_mid, H, 0, s));
+  const NormKernel nk = std::is_same<Attn, PrefillAttn>::value ? NORM_WARP : seq_norm_kernel(H);
+  FO1_RUN(rmsnorm(x_in, H, L.ln1, b.xn, H, rows, H, c.rms_eps, nk, s));
+  FO1_RUN(linear(b.xn, H, L.qkv_w, H, b.qkv, ldq, FO1_BF16, rows, ldq, H, L.qkv_b, FO1_BF16, FO1_EPI_NONE, nullptr, 0, 0, s));
+  FO1_TRY(layer_attention(m, at, b, rows, cs, kc, vc, s, dry));
+  FO1_RUN(linear(b.att, QD, L.o_w, QD, b.x_mid, H, FO1_BF16, rows, H, QD, nullptr, 0, FO1_EPI_NONE, x_in, H, 0, s));
+  FO1_RUN(rmsnorm(b.x_mid, H, L.ln2, b.xn, H, rows, H, c.rms_eps, nk, s));
+  FO1_RUN(linear(b.xn, H, L.gateup_w, H, b.h, Ip, FO1_BF16, rows, 2 * Ip, H, nullptr, 0, FO1_EPI_SILU, nullptr, 0, 1, s));
+  FO1_RUN(linear(b.h, Ip, L.down_w, Ip, x_out, H, FO1_BF16, rows, H, Ip, nullptr, 0, FO1_EPI_NONE, b.x_mid, H, 0, s));
   return FO1_OK;
 }
 
@@ -713,32 +559,19 @@ struct DecodeBufs {
   float *cs_dec, *logits, *mg_ssq, *mg_amax_v;
   int *mg_amax_i, *mg_sync, *samp_tok;
   SampleRowParams* samp;
-  BeamArgs* beam = nullptr;       // DEC_BEAM
-  LookupArgs* lk = nullptr;       // prompt lookup (lookup.cuh)
-};
-
-// a beam-search call: the device state (beam.cuh) and the host table of length-penalty divisors
-struct BeamRun {
-  BeamArgs a;
-  std::vector<float> lp_div;
-};
-
-// a prompt-lookup call: the device state (lookup.cuh) and the caller's descriptor
-struct LookupRun {
-  LookupArgs a;
-  const fo1_lookup_desc* desc;
 };
 
 // the tokens of the current output column into new_tok (scored: also the column's scores), then their recording; every kernel reads
 // the column from *st.step, as the captured decode step does.  `advance`: the column came from a decode step (not the prefill)
-static int decode_column(DecodeMode mode, const DecodeBufs& g, const ColumnSink& k, const fo1_score_desc* sc, int B, int V, int advance,
-                         cudaStream_t s) {
+static int decode_column(const GenerateCall& q, const DecodeBufs& g, int B, int V, int advance, cudaStream_t s) {
+  const ColumnSink& k = q.k;
   const DecodeState& st = k.st;
-  if (mode == DEC_BEAM) return beam_column(*g.beam, g.logits, st, advance, s);
-  if (mode == DEC_SCORED) {
+  const fo1_score_desc* sc = q.sc;
+  if (q.mode == DEC_BEAM) return beam_column(q.beam, g.logits, st, advance, s);
+  if (q.mode == DEC_SCORED) {
     FO1_TRY(score_rows(g.logits, V, B, V, g.samp, st.step, st.new_tok, true, st.finished, k.max_new, sc->logprobs, k.max_new, sc->scores,
                        sc->logits, V, s));
-  } else if (mode == DEC_SAMPLED) {
+  } else if (q.mode == DEC_SAMPLED) {
     FO1_TRY(sample_rows(g.logits, V, B, V, g.samp, st.step, 0, st.new_tok, s));       // the Philox step is read from *st.step
   } else {
     launch_k(argmax_kernel, dim3(B), dim3(1024), 0, s, g.logits, V, st.new_tok);
@@ -750,58 +583,97 @@ static int decode_column(DecodeMode mode, const DecodeBufs& g, const ColumnSink&
   return FO1_OK;
 }
 
-// buffer plan, integer tables and the prefill; then (unless `dry`, the pass that sizes the arena) the decode state and column 0
 // the own rows of sequence b in a shared-prefix prefill (L_b without a group)
 static int prefix_of(const fo1_prefix_desc* px, int b) { return px && px->seq_group[b] >= 0 ? px->prefix_lens[px->seq_group[b]] : 0; }
 
-// host and device tables of a shared-prefix prefill (PrefixTables); n_pre: sum P_g
-static int prefix_tables(Model* m, const fo1_generate_desc* d, const fo1_prefix_desc* px, int n_pre, PrefixTables& p, cudaStream_t s) {
-  const int B = d->n_seqs, G = px->n_groups;
-  p.n_pre = n_pre; p.n_groups = G;
-  std::vector<int> cu(1, 0), row_gt, grp_off(1, 0), members, own_seq, own_t, pre(B), own(B), rowseg, tiles;
-  std::string key = "llmpx:" + std::to_string(m->kv_cap);
+// the prefill's attention plan over T packed rows (b: the layer buffers it reads and writes) and the last packed row of every sequence,
+// from integer tables cached per shape.  The packed rows are one causal segment per sequence, or with a shared prefix the groups' prefix
+// rows (one segment per group) followed by every sequence's own rows.  The cache-write map has one group per sequence with its slot as
+// the member; beam search gives each prompt its N slots; a shared prefix puts the prefix groups with their members first, then one
+// group per sequence for its own rows at positions P_b + i.
+static int prefill_plan(Model* m, const GenerateCall& q, const LayerBuf& b, int T, PrefillAttn& p, const int** d_last, cudaStream_t s) {
+  const fo1_model_config& c = m->cfg;
+  const fo1_generate_desc* d = q.d;
+  const fo1_prefix_desc* px = q.px;
+  const int B = d->n_seqs, G = px ? px->n_groups : 0, N = q.bmd ? q.beam.N : 1;
+  const int hd = c.llm_head_dim, QD = c.llm_heads * hd, KD = c.llm_kv_heads * hd, ldq = QD + 2 * KD;
+  std::vector<int> cu(1, 0), row_gt, grp_off(1, 0), members, last, pre(B), own(B), tiles, rowseg;
+  std::string key = "llm:" + std::to_string(N) + ":" + std::to_string(px ? m->kv_cap : 0);
   for (int g = 0; g < G; ++g) {
     cu.push_back(cu.back() + px->prefix_lens[g]);
     for (int t = 0; t < px->prefix_lens[g]; ++t) { row_gt.push_back(g); row_gt.push_back(t); }
-    for (int b = 0; b < B; ++b) if (px->seq_group[b] == g) members.push_back(b);
+    for (int i = 0; i < B; ++i) if (px->seq_group[i] == g) members.push_back(i);
     grp_off.push_back((int)members.size());
     key += ":" + std::to_string(px->prefix_lens[g]);
   }
-  for (int b = 0; b < B; ++b) {
-    pre[b] = prefix_of(px, b); own[b] = d->seq_lens[b] - pre[b];
-    for (int i = 0; i < own[b]; ++i) { own_seq.push_back(b); own_t.push_back(pre[b] + i); }
-    key += "/" + std::to_string(px->seq_group[b]) + ":" + std::to_string(d->seq_lens[b]);
+  int r = cu.back();
+  for (int i = 0; i < B; ++i) {
+    pre[i] = prefix_of(px, i); own[i] = d->seq_lens[i] - pre[i];
+    for (int t = 0; t < own[i]; ++t) { row_gt.push_back(G + i); row_gt.push_back(pre[i] + t); }
+    for (int j = 0; j < N; ++j) members.push_back(i * N + j);
+    grp_off.push_back((int)members.size());
+    r += own[i];
+    last.push_back(r - 1);
+    if (!px) cu.push_back(r);
+    key += "/" + std::to_string(px ? px->seq_group[i] : -1) + ":" + std::to_string(d->seq_lens[i]);
   }
-  FO1_TRY(cached_ints(m, key + ":cu", cu, &p.cu, s));
-  attention_tile_table(cu, tiles);
-  p.n_tiles = (int)tiles.size() / 2;
-  FO1_TRY(cached_ints(m, key + ":til", tiles, &p.tiles, s));
-  FO1_TRY(cached_ints(m, key + ":gt", row_gt, &p.row_gt, s));
+  const int* gt = nullptr;
+  FO1_TRY(cached_ints(m, key + ":gt", row_gt, &gt, s));
+  p.row_gt = reinterpret_cast<const int2*>(gt);
   FO1_TRY(cached_ints(m, key + ":go", grp_off, &p.grp_off, s));
   FO1_TRY(cached_ints(m, key + ":mem", members, &p.members, s));
-  FO1_TRY(cached_ints(m, key + ":os", own_seq, &p.own_seq, s));
-  FO1_TRY(cached_ints(m, key + ":ot", own_t, &p.own_t, s));
-  prefix_attention_tables(pre.data(), own.data(), B, m->kv_cap, rowseg, tiles);
-  p.n_own_tiles = (int)tiles.size() / 2;
-  FO1_TRY(cached_ints(m, key + ":ors", rowseg, &p.own_rowseg, s));
-  FO1_TRY(cached_ints(m, key + ":otil", tiles, &p.own_tiles, s));
+  FO1_TRY(cached_ints(m, key + ":last", last, d_last, s));
+
+  AttnArgs& a = p.causal;
+  a = AttnArgs();
+  a.q = b.qkv; a.k = b.qkv + QD; a.v = b.qkv + QD + KD; a.o = b.att;
+  a.ldq = a.ldk = a.ldv = ldq; a.ldo = QD;
+  a.n_seqs = (int)cu.size() - 1; a.total_rows = cu.back(); a.max_seqlen = 0; a.rowseg = b.rowseg;
+  for (int i = 0; i < a.n_seqs; ++i) {
+    const int len = cu[i + 1] - cu[i];
+    a.max_seqlen = std::max(a.max_seqlen, len);
+    a.flops += 2.0 * (double)len * len * QD;   // causal: half of 4 L^2 d
+  }
+  a.q_heads = c.llm_heads; a.kv_heads = c.llm_kv_heads; a.head_dim = hd;
+  a.scale = 1.0f / sqrtf((float)hd); a.causal = 1;
+  FO1_TRY(cached_ints(m, key + ":cu", cu, &a.cu_seqlens, s));
+  attention_tile_table(cu, tiles);        // query tiles restart at every segment
+  a.n_tiles = (int)tiles.size() / 2;
+  FO1_TRY(cached_ints(m, key + ":til", tiles, &a.tiles, s));
+
+  AttnArgs& o = p.own;
+  o = a;
+  o.total_rows = 0;
+  if (px) {
+    const int np = a.total_rows;
+    o.q = b.qkv + (size_t)np * ldq; o.o = b.att + (size_t)np * QD;
+    o.ldk = o.ldv = KD;
+    o.cu_seqlens = nullptr; o.n_seqs = m->kv_batch; o.total_rows = T - np; o.max_seqlen = 0; o.flops = 0.0;
+    o.causal = 0; o.kv_rows = m->kv_batch * m->kv_cap;
+    prefix_attention_tables(pre.data(), own.data(), B, m->kv_cap, rowseg, tiles);
+    o.n_tiles = (int)tiles.size() / 2;
+    FO1_TRY(cached_ints(m, key + ":ors", rowseg, &o.rowseg, s));
+    FO1_TRY(cached_ints(m, key + ":otil", tiles, &o.tiles, s));
+  }
   return FO1_OK;
 }
 
-static int llm_prefill(Model* m, fo1_generate_desc* d, const fo1_prefix_desc* px, const fo1_sampling_desc* sp, const fo1_score_desc* sc,
-                       DecodeMode mode, const ColumnSink& k, cudaStream_t s, bool dry, DecodeBufs& g, BeamRun* bm = nullptr,
-                       LookupRun* lk = nullptr) {
+// buffer plan, integer tables and the prefill; then (unless `dry`, the pass that sizes the arena) the decode state and column 0
+static int llm_prefill(Model* m, GenerateCall& q, cudaStream_t s, bool dry, DecodeBufs& g) {
   const fo1_model_config& c = m->cfg;
   Arena& A = m->arena;
+  fo1_generate_desc* d = q.d;
+  const fo1_prefix_desc* px = q.px;
+  const bool beam = q.bmd != nullptr, lookup = q.lkd != nullptr;
   const int B = d->n_seqs, H = c.llm_hidden, hd = c.llm_head_dim, V = c.llm_vocab;
   const int QD = c.llm_heads * hd, KD = c.llm_kv_heads * hd, ldq = QD + 2 * KD;
   const int Ip = (c.llm_inter + 31) / 32 * 32;
   long long T = 0;      // packed rows through the layers: every sequence's rows, or (px) the prefix rows then the own rows
-  int max_len = 0, n_pre = 0;
-  for (int b = 0; b < B; ++b) { T += d->seq_lens[b] - prefix_of(px, b); max_len = std::max(max_len, d->seq_lens[b]); }
+  int n_pre = 0;
+  for (int b = 0; b < B; ++b) T += d->seq_lens[b] - prefix_of(px, b);
   for (int gi = 0; px && gi < px->n_groups; ++gi) n_pre += px->prefix_lens[gi];
   T += n_pre;
-  const int RD = bm ? B * bm->a.N : lk ? B * (lk->a.K + 1) : B;   // rows of a decode step: one per sequence, beam or verify row
+  const int RD = beam ? B * q.beam.N : lookup ? B * (q.lookup.K + 1) : B;   // rows of a decode step: one per sequence, beam or verify row
   const int R = (int)std::max<long long>(T, RD);
 
   g = DecodeBufs();
@@ -817,7 +689,6 @@ static int llm_prefill(Model* m, fo1_generate_desc* d, const fo1_prefix_desc* px
   g.cs_dec = A.alloc<float>((size_t)RD * hd);
   buf.dec_part = A.alloc<float>((size_t)RD * c.llm_heads * kDecSplits * (128 + 4));
   buf.rowseg = A.alloc<int>((size_t)R * 2);
-  for (int b = 0; b < B; ++b) buf.attn_flops += 2.0 * (double)d->seq_lens[b] * d->seq_lens[b] * QD;   // causal: half of 4 L^2 d
   bf16* last = A.alloc<bf16>((size_t)B * H);
   g.lastn = A.alloc<bf16>((size_t)RD * H);
   g.logits = A.alloc<float>((size_t)RD * V);
@@ -830,78 +701,35 @@ static int llm_prefill(Model* m, fo1_generate_desc* d, const fo1_prefix_desc* px
   // FO1_MEGA_MAX_B lowers the threshold, FO1_NO_MEGA disables the kernel.
   int mega_max_b = 32;
   if (const char* e = getenv("FO1_MEGA_MAX_B")) mega_max_b = std::max(0, std::min(32, atoi(e)));
-  g.mega_grid = (m->llm.mega_ok && !bm && !lk && B <= mega_max_b && getenv("FO1_NO_MEGA") == nullptr) ? decode_mega_grid() : 0;
+  g.mega_grid = (m->llm.mega_ok && !beam && !lookup && B <= mega_max_b && getenv("FO1_NO_MEGA") == nullptr) ? decode_mega_grid() : 0;
   g.mg_ssq = A.alloc<float>((size_t)2 * std::max(g.mega_grid, 1) * 32);
   g.mg_amax_v = A.alloc<float>((size_t)std::max(g.mega_grid, 1) * 32);
   g.mg_amax_i = A.alloc<int>((size_t)std::max(g.mega_grid, 1) * 32);
   g.mg_sync = A.alloc<int>((size_t)B * c.llm_kv_heads + 8);
   // sampled or scored decoding: the per-sequence parameters and the tokens the persistent kernel's CTA b drew
-  g.samp = mode == DEC_SAMPLED || mode == DEC_SCORED ? A.alloc<SampleRowParams>(B) : nullptr;
-  g.samp_tok = mode == DEC_SAMPLED || mode == DEC_SCORED ? A.alloc<int>(B) : nullptr;
-  if (bm) {   // beam search: its state and scratch (sized by the dry run like everything else)
-    beam_alloc(A, bm->a);
-    g.beam = &bm->a;
-  }
-  if (lk) {
-    lookup_alloc(A, lk->a, lk->desc);
-    g.lk = &lk->a;
-  }
+  g.samp = q.mode == DEC_SAMPLED || q.mode == DEC_SCORED ? A.alloc<SampleRowParams>(B) : nullptr;
+  g.samp_tok = q.mode == DEC_SAMPLED || q.mode == DEC_SCORED ? A.alloc<int>(B) : nullptr;
+  if (beam) beam_alloc(A, q.beam);   // beam search: its state and scratch (sized by the dry run like everything else)
+  if (lookup) lookup_alloc(A, q.lookup, q.lkd);
 
-  // ---- integer tables of the packed batch ----
-  const int *d_cu = nullptr, *d_row_seq = nullptr, *d_row_t = nullptr, *d_last = nullptr;
-  PrefixTables ptab;
-  if (!dry && px) {
-    FO1_TRY(prefix_tables(m, d, px, n_pre, ptab, s));
-    std::vector<int> lastrow;
-    int r = n_pre;
-    std::string key = "llmpx";
-    for (int b = 0; b < B; ++b) { r += d->seq_lens[b] - prefix_of(px, b); lastrow.push_back(r - 1); key += ":" + std::to_string(r); }
-    FO1_TRY(cached_ints(m, key + ":last", lastrow, &d_last, s));
-  }
-  if (px) buf.px = &ptab;
+  // ---- integer tables and inputs ----
+  PrefillAttn pa = {};
+  const int* d_last = nullptr;
   if (!dry) {
-    std::vector<int> cu(1, 0), row_seq, row_t, lastrow;
-    std::string key = "llm";
-    for (int b = 0; b < B && !px; ++b) {
-      for (int t = 0; t < d->seq_lens[b]; ++t) { row_seq.push_back(b); row_t.push_back(t); }
-      cu.push_back(cu.back() + d->seq_lens[b]);
-      lastrow.push_back(cu.back() - 1);
-      key += ":" + std::to_string(d->seq_lens[b]);
-    }
-    if (!px && bm) {     // prompt b's rows go to its N cache slots b * N .. b * N + N - 1 (kv_fanout_kernel)
-      const int N = bm->a.N;
-      std::vector<int> gt, off, mem;
-      for (int r = 0; r < (int)row_seq.size(); ++r) { gt.push_back(row_seq[r]); gt.push_back(row_t[r]); }
-      for (int b = 0; b <= B; ++b) off.push_back(b * N);
-      for (int r = 0; r < B * N; ++r) mem.push_back(r);
-      const std::string bk = key + ":beam" + std::to_string(N);
-      FO1_TRY(cached_ints(m, bk + ":gt", gt, &buf.fan_gt, s));
-      FO1_TRY(cached_ints(m, bk + ":off", off, &buf.fan_off, s));
-      FO1_TRY(cached_ints(m, bk + ":mem", mem, &buf.fan_mem, s));
-    }
-    if (!px) {
-      FO1_TRY(cached_ints(m, key + ":cu", cu, &d_cu, s));
-      FO1_TRY(cached_ints(m, key + ":rs", row_seq, &d_row_seq, s));
-      FO1_TRY(cached_ints(m, key + ":rt", row_t, &d_row_t, s));
-      FO1_TRY(cached_ints(m, key + ":last", lastrow, &d_last, s));
-      std::vector<int> tiles;
-      attention_tile_table(cu, tiles);        // query tiles restart at every prompt
-      FO1_TRY(cached_ints(m, key + ":til", tiles, &buf.tiles, s));
-      buf.n_tiles = (int)tiles.size() / 2;
-    }
+    FO1_TRY(prefill_plan(m, q, buf, (int)T, pa, &d_last, s));
     FO1_CUDA(cudaMemcpyAsync(d_lens, d->seq_lens, B * sizeof(int), cudaMemcpyHostToDevice, s));
     if (d->rope_deltas_device != nullptr) FO1_CUDA(cudaMemcpyAsync(d_deltas, d->rope_deltas_device, B * sizeof(int), cudaMemcpyDeviceToDevice, s));
     else FO1_CUDA(cudaMemcpyAsync(d_deltas, d->rope_deltas, B * sizeof(int), cudaMemcpyHostToDevice, s));
-    if (d->n_stop_ids > 0) FO1_CUDA(cudaMemcpyAsync(k.st.stop_ids, d->stop_ids, d->n_stop_ids * sizeof(int), cudaMemcpyHostToDevice, s));
-    if (bm) {
-      FO1_CUDA(cudaMemcpyAsync(const_cast<int*>(bm->a.prompt_len), d->seq_lens, B * sizeof(int), cudaMemcpyHostToDevice, s));
-      FO1_CUDA(cudaMemcpyAsync(const_cast<float*>(bm->a.lp_div), bm->lp_div.data(), bm->lp_div.size() * sizeof(float), cudaMemcpyHostToDevice, s));
+    if (d->n_stop_ids > 0) FO1_CUDA(cudaMemcpyAsync(q.k.st.stop_ids, d->stop_ids, d->n_stop_ids * sizeof(int), cudaMemcpyHostToDevice, s));
+    if (beam) {
+      FO1_CUDA(cudaMemcpyAsync(const_cast<int*>(q.beam.prompt_len), d->seq_lens, B * sizeof(int), cudaMemcpyHostToDevice, s));
+      FO1_CUDA(cudaMemcpyAsync(const_cast<float*>(q.beam.lp_div), q.lp_div.data(), q.lp_div.size() * sizeof(float), cudaMemcpyHostToDevice, s));
     }
-    if (lk) FO1_TRY(lookup_upload(lk->a, lk->desc, s));
-    if (mode == DEC_SAMPLED || mode == DEC_SCORED) {
+    if (lookup) FO1_TRY(lookup_upload(q.lookup, q.lkd, s));
+    if (q.mode == DEC_SAMPLED || q.mode == DEC_SCORED) {
       // a scored greedy call samples with top_k 1 (bit-identical to greedy) so that both paths score in the sampler's per-row pass
       std::vector<SampleRowParams> h(B);
-      for (int b = 0; b < B; ++b) h[b] = score_row_params(sp, sc ? sc->raw_rows : nullptr, b);
+      for (int b = 0; b < B; ++b) h[b] = score_row_params(q.sp, q.sc ? q.sc->raw_rows : nullptr, b);
       FO1_CUDA(cudaMemcpyAsync(g.samp, h.data(), B * sizeof(SampleRowParams), cudaMemcpyHostToDevice, s));
     }
   }
@@ -909,9 +737,9 @@ static int llm_prefill(Model* m, fo1_generate_desc* d, const fo1_prefix_desc* px
   // ---- prefill ----
   const bf16* x = static_cast<const bf16*>(d->inputs_embeds);
   const int* pos = d->position_ids;
-  if (px) {   // one packed matrix (prefix rows, then own rows) and one position table; rowseg of the prefix segments
+  FO1_RUN(attention_rowseg(pa.causal.cu_seqlens, pa.causal.n_seqs, pa.causal.total_rows, buf.rowseg, s));
+  if (px) {   // one packed matrix (prefix rows, then own rows) and one position table
     const size_t no = (size_t)T - n_pre;
-    FO1_RUN(attention_rowseg(ptab.cu, px->n_groups, n_pre, buf.rowseg, s));
     if (!dry) {
       FO1_CUDA(cudaMemcpyAsync(g.xb, px->prefix_embeds, (size_t)n_pre * H * sizeof(bf16), cudaMemcpyDeviceToDevice, s));
       FO1_CUDA(cudaMemcpyAsync(g.xb + (size_t)n_pre * H, d->inputs_embeds, no * H * sizeof(bf16), cudaMemcpyDeviceToDevice, s));
@@ -926,13 +754,11 @@ static int llm_prefill(Model* m, fo1_generate_desc* d, const fo1_prefix_desc* px
     }
     x = g.xb;
     pos = pos_all;
-  } else {
-    FO1_RUN(attention_rowseg(d_cu, B, (int)T, buf.rowseg, s));
   }
   FO1_RUN(mrope_table(pos, cs_pre, (int)T, hd, c.mrope_section[0], c.mrope_section[1], c.mrope_section[2], c.rope_theta, s));
   for (int li = 0; li < c.llm_layers; ++li) {
     bf16* xo = (li & 1) ? g.xb : g.xa;
-    FO1_TRY(llm_layer(m, li, x, xo, buf, (int)T, cs_pre, true, d_cu, B, max_len, d_row_seq, d_row_t, nullptr, s, dry));
+    FO1_TRY(llm_layer(m, li, x, xo, buf, (int)T, cs_pre, pa, s, dry));
     x = xo;
   }
   if (d->all_logits) {
@@ -947,20 +773,20 @@ static int llm_prefill(Model* m, fo1_generate_desc* d, const fo1_prefix_desc* px
   }
   if (dry) return FO1_OK;
   if (d->prefill_logits) FO1_CUDA(cudaMemcpyAsync(d->prefill_logits, g.logits, (size_t)B * V * sizeof(float), cudaMemcpyDeviceToDevice, s));
-  if (bm) {
-    FO1_TRY(beam_init(bm->a, k.st, d_lens, d_deltas, s));
+  if (beam) {
+    FO1_TRY(beam_init(q.beam, q.k.st, d_lens, d_deltas, s));
   } else {
-    decode_init_kernel<<<ceil_div(B, 128), 128, 0, s>>>(k.st, d_lens, d_deltas, B);
+    decode_init_kernel<<<ceil_div(B, 128), 128, 0, s>>>(q.k.st, d_lens, d_deltas, B);
     FO1_LAUNCH_CHECK();
   }
   if (d->max_new_tokens <= 0) return FO1_OK;
-  return decode_column(mode, g, k, sc, B, V, 0, s);
+  return decode_column(q, g, B, V, 0, s);
 }
 
 // the rest of the decode loop as ONE cooperative launch of the persistent kernel
-static int decode_persistent(Model* m, fo1_generate_desc* d, const fo1_score_desc* sc, DecodeMode mode, const ColumnSink& k,
-                             const DecodeBufs& g, cudaStream_t s) {
+static int decode_persistent(Model* m, const GenerateCall& q, const DecodeBufs& g, cudaStream_t s) {
   const fo1_model_config& c = m->cfg;
+  fo1_generate_desc* d = q.d;
   const int B = d->n_seqs;
   MegaArgs a;
   memset(&a, 0, sizeof(a));
@@ -972,71 +798,70 @@ static int decode_persistent(Model* m, fo1_generate_desc* d, const fo1_score_des
   a.kc = static_cast<bf16*>(m->kv_cache); a.vc = a.kc + (size_t)c.llm_layers * a.kv_layer_stride; a.cap = m->kv_cap;
   a.x = g.xa; a.x_mid = g.layer.x_mid; a.qkv = g.layer.qkv; a.att = g.layer.att; a.h = g.layer.h;
   a.ssq = g.mg_ssq; a.cs = g.cs_dec; a.att_part = g.layer.dec_part; a.att_count = g.mg_sync + 8;
-  a.amax_val = g.mg_amax_v; a.amax_idx = g.mg_amax_i; a.sink = k;
+  a.amax_val = g.mg_amax_v; a.amax_idx = g.mg_amax_i; a.sink = q.k;
   a.logits = g.logits; a.samp = g.samp; a.samp_tok = g.samp_tok;
-  if (sc) { a.sc_logprobs = sc->logprobs; a.sc_scores = sc->scores; a.sc_logits = sc->logits; }
+  if (q.sc) { a.sc_logprobs = q.sc->logprobs; a.sc_scores = q.sc->scores; a.sc_logits = q.sc->logits; }
   a.n_steps = d->max_new_tokens - 1; a.bar = reinterpret_cast<unsigned*>(g.mg_sync);
   const int pairs = B * c.llm_kv_heads;
   a.n_splits = std::max(1, std::min(kMgMaxSplits, g.mega_grid / std::max(1, pairs)));
   FO1_CUDA(cudaMemsetAsync(g.mg_sync, 0, ((size_t)pairs + 8) * sizeof(int), s));
-  FO1_TRY(decode_mega_run(a, mode, s));
+  FO1_TRY(decode_mega_run(a, q.mode, s));
   m->last_decode_path = 1;
   d->steps_run = d->max_new_tokens - 1;
   return FO1_OK;
 }
 
+// one decode forward over R rows: the embedding of tok, the M-RoPE table of pos3 ([3][R]), the layers with attention `at`, the final
+// norm and the LM head into g.logits
+static int decode_forward(Model* m, const DecodeBufs& g, const int* tok, const int* pos3, int R, const DecodeAttn& at, cudaStream_t s) {
+  const fo1_model_config& c = m->cfg;
+  const int H = c.llm_hidden, V = c.llm_vocab;
+  launch_k(embed_tokens_kernel, dim3(R), dim3(256), 0, s, tok, m->llm.embed, g.xa, H);
+  FO1_LAUNCH_CHECK();
+  FO1_TRY(mrope_table(pos3, g.cs_dec, R, c.llm_head_dim, c.mrope_section[0], c.mrope_section[1], c.mrope_section[2], c.rope_theta, s));
+  const bf16* xin = g.xa;
+  for (int li = 0; li < c.llm_layers; ++li) {
+    bf16* xo = (li & 1) ? g.xa : g.xb;
+    FO1_TRY(llm_layer(m, li, xin, xo, g.layer, R, g.cs_dec, at, s, false));
+    xin = xo;
+  }
+  FO1_TRY(rmsnorm(xin, H, m->llm.norm, g.lastn, H, R, H, c.rms_eps, seq_norm_kernel(H), s));
+  return linear(g.lastn, H, m->llm.lm_head, H, g.logits, V, FO1_F32, R, V, H, nullptr, 0, FO1_EPI_NONE, nullptr, 0, 0, s);
+}
+
 // the rest of the decode loop, per kernel: every step is the SAME launch sequence reading its state from device memory; the first step
 // runs eagerly (warms every kernel), the second is captured into a CUDA graph that is replayed afterwards
-static int decode_per_kernel(Model* m, fo1_generate_desc* d, const fo1_score_desc* sc, DecodeMode mode, const ColumnSink& k,
-                             const DecodeBufs& g, const int32_t* h_progress, cudaStream_t s) {
+static int decode_per_kernel(Model* m, const GenerateCall& q, const DecodeBufs& g, cudaStream_t s) {
   const fo1_model_config& c = m->cfg;
-  const int B = g.beam ? g.beam->S * g.beam->N : d->n_seqs, H = c.llm_hidden, hd = c.llm_head_dim, V = c.llm_vocab;
+  fo1_generate_desc* d = q.d;
+  const ColumnSink& k = q.k;
+  const bool lookup = q.lkd != nullptr;
+  const int B = q.bmd ? q.beam.S * q.beam.N : d->n_seqs, V = c.llm_vocab;
   LlmState* ls = static_cast<LlmState*>(m->llm_state);
-  const int R = g.lk ? B * (g.lk->K + 1) : B;     // rows of a step
+  const int R = lookup ? B * (q.lookup.K + 1) : B;     // rows of a step
+  const int32_t* h_progress = q.stm ? q.stm->progress : nullptr;
   // programmatic dependent launch: each kernel of the step starts (prologue, weight prefetch) while its predecessor drains
   const bool use_pdl = getenv("FO1_NO_PDL") == nullptr;
   auto enqueue_step = [&]() -> int {
     PdlScope pdl(use_pdl);
     SplitKScope sk(true);       // M = number of sequences in every GEMM of a decode step
-    launch_k(embed_tokens_kernel, dim3(B), dim3(256), 0, s, k.st.cur_tok, m->llm.embed, g.xa, H);
-    FO1_LAUNCH_CHECK();
-    FO1_TRY(mrope_table(k.st.pos3, g.cs_dec, B, hd, c.mrope_section[0], c.mrope_section[1], c.mrope_section[2], c.rope_theta, s));
-    const bf16* xin = g.xa;
-    for (int li = 0; li < c.llm_layers; ++li) {
-      bf16* xo = (li & 1) ? g.xa : g.xb;
-      FO1_TRY(llm_layer(m, li, xin, xo, g.layer, B, g.cs_dec, false, nullptr, B, 0, nullptr, nullptr, &k.st, s, false));
-      xin = xo;
-    }
-    FO1_TRY(rmsnorm(xin, H, m->llm.norm, g.lastn, H, B, H, c.rms_eps, seq_norm_kernel(H), s));
-    FO1_TRY(linear(g.lastn, H, m->llm.lm_head, H, g.logits, V, FO1_F32, B, V, H, nullptr, 0, FO1_EPI_NONE, nullptr, 0, 0, s));
-    return decode_column(mode, g, k, sc, B, V, 1, s);
+    FO1_TRY(decode_forward(m, g, k.st.cur_tok, k.st.pos3, B, DecodeAttn{k.st.cache_len, nullptr, B}, s));
+    return decode_column(q, g, B, V, 1, s);
   };
   // prompt lookup: drafts, then ONE verify step over R = B * (K + 1) rows, each computing the plain step's bits for its position
   // (block norms, GEMMs with the M = B choice, the K/V append and attention through the row map), then the acceptance
   auto enqueue_verify = [&]() -> int {
-    const LookupArgs& a = *g.lk;
+    const LookupArgs& a = q.lookup;
     PdlScope pdl(use_pdl);
     SplitKScope sk(true);
     GemmChoiceScope gc(B);
     FO1_TRY(lookup_drafts(a.corpus, a.ld, a.corpus_len, B, a.K, a.max_ngram, k.st.stop_ids, k.n_stop, a.col, k.max_new, a.drafts, a.n_draft, s));
     FO1_TRY(lookup_rows(a, k.st, s));
-    launch_k(embed_tokens_kernel, dim3(R), dim3(256), 0, s, (const int*)a.row_tok, m->llm.embed, g.xa, H);
-    FO1_LAUNCH_CHECK();
-    FO1_TRY(mrope_table(a.row_pos, g.cs_dec, R, hd, c.mrope_section[0], c.mrope_section[1], c.mrope_section[2], c.rope_theta, s));
-    LayerBuf lb = g.layer;
-    lb.row_slot = a.row_slot; lb.row_idx = a.row_idx; lb.n_seqs = B;
-    const bf16* xin = g.xa;
-    for (int li = 0; li < c.llm_layers; ++li) {
-      bf16* xo = (li & 1) ? g.xa : g.xb;
-      FO1_TRY(llm_layer(m, li, xin, xo, lb, R, g.cs_dec, false, nullptr, B, 0, nullptr, nullptr, &k.st, s, false));
-      xin = xo;
-    }
-    FO1_TRY(rmsnorm(xin, H, m->llm.norm, g.lastn, H, R, H, c.rms_eps, seq_norm_kernel(H), s));
-    FO1_TRY(linear(g.lastn, H, m->llm.lm_head, H, g.logits, V, FO1_F32, R, V, H, nullptr, 0, FO1_EPI_NONE, nullptr, 0, 0, s));
-    if (mode == DEC_SCORED) {
-      FO1_TRY(score_rows_lookup(g.logits, V, R, a.K + 1, V, g.samp, a.row_col, a.row_out, a.row_lp, k.st.finished, k.max_new, B, sc->scores,
-                                sc->logits, s));
-    } else if (mode == DEC_SAMPLED) {
+    FO1_TRY(decode_forward(m, g, a.row_tok, a.row_pos, R, DecodeAttn{a.row_idx, a.row_slot, B}, s));
+    if (q.mode == DEC_SCORED) {
+      FO1_TRY(score_rows_lookup(g.logits, V, R, a.K + 1, V, g.samp, a.row_col, a.row_out, a.row_lp, k.st.finished, k.max_new, B, q.sc->scores,
+                                q.sc->logits, s));
+    } else if (q.mode == DEC_SAMPLED) {
       FO1_TRY(sample_rows(g.logits, V, R, V, a.row_prm, a.row_col, 1, a.row_out, s));   // each row's Philox step is its own column
     } else {
       launch_k(argmax_kernel, dim3(R), dim3(1024), 0, s, (const float*)g.logits, V, a.row_out);
@@ -1044,19 +869,19 @@ static int decode_per_kernel(Model* m, fo1_generate_desc* d, const fo1_score_des
     }
     return lookup_accept(a, k, s);
   };
-  auto enqueue = [&]() -> int { return g.lk ? enqueue_verify() : enqueue_step(); };
+  auto enqueue = [&]() -> int { return lookup ? enqueue_verify() : enqueue_step(); };
   cudaGraphExec_t gexec = nullptr;
   m->last_decode_path = 0;
   const bool want_graph = !g_prof_on && d->max_new_tokens > 3 && getenv("FO1_NO_GRAPH") == nullptr;
   d->steps_run = 0;
   int rc = FO1_OK;
   cudaEvent_t poll_ev[2] = {nullptr, nullptr};
-  if (g.lk != nullptr && d->early_exit_interval > 0)
+  if (lookup && d->early_exit_interval > 0)
     for (cudaEvent_t& e : poll_ev) FO1_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
   for (int step = 1; step < d->max_new_tokens; ++step) {
     if (gexec != nullptr) {
       if (cudaGraphLaunch(gexec, s) != cudaSuccess) { set_error("cudaGraphLaunch failed: %s", cudaGetErrorString(cudaGetLastError())); rc = FO1_ERR_CUDA; break; }
-      count_launch((uint64_t)c.llm_layers * 9 + (g.lk ? 8 : 6));
+      count_launch((uint64_t)c.llm_layers * 9 + (lookup ? 8 : 6));
     } else if (want_graph && step == 2) {
       cudaGraph_t graph = nullptr;
       if (cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
@@ -1084,7 +909,7 @@ static int decode_per_kernel(Model* m, fo1_generate_desc* d, const fo1_score_des
     // prompt lookup: sequences end after a varying number of steps, so the loop polls after every step, one step behind: it waits for
     // the previous step's n_active while this step runs, so the device never waits for the host and at most one step runs past the
     // end of the last sequence
-    if (g.lk != nullptr && d->early_exit_interval > 0) {
+    if (lookup && d->early_exit_interval > 0) {
       const int slot = step & 1;
       if (cudaMemcpyAsync(ls->h_flag + slot, k.st.n_active, sizeof(int), cudaMemcpyDeviceToHost, s) != cudaSuccess ||
           cudaEventRecord(poll_ev[slot], s) != cudaSuccess) {
@@ -1169,7 +994,9 @@ int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, co
     FO1_CHECK_ARG(d->seq_lens[b] > 0, "fo1_llm_generate: sequence %d is empty", b);
     max_len = std::max(max_len, d->seq_lens[b]);
   }
-  ColumnSink k = {};
+  GenerateCall q{};
+  q.d = d; q.px = px; q.sp = sp; q.sc = sc; q.stm = stm; q.bmd = bmd; q.lkd = lkd;
+  ColumnSink& k = q.k;
   if (stm) {
     FO1_TRY(stream_resolve(stm, &k.stream));
     __atomic_store_n(stm->progress, d->max_new_tokens > 0 ? 0 : FO1_STREAM_DONE, __ATOMIC_RELEASE);   // before anything is enqueued
@@ -1178,18 +1005,15 @@ int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, co
   FO1_TRY(ensure_state(m, rows, d->n_stop_ids, &k.st));
   k.n_stop = d->n_stop_ids; k.pad_id = d->pad_id; k.max_new = d->max_new_tokens;
   k.out_tokens = d->out_tokens; k.out_lens = d->out_lens;
-  const DecodeMode mode = bmd ? DEC_BEAM : sc ? DEC_SCORED : sp ? DEC_SAMPLED : DEC_GREEDY;
+  q.mode = bmd ? DEC_BEAM : sc ? DEC_SCORED : sp ? DEC_SAMPLED : DEC_GREEDY;
   // a shared-prefix call rounds the slot up to 64 rows: the cache-reading attention's last key tile stays inside the slot; a lookup
   // call's verify rows write up to K rows past the sequence's last position
   const int n_drafts = lkd ? std::min(lkd->num_tokens, kLookupMaxDrafts) : 0;
   const int cap = max_len + std::max(d->max_new_tokens, 1) + n_drafts;
   FO1_TRY(ensure_kv(m, rows, px ? (cap + 63) / 64 * 64 : cap));
   FO1_TRY(int_cache_trim(m));
-  BeamRun brun;
-  BeamRun* bm = nullptr;
   if (bmd) {
-    BeamArgs& a = brun.a;
-    memset(&a, 0, sizeof(a));
+    BeamArgs& a = q.beam;
     a.S = d->n_seqs; a.N = bmd->num_beams; a.K = bmd->n_keep; a.V = c.llm_vocab; a.max_new = d->max_new_tokens;
     a.num_return = bmd->num_return; a.early_stopping = bmd->early_stopping; a.lp_positive = bmd->length_penalty > 0.0 ? 1 : 0;
     a.n_stop = d->n_stop_ids; a.pad_id = d->pad_id; a.stop_ids = k.st.stop_ids;
@@ -1199,40 +1023,34 @@ int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, co
     a.steps_run = bmd->steps_run; a.out_tokens = d->out_tokens; a.out_lens = d->out_lens; a.beam_indices = bmd->beam_indices;
     a.seq_scores = bmd->sequence_scores; a.out_logprobs = bmd->logprobs; a.scores = bmd->scores; a.logits = bmd->logits;
     // HF divides by (len ** length_penalty), a Python float that torch rounds to fp32
-    for (int i = 0; i <= a.max_new; ++i) brun.lp_div.push_back((float)std::pow((double)i, bmd->length_penalty));
-    bm = &brun;
+    for (int i = 0; i <= a.max_new; ++i) q.lp_div.push_back((float)std::pow((double)i, bmd->length_penalty));
   }
-  LookupRun lrun;
-  LookupRun* lk = nullptr;
   if (lkd) {
-    LookupArgs& a = lrun.a;
-    memset(&a, 0, sizeof(a));
+    LookupArgs& a = q.lookup;
     a.B = d->n_seqs; a.K = n_drafts; a.max_ngram = lkd->max_ngram; a.max_new = d->max_new_tokens;
     int longest = 0;
     for (int b = 0; b < d->n_seqs; ++b) longest = std::max(longest, lkd->corpus_offsets[b + 1] - lkd->corpus_offsets[b]);
     a.ld = (long long)longest + std::max(d->max_new_tokens, 1);
     a.logprobs = sc ? sc->logprobs : nullptr;
-    lrun.desc = lkd;
-    lk = &lrun;
   }
   m->arena.reset(true);
   DecodeBufs g;
-  FO1_TRY(llm_prefill(m, d, px, sp, sc, mode, k, s, true, g, bm, lk));
+  FO1_TRY(llm_prefill(m, q, s, true, g));
   FO1_TRY(arena_ensure(m, m->arena.peak));
   m->arena.reset(false);
-  if (d->max_new_tokens > 0 && !bm) {  // out_tokens pre-filled with pad so an early exit leaves a clean tail
+  if (d->max_new_tokens > 0 && !bmd) {  // out_tokens pre-filled with pad so an early exit leaves a clean tail
     const long long n = (long long)d->n_seqs * d->max_new_tokens;
     fill_int_kernel<<<(int)std::min<long long>((n + 255) / 256, 1024), 256, 0, s>>>(d->out_tokens, d->pad_id, n);
     FO1_LAUNCH_CHECK();
     FO1_CUDA(cudaMemsetAsync(d->out_lens, 0, d->n_seqs * sizeof(int), s));
     if (sc && sc->logprobs) FO1_CUDA(cudaMemsetAsync(sc->logprobs, 0, (size_t)n * sizeof(float), s));      // 0 past out_lens
   }
-  FO1_TRY(llm_prefill(m, d, px, sp, sc, mode, k, s, false, g, bm, lk));
+  FO1_TRY(llm_prefill(m, q, s, false, g));
   if (d->max_new_tokens <= 0) return FO1_OK;
-  if (lk) FO1_TRY(lookup_init(lk->a, k.st, g.samp, s));
-  if (g.mega_grid > 0 && d->max_new_tokens > 1) return decode_persistent(m, d, sc, mode, k, g, s);
-  FO1_TRY(decode_per_kernel(m, d, sc, mode, k, g, stm ? stm->progress : nullptr, s));
-  return bm ? beam_finalize(bm->a, s) : FO1_OK;
+  if (lkd) FO1_TRY(lookup_init(q.lookup, k.st, g.samp, s));
+  if (g.mega_grid > 0 && d->max_new_tokens > 1) return decode_persistent(m, q, g, s);
+  FO1_TRY(decode_per_kernel(m, q, g, s));
+  return bmd ? beam_finalize(q.beam, s) : FO1_OK;
 }
 
 // -------------------------------------------------------------------------------- splice plan (host, integer)
@@ -1412,6 +1230,6 @@ extern "C" int fo1_decode_attention(const fo1_decode_attn_desc* d, void* stream)
   const size_t need = fo1_decode_attention_workspace_bytes(d->n_seqs, d->q_heads);
   if (d->workspace == nullptr || d->workspace_bytes < need) { set_error("fo1_decode_attention: workspace %zu B < required %zu B", d->workspace_bytes, need); return FO1_ERR_WORKSPACE; }
   return decode_attention(static_cast<const bf16*>(d->q), d->ldq, static_cast<const bf16*>(d->k_cache), static_cast<const bf16*>(d->v_cache), d->cache_len,
-                          d->n_seqs, d->cap, d->q_heads, d->kv_heads, d->head_dim, d->scale, static_cast<bf16*>(d->out), d->ldo,
+                          nullptr, d->n_seqs, d->n_seqs, d->cap, d->q_heads, d->kv_heads, d->head_dim, d->scale, static_cast<bf16*>(d->out), d->ldo,
                           static_cast<float*>(d->workspace), static_cast<cudaStream_t>(stream));
 }

@@ -19,6 +19,25 @@ __global__ void vit_rope_table_kernel(const int* __restrict__ pos_hw, float* __r
   cs[(long long)T * half + i] = sinf(ang);
 }
 
+// rotate the pair (p[j], p[j + half]) of the 8 consecutive j of chunk c by row t's angles (rotate_half convention) into (ra, rb)
+__device__ __forceinline__ void rope_rotate8(const bf16* p, int half, const float* __restrict__ cs, int T, int t, int c, uint4& ra, uint4& rb) {
+  const uint4 a = *reinterpret_cast<const uint4*>(p), b = *reinterpret_cast<const uint4*>(p + half);
+  const float4* cp = reinterpret_cast<const float4*>(cs + (long long)t * half + c * 8);
+  const float4* sp = reinterpret_cast<const float4*>(cs + (long long)T * half + (long long)t * half + c * 8);
+  const float4 c0 = cp[0], c1 = cp[1], s0 = sp[0], s1 = sp[1];
+  const float co[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w}, si[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
+  const uint32_t au[4] = {a.x, a.y, a.z, a.w}, bu[4] = {b.x, b.y, b.z, b.w};
+  uint32_t oa[4], ob[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const float x1l = bf16_lo(au[k]), x1h = bf16_hi(au[k]), x2l = bf16_lo(bu[k]), x2h = bf16_hi(bu[k]);
+    oa[k] = pack_bf16(x1l * co[2 * k] - x2l * si[2 * k], x1h * co[2 * k + 1] - x2h * si[2 * k + 1]);
+    ob[k] = pack_bf16(x2l * co[2 * k] + x1l * si[2 * k], x2h * co[2 * k + 1] + x1h * si[2 * k + 1]);
+  }
+  ra = make_uint4(oa[0], oa[1], oa[2], oa[3]);
+  rb = make_uint4(ob[0], ob[1], ob[2], ob[3]);
+}
+
 // x: rows of pitch ld holding n_heads consecutive heads of hd dims (q heads then k heads); rotates the pair
 // (x[j], x[j + hd/2]) by angle[j] (rotate_half convention).  One thread = 8 consecutive j: 16-byte loads/stores.
 __global__ void __launch_bounds__(256) rope_apply_kernel(bf16* __restrict__ x, long long ld, const float* __restrict__ cs, int T,
@@ -31,30 +50,22 @@ __global__ void __launch_bounds__(256) rope_apply_kernel(bf16* __restrict__ x, l
     const int h = (int)(r % n_heads);
     const int t = (int)(r / n_heads);
     bf16* p = x + (long long)t * ld + (long long)h * hd + c * 8;
-    const uint4 a = *reinterpret_cast<const uint4*>(p), b = *reinterpret_cast<const uint4*>(p + half);
-    const float4* cp = reinterpret_cast<const float4*>(cs + (long long)t * half + c * 8);
-    const float4* sp = reinterpret_cast<const float4*>(cs + (long long)T * half + (long long)t * half + c * 8);
-    const float4 c0 = cp[0], c1 = cp[1], s0 = sp[0], s1 = sp[1];
-    const float co[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w}, si[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
-    const uint32_t au[4] = {a.x, a.y, a.z, a.w}, bu[4] = {b.x, b.y, b.z, b.w};
-    uint32_t oa[4], ob[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float x1l = bf16_lo(au[k]), x1h = bf16_hi(au[k]), x2l = bf16_lo(bu[k]), x2h = bf16_hi(bu[k]);
-      oa[k] = pack_bf16(x1l * co[2 * k] - x2l * si[2 * k], x1h * co[2 * k + 1] - x2h * si[2 * k + 1]);
-      ob[k] = pack_bf16(x2l * co[2 * k] + x1l * si[2 * k], x2h * co[2 * k + 1] + x1h * si[2 * k + 1]);
-    }
-    *reinterpret_cast<uint4*>(p) = make_uint4(oa[0], oa[1], oa[2], oa[3]);
-    *reinterpret_cast<uint4*>(p + half) = make_uint4(ob[0], ob[1], ob[2], ob[3]);
+    uint4 ra, rb;
+    rope_rotate8(p, half, cs, T, t, c, ra, rb);
+    *reinterpret_cast<uint4*>(p) = ra;
+    *reinterpret_cast<uint4*>(p + half) = rb;
   }
 }
 
-// decode step: the same rotation over the q and k heads of row b, with the rotated K head and the V row appended to
-// the cache at index cache_len[b] in the same pass (one launch instead of rope + append)
-// row t's K/V goes to index idx[t] of cache slot slot[t] (slot == nullptr: slot t)
-__device__ __forceinline__ void rope_kv_append_rows(bf16* __restrict__ x, long long ld, const float* __restrict__ cs, int T, int q_heads,
-                                                    int kv_heads, int hd, const int* __restrict__ slot, const int* __restrict__ idx,
-                                                    bf16* __restrict__ kc, bf16* __restrict__ vc, int cap) {
+// decode step: the same rotation over the q and k heads of row t, with the rotated K head and the V row appended to the cache in the
+// same pass (one launch instead of rope + append).  Row t's K/V goes to index idx[t] of cache slot t, or (MAPPED: the prompt-lookup
+// verify step) of slot row_slot[t].
+template <bool MAPPED>
+__global__ void __launch_bounds__(256) rope_kv_append_kernel(bf16* __restrict__ x, long long ld, const float* __restrict__ cs, int T,
+                                                             int q_heads, int kv_heads, int hd, const int* __restrict__ row_slot,
+                                                             const int* __restrict__ idx, bf16* __restrict__ kc, bf16* __restrict__ vc, int cap) {
+  griddep_launch();
+  griddep_wait();
   const int half = hd / 2, chunks = half / 8, n_heads = q_heads + kv_heads, kv_dim = kv_heads * hd;
   const long long n_rot = (long long)T * n_heads * chunks, n_v = (long long)T * (kv_dim / 8);
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n_rot + n_v; i += (long long)gridDim.x * blockDim.x) {
@@ -62,7 +73,7 @@ __device__ __forceinline__ void rope_kv_append_rows(bf16* __restrict__ x, long l
       const long long j = i - n_rot;
       const int t = (int)(j / (kv_dim / 8)), c = (int)(j % (kv_dim / 8));
       const bf16* src = x + (long long)t * ld + (long long)n_heads * hd + c * 8;
-      *reinterpret_cast<uint4*>(vc + ((long long)(slot ? slot[t] : t) * cap + idx[t]) * kv_dim + c * 8) = *reinterpret_cast<const uint4*>(src);
+      *reinterpret_cast<uint4*>(vc + ((long long)(MAPPED ? row_slot[t] : t) * cap + idx[t]) * kv_dim + c * 8) = *reinterpret_cast<const uint4*>(src);
       continue;
     }
     const int c = (int)(i % chunks);
@@ -70,58 +81,27 @@ __device__ __forceinline__ void rope_kv_append_rows(bf16* __restrict__ x, long l
     const int h = (int)(r % n_heads);
     const int t = (int)(r / n_heads);
     bf16* p = x + (long long)t * ld + (long long)h * hd + c * 8;
-    const uint4 a = *reinterpret_cast<const uint4*>(p), b = *reinterpret_cast<const uint4*>(p + half);
-    const float4* cp = reinterpret_cast<const float4*>(cs + (long long)t * half + c * 8);
-    const float4* sp = reinterpret_cast<const float4*>(cs + (long long)T * half + (long long)t * half + c * 8);
-    const float4 c0 = cp[0], c1 = cp[1], s0 = sp[0], s1 = sp[1];
-    const float co[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w}, si[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
-    const uint32_t au[4] = {a.x, a.y, a.z, a.w}, bu[4] = {b.x, b.y, b.z, b.w};
-    uint32_t oa[4], ob[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float x1l = bf16_lo(au[k]), x1h = bf16_hi(au[k]), x2l = bf16_lo(bu[k]), x2h = bf16_hi(bu[k]);
-      oa[k] = pack_bf16(x1l * co[2 * k] - x2l * si[2 * k], x1h * co[2 * k + 1] - x2h * si[2 * k + 1]);
-      ob[k] = pack_bf16(x2l * co[2 * k] + x1l * si[2 * k], x2h * co[2 * k + 1] + x1h * si[2 * k + 1]);
-    }
-    const uint4 va = make_uint4(oa[0], oa[1], oa[2], oa[3]), vb = make_uint4(ob[0], ob[1], ob[2], ob[3]);
+    uint4 ra, rb;
+    rope_rotate8(p, half, cs, T, t, c, ra, rb);
     if (h < q_heads) {
-      *reinterpret_cast<uint4*>(p) = va;
-      *reinterpret_cast<uint4*>(p + half) = vb;
+      *reinterpret_cast<uint4*>(p) = ra;
+      *reinterpret_cast<uint4*>(p + half) = rb;
     } else {   // K heads are only consumed from the cache
-      bf16* kp = kc + ((long long)(slot ? slot[t] : t) * cap + idx[t]) * kv_dim + (long long)(h - q_heads) * hd + c * 8;
-      *reinterpret_cast<uint4*>(kp) = va;
-      *reinterpret_cast<uint4*>(kp + half) = vb;
+      bf16* kp = kc + ((long long)(MAPPED ? row_slot[t] : t) * cap + idx[t]) * kv_dim + (long long)(h - q_heads) * hd + c * 8;
+      *reinterpret_cast<uint4*>(kp) = ra;
+      *reinterpret_cast<uint4*>(kp + half) = rb;
     }
   }
 }
-__global__ void __launch_bounds__(256) rope_kv_append_kernel(bf16* __restrict__ x, long long ld, const float* __restrict__ cs, int T,
-                                                             int q_heads, int kv_heads, int hd, const int* __restrict__ cache_len,
-                                                             bf16* __restrict__ kc, bf16* __restrict__ vc, int cap) {
-  griddep_launch();
-  griddep_wait();
-  rope_kv_append_rows(x, ld, cs, T, q_heads, kv_heads, hd, nullptr, cache_len, kc, vc, cap);
-}
-// the prompt-lookup verify step: row t into (slot row_slot[t], index row_idx[t])
-__global__ void __launch_bounds__(256) rope_kv_append_map_kernel(bf16* __restrict__ x, long long ld, const float* __restrict__ cs, int T,
-                                                                 int q_heads, int kv_heads, int hd, const int* __restrict__ row_slot,
-                                                                 const int* __restrict__ row_idx, bf16* __restrict__ kc, bf16* __restrict__ vc,
-                                                                 int cap) {
-  griddep_launch();
-  griddep_wait();
-  rope_kv_append_rows(x, ld, cs, T, q_heads, kv_heads, hd, row_slot, row_idx, kc, vc, cap);
-}
 
-int rope_kv_append(bf16* qkv, long long ld, const float* cos_sin, int T, int q_heads, int kv_heads, int head_dim, const int* cache_len,
-                   bf16* kc, bf16* vc, int cap, cudaStream_t s, const int* row_slot) {
+int rope_kv_append(bf16* qkv, long long ld, const float* cos_sin, int T, int q_heads, int kv_heads, int head_dim, const int* idx,
+                   const int* row_slot, bf16* kc, bf16* vc, int cap, cudaStream_t s) {
   FO1_CHECK_ARG(head_dim % 16 == 0 && ld % 8 == 0, "rope_kv_append: head_dim %d must be a multiple of 16 and the pitch of 8", head_dim);
   if (T == 0) return FO1_OK;
   const long long n = (long long)T * (q_heads + kv_heads) * (head_dim / 16) + (long long)T * kv_heads * head_dim / 8;
   const int blocks = (int)((n + 255) / 256 < device_sm_count() * 16 ? (n + 255) / 256 : device_sm_count() * 16);
-  if (row_slot != nullptr)
-    launch_k(rope_kv_append_map_kernel, dim3(blocks), dim3(256), 0, s, qkv, ld, cos_sin, T, q_heads, kv_heads, head_dim, row_slot, cache_len,
-             kc, vc, cap);
-  else
-    launch_k(rope_kv_append_kernel, dim3(blocks), dim3(256), 0, s, qkv, ld, cos_sin, T, q_heads, kv_heads, head_dim, cache_len, kc, vc, cap);
+  launch_k(row_slot != nullptr ? rope_kv_append_kernel<true> : rope_kv_append_kernel<false>, dim3(blocks), dim3(256), 0, s, qkv, ld, cos_sin,
+           T, q_heads, kv_heads, head_dim, row_slot, idx, kc, vc, cap);
   FO1_LAUNCH_CHECK();
   return FO1_OK;
 }
