@@ -12,6 +12,10 @@ import numpy as np
 from PIL import Image
 
 
+# the drivers prepare (and hold on the device) this many batches of inputs at a time, and run each window through the decode slots
+WINDOW = 8
+
+
 def batches(items: Sequence, n: int) -> Iterable[Sequence]:
     for i in range(0, len(items), n):
         yield items[i:i + n]

@@ -1,5 +1,6 @@
 """Batched COCO detection evaluation -- the reference's ``evaluation/eval_coco.py`` (eval_coco.py:12-103) with its per-image loop
-(:36-88) run ``--batch_size`` images at a time through ``model.generate_batch``: same inputs (the UPN proposal jsonl, the
+(:36-88) run through ``model.generate_iter`` with ``--batch_size`` decode slots (a finished image hands its slot to the next one;
+items are prepared ``WINDOW`` batches at a time): same inputs (the UPN proposal jsonl, the
 COCO ``instances`` json for the category ids), same prompt per item (``conversations[0]['value']``), same
 ``prepare_inputs`` arguments (max_tokens=4096, top_p=0.05, temperature=0.0), same post-processing
 (``extract_predictions_to_indexes`` -> one COCO result dict per (label, region index) whose label is a COCO category)
@@ -13,7 +14,7 @@ from tqdm import tqdm
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-from evaluation.common import ImageSource, Throughput, batches  # noqa: E402
+from evaluation.common import WINDOW, ImageSource, Throughput, batches  # noqa: E402
 from vlm_fo1.mm_utils import extract_predictions_to_indexes, prepare_inputs  # noqa: E402
 from vlm_fo1.model.builder import load_pretrained_model  # noqa: E402
 
@@ -42,7 +43,7 @@ def eval_coco(model_id, eval_data_path, original_data_path, img_folder, out_dir=
     out_data_path = f'{output_path}/{filename}_predictions.json'
     thr = Throughput()
 
-    for chunk in tqdm(list(batches(data_list, batch_size))):
+    for chunk in tqdm(list(batches(data_list, WINDOW * batch_size))):
         kwargs_list = []
         for data in chunk:
             image_path = src.path(data['image'], sizes.get(data['image'], (640, 480)))
@@ -52,21 +53,14 @@ def eval_coco(model_id, eval_data_path, original_data_path, img_folder, out_dir=
                          "bbox_list": data['bbox_list']}]
             kwargs_list.append(prepare_inputs(model_id, model, image_processors, tokenizer, messages, device=device, max_tokens=max_tokens,
                                               top_p=0.05, temperature=0.0, do_sample=False))
-        try:
-            outputs = model.generate_batch(kwargs_list)
-        except Exception as exc:      # the reference skips a failing image (:63-65); a failing batch is retried image by image
-            print(f"Error in batch ({exc!r}); retrying one by one")
-            outputs = []
-            for data, kw in zip(chunk, kwargs_list):
-                try:
-                    outputs.append(model.generate(**kw))
-                except Exception:
-                    print(f"Error: {data['id']}")
-                    outputs.append(None)
-        for data, kw, output_ids in zip(chunk, kwargs_list, outputs):
-            if output_ids is None:
+            kwargs_list[-1]["streamer"] = None       # many images decode at once: nothing is streamed
+        # the reference skips a failing image (:63-65): a request whose admission fails is reported and left out
+        outputs = dict(model.generate_iter(kwargs_list, batch_size=batch_size,
+                                           on_error=lambda i, exc: print(f"Error: {chunk[i]['id']} ({exc!r})")))
+        for i, (data, kw) in enumerate(zip(chunk, kwargs_list)):
+            if i not in outputs:
                 continue
-            ans = tokenizer.decode(output_ids[0, kw['inputs'].shape[1]:]).strip()
+            ans = tokenizer.decode(outputs[i][0, kw['inputs'].shape[1]:]).strip()
             print('ans:', ans)
             bbox_list, score_list = data['bbox_list'], data['score_list']
             for k, v in extract_predictions_to_indexes(ans).items():

@@ -1,5 +1,5 @@
 """Batched counting evaluation -- the reference's ``evaluation/eval_countbench.py`` (eval_countbench.py:13-64) with its per-image
-loop run ``--batch_size`` images at a time: same json (``question`` / ``answer`` / ``image`` / ``bboxes``), same
+loop run through ``model.generate_iter`` with ``--batch_size`` decode slots (items prepared ``WINDOW`` batches at a time): same json (``question`` / ``answer`` / ``image`` / ``bboxes``), same
 ``prepare_inputs`` arguments, same answer extraction (strip ``<regionN>``, first integer not preceded by "region", else 0),
 accuracy printed the same way.  ``--synthetic_images DIR`` as in eval_coco.py."""
 import json
@@ -11,7 +11,7 @@ from tqdm import tqdm
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-from evaluation.common import ImageSource, Throughput, batches, size_from_boxes  # noqa: E402
+from evaluation.common import WINDOW, ImageSource, Throughput, batches, size_from_boxes  # noqa: E402
 from vlm_fo1.mm_utils import prepare_inputs  # noqa: E402
 from vlm_fo1.model.builder import load_pretrained_model  # noqa: E402
 
@@ -32,7 +32,7 @@ def eval_countbench(data_path, image_path, model_id, device, batch_size=8, limit
     src = ImageSource(image_path, synthetic_images)
     gt_list, pred_list = [], []
     thr = Throughput()
-    for chunk in tqdm(list(batches(data, batch_size))):
+    for chunk in tqdm(list(batches(data, WINDOW * batch_size))):
         kwargs_list = []
         for item in chunk:
             im = src.path(item['image'], size_from_boxes(item['bboxes']))
@@ -41,8 +41,10 @@ def eval_countbench(data_path, image_path, model_id, device, batch_size=8, limit
                          "bbox_list": item['bboxes']}]
             kwargs_list.append(prepare_inputs(model_id, model, image_processors, tokenizer, messages, device=device, max_tokens=max_tokens,
                                               top_p=0.05, temperature=0.0, do_sample=False))
-        outputs_ids = model.generate_batch(kwargs_list)
-        for item, kw, output_ids in zip(chunk, kwargs_list, outputs_ids):
+            kwargs_list[-1]["streamer"] = None       # many images decode at once: nothing is streamed
+        outputs_ids = dict(model.generate_iter(kwargs_list, batch_size=batch_size))
+        for i, (item, kw) in enumerate(zip(chunk, kwargs_list)):
+            output_ids = outputs_ids[i]
             outputs = tokenizer.decode(output_ids[0, kw['inputs'].shape[1]:]).strip()
             pred = count_from_answer(outputs)
             pred_list.append(pred)

@@ -568,6 +568,56 @@ int fo1_lookup_drafts(const int32_t* corpus, int64_t ld, const int32_t* lens, in
                       const int32_t* stop_ids, int32_t n_stop, const int32_t* emitted, int32_t max_new_tokens, int32_t* drafts,
                       int32_t* n_draft, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Slot pool: in-flight batching of many requests (replaces the reference callers' one-image-at-a-time generate loop,
+ * eval_coco.py:36-88 / eval_countbench.py:30-60, for a whole request list).  n_slots K/V cache slots and decode-state rows live
+ * across calls; the host repeats: admit waiting requests into free slots (fo1_slots_admit), decode every slot until at most exit_at
+ * sequences still run (fo1_slots_decode), take out the finished ones.  A slot's output column is its own: its index in the slot's
+ * output row, the Philox step of its sampler, and what is tested against its own max_new_tokens; a slot that reaches its limit or a
+ * stop id finishes and stays idle (its cache stops growing) until it is admitted again.  Every step runs all n_slots rows, so the
+ * decode attention's key split and the decode path follow n_slots for the life of the pool: each request's tokens and length equal
+ * its tokens and length in a static fo1_llm_generate_sampled call of n_slots sequences on the same decode path, whatever its
+ * companions and whenever it was admitted.  Greedy and sampled decoding; no scores, streaming, beams, lookup or shared prefixes.
+ * While a pool is open it owns the model's K/V cache: every fo1_llm_generate* call is refused.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct {
+  int32_t n_slots;              /* 1 .. 65535 */
+  int32_t cap;                  /* K/V rows per slot: a request needs prompt length + max_new_tokens <= cap */
+  int32_t max_new_tokens;       /* the widest per-request limit: the pitch of out_tokens (1 .. cap - 1) */
+  const int32_t* stop_ids;      /* HOST [n_stop_ids] */
+  int32_t n_stop_ids;
+  int32_t pad_id;
+  int32_t sampled;              /* 1: some request may sample (a greedy one then draws with top_k 1, bit-identical to greedy) */
+  int32_t early_exit_interval;  /* >= 1: the per-kernel path polls the running count every k steps */
+  int32_t* out_tokens;          /* DEVICE [n_slots][max_new_tokens]: slot b's current or last request, pad_id past its length */
+  int32_t* out_lens;            /* DEVICE [n_slots] */
+  int32_t* finished;            /* DEVICE [n_slots]: 1 once the slot's request has stopped (and for a slot never admitted) */
+} fo1_slots_desc;
+/* Opens the pool (all slots idle).  Refused while one is open. */
+int fo1_slots_open(fo1_model* m, const fo1_slots_desc* o, void* stream);
+
+typedef struct {
+  int32_t n;                             /* requests admitted, 1 .. n_slots */
+  const int32_t* slots;                  /* HOST [n]: distinct free slots */
+  const int32_t* seq_lens;               /* HOST [n]: prompt lengths after the splice */
+  const void* inputs_embeds;             /* DEVICE bf16 [sum seq_lens][llm_hidden], packed */
+  const int32_t* position_ids;           /* DEVICE int32 [3][sum seq_lens] */
+  const int32_t* rope_deltas_device;     /* DEVICE int32 [n] (what fo1_splice_plan_batch wrote) */
+  const int32_t* max_new_tokens;         /* HOST [n]: each request's own limit, 1 .. the pool's max_new_tokens */
+  const fo1_sampling_desc* sampling;     /* NULL: greedy; else per request (a pool opened with sampled = 1) */
+} fo1_slots_admit_desc;
+/* Prefills the n requests into their slots (the prefill of fo1_llm_generate with the slots as the cache-write members) and records
+ * column 0.  Checked on the host before any launch: slot in range, slot free (never admitted, or seen finished by the last
+ * fo1_slots_decode), no slot twice, 1 <= max_new_tokens <= the pool's, prompt + max_new_tokens <= cap, sampling parameters. */
+int fo1_slots_admit(fo1_model* m, const fo1_slots_admit_desc* a, void* stream);
+/* Decodes every slot until at most exit_at requests still run (0: all stopped): one launch of the persistent kernel (n_slots <= 32
+ * and a supported model shape), else the per-kernel loop polling every early_exit_interval steps.  *steps_run = the decode steps
+ * run (0 when no more than exit_at run already).  Synchronises the stream; on return out_tokens / out_lens / finished are final for
+ * every finished slot, until it is admitted again. */
+int fo1_slots_decode(fo1_model* m, int32_t exit_at, int32_t* steps_run, void* stream);
+/* Closes the pool (synchronises the device). */
+int fo1_slots_close(fo1_model* m);
+
 #ifdef __cplusplus
 }
 #endif

@@ -108,6 +108,20 @@ class LookupDesc(C.Structure):
                 ("corpus_offsets", C.POINTER(C.c_int32)), ("steps", C.c_void_p), ("accepted", C.c_void_p)]
 
 
+class SlotsDesc(C.Structure):
+    """fo1_slots_desc: HOST parameters and stop ids; DEVICE int32 outputs tokens [n_slots][max_new], lens [n_slots], finished [n_slots]."""
+    _fields_ = [("n_slots", C.c_int32), ("cap", C.c_int32), ("max_new_tokens", C.c_int32), ("stop_ids", C.POINTER(C.c_int32)),
+                ("n_stop_ids", C.c_int32), ("pad_id", C.c_int32), ("sampled", C.c_int32), ("early_exit_interval", C.c_int32),
+                ("out_tokens", C.c_void_p), ("out_lens", C.c_void_p), ("finished", C.c_void_p)]
+
+
+class SlotsAdmitDesc(C.Structure):
+    """fo1_slots_admit_desc: HOST slots / seq_lens / max_new_tokens [n]; DEVICE embeddings, positions [3][sum L], rope deltas [n]."""
+    _fields_ = [("n", C.c_int32), ("slots", C.POINTER(C.c_int32)), ("seq_lens", C.POINTER(C.c_int32)), ("inputs_embeds", C.c_void_p),
+                ("position_ids", C.c_void_p), ("rope_deltas_device", C.c_void_p), ("max_new_tokens", C.POINTER(C.c_int32)),
+                ("sampling", C.POINTER(SamplingDesc))]
+
+
 FO1_STREAM_DONE = 1 << 30
 
 _lib = None
@@ -161,6 +175,14 @@ def lib() -> C.CDLL:
     L.fo1_llm_generate_lookup.restype = C.c_int
     L.fo1_llm_generate_lookup.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(LookupDesc), C.POINTER(PrefixDesc), C.POINTER(SamplingDesc),
                                           C.POINTER(ScoreDesc), C.c_void_p]
+    L.fo1_slots_open.restype = C.c_int
+    L.fo1_slots_open.argtypes = [C.c_void_p, C.POINTER(SlotsDesc), C.c_void_p]
+    L.fo1_slots_admit.restype = C.c_int
+    L.fo1_slots_admit.argtypes = [C.c_void_p, C.POINTER(SlotsAdmitDesc), C.c_void_p]
+    L.fo1_slots_decode.restype = C.c_int
+    L.fo1_slots_decode.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.c_void_p]
+    L.fo1_slots_close.restype = C.c_int
+    L.fo1_slots_close.argtypes = [C.c_void_p]
     L.fo1_lookup_drafts.restype = C.c_int
     L.fo1_lookup_drafts.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p,
                                     C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]

@@ -45,6 +45,9 @@ struct ColumnSink {
   int n_stop, pad_id, max_new;
   int *out_tokens, *out_lens;     // [B][max_new], [B]
   StreamArgs stream;
+  // slot pool (nullptr: a generate call): slot b's own output column col[b] -- its output index and its Philox step -- and its own
+  // limit max_new_row[b] <= max_new (the pitch of out_tokens)
+  int *col, *max_new_row;
 };
 
 // Recording column `step` is one block's work: column_prologue and column_epilogue by every thread, record_token in between by one
@@ -68,6 +71,22 @@ __device__ __forceinline__ void column_prologue(const ColumnSink& k, int step, b
 template <bool STREAM>
 __device__ __forceinline__ void record_token(const ColumnSink& k, int B, int b, int step, int tok, bool advance, bool publish, bool cancel) {
   const DecodeState& st = k.st;
+  if (k.col != nullptr) {     // slot pool: a finished slot is idle (its row stays as recorded, its cache stops growing) until refilled
+    if (st.finished[b]) return;
+    const int c = k.col[b];
+    k.out_tokens[(long long)b * k.max_new + c] = tok;
+    k.out_lens[b] = c + 1;
+    k.col[b] = c + 1;
+    bool stop = c + 1 >= k.max_new_row[b];
+    for (int i = 0; i < k.n_stop; ++i) stop |= (tok == st.stop_ids[i]);
+    if (stop) { st.finished[b] = 1; atomicSub(st.n_active, 1); }
+    st.cur_tok[b] = tok;
+    if (advance) {
+      st.cache_len[b] += 1;
+      st.pos3[b] += 1; st.pos3[B + b] += 1; st.pos3[2 * B + b] += 1;
+    }
+    return;
+  }
   if (step < k.max_new) {
     if (!st.finished[b]) {
       k.out_tokens[(long long)b * k.max_new + step] = tok;

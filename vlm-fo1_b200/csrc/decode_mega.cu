@@ -722,7 +722,9 @@ __global__ void __launch_bounds__(kMgThreads, 1) decode_mega_kernel(const MegaAr
             if (threadIdx.x == 0 && a.sc_logprobs != nullptr) a.sc_logprobs[(long long)b * a.sink.max_new + step] = lp;
           }
         } else {
-          const int tok = sample_row<kMgThreads>(a.logits + (long long)b * a.V, a.V, a.samp[b], __ldcg(a.sink.st.step), sm);
+          // the Philox step is the output column: the call's step counter, or (slot pool) the slot's own column
+          const int col = a.sink.col != nullptr ? __ldcg(a.sink.col + b) : __ldcg(a.sink.st.step);
+          const int tok = sample_row<kMgThreads>(a.logits + (long long)b * a.V, a.V, a.samp[b], col, sm);
           if (threadIdx.x == 0) a.samp_tok[b] = tok;
         }
       }
@@ -768,7 +770,7 @@ __global__ void __launch_bounds__(kMgThreads, 1) decode_mega_kernel(const MegaAr
       column_epilogue<STREAM>(a.sink, step, publish, cancel);
     }
     MG_STAMP(slot, 0); mg_grid_sync(a.bar, gen); MG_STAMP(slot, 1); ++slot;
-    if (__ldcg(a.sink.st.n_active) <= 0) break;           // every sequence has emitted a stop id (the tail of out_tokens is pad already)
+    if (__ldcg(a.sink.st.n_active) <= a.exit_at) break;   // (exit_at 0: every sequence has stopped; the tail of out_tokens is pad already)
   }
   mg_wait<0>();
 }

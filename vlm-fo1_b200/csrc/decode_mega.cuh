@@ -29,6 +29,7 @@ struct MegaArgs {
   float* amax_val; int* amax_idx;   // [grid][32]
   ColumnSink sink;            // loop state, outputs and (STREAM) their mirror; CTA 0 records every column
   int n_steps;                // decode iterations to run at most
+  int exit_at;                // the loop ends once at most this many sequences are running (0: all stopped)
   unsigned* bar;              // grid barrier counter (zeroed by the host before the launch)
   int n_splits;
   unsigned long long* prof;   // [grid][prof_slots][2] barrier enter / leave stamps of the first iteration (FO1_MEGA_PROF; nullptr: off)

@@ -91,6 +91,7 @@ struct Model {
   void* decode_graph = nullptr;  // cudaGraphExec_t
   std::string decode_graph_key;
   void* llm_state = nullptr;     // struct LlmState*, owned by llm.cu
+  void* slot_pool = nullptr;     // struct SlotPool* while a slot pool is open (fo1_slots_open), owned by llm.cu
 
   const WeightRef* find(const std::string& name) const {
     auto it = weights.find(name);

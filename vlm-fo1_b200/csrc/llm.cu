@@ -353,6 +353,32 @@ __global__ void __launch_bounds__(1024) decode_update_kernel(ColumnSink k, int B
 __global__ void fill_int_kernel(int* p, int v, long long n) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) p[i] = v;
 }
+// slot pool: after the prefill of n admitted sequences, decode_init_kernel for the listed slots (B = the pool's slot count): lengths,
+// positions, column 0, limit and sampling parameters (prm: the admitted rows', copied to pool_prm), output rows refilled with pad, then
+// column 0 (tok[i], drawn from the prefill's last row) recorded as a decode step records one
+__global__ void __launch_bounds__(256) slots_admit_kernel(ColumnSink k, int B, int n, const int* __restrict__ slots,
+                                                          const int* __restrict__ max_new, const int* __restrict__ seq_lens,
+                                                          const int* __restrict__ deltas, const int* __restrict__ tok,
+                                                          const SampleRowParams* __restrict__ prm, SampleRowParams* __restrict__ pool_prm) {
+  const DecodeState& st = k.st;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const int b = slots[i];
+    st.cache_len[b] = seq_lens[i];
+    const int p = seq_lens[i] + deltas[i];
+    st.pos3[b] = p; st.pos3[B + b] = p; st.pos3[2 * B + b] = p;
+    st.finished[b] = 0;
+    k.col[b] = 0;
+    k.max_new_row[b] = max_new[i];
+    if (prm != nullptr) pool_prm[b] = prm[i];
+  }
+  for (long long j = threadIdx.x; j < (long long)n * k.max_new; j += blockDim.x)
+    k.out_tokens[(long long)slots[j / k.max_new] * k.max_new + j % k.max_new] = k.pad_id;
+  __syncthreads();
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    atomicAdd(st.n_active, 1);
+    record_token<false>(k, B, slots[i], 0, tok[i], false, false, false);
+  }
+}
 
 // ------------------------------------------------------------------------------------------ host
 struct LlmState {
@@ -413,7 +439,9 @@ static int llm_resolve(Model* m) {
 }
 int llm_finalize(Model* m) { return m->cfg.llm_layers > 0 ? llm_resolve(m) : FO1_OK; }
 
+static void slots_free(Model* m);
 void llm_destroy_state(Model* m) {
+  slots_free(m);
   if (m->llm.mega_layers) { cudaFree(m->llm.mega_layers); m->llm.mega_layers = nullptr; }
   LlmState* s = static_cast<LlmState*>(m->llm_state);
   if (!s) return;
@@ -464,8 +492,19 @@ static int ensure_state(Model* m, int B, int n_stop, DecodeState* st) {
 // size; the width alone decides for models wider than it serves
 static NormKernel seq_norm_kernel(int H) { return H <= kNormBlockMaxCols ? NORM_BLOCK : NORM_WARP; }
 
+// an open slot pool (fo1_slots_open): its loop state, column sink and per-slot sampling parameters live across calls
+struct SlotPool {
+  int n_slots, interval;
+  DecodeMode mode;                  // DEC_SAMPLED when any slot may sample, else DEC_GREEDY
+  ColumnSink k;                     // k.col / k.max_new_row: [n_slots] each, in `ints`
+  int* ints = nullptr;              // col, max_new_row, then the admission's slots / max_new / 0 (n_slots each, + 1)
+  SampleRowParams* prm = nullptr;   // [n_slots]
+  std::vector<int> busy;            // host: admitted and not seen finished by the last fo1_slots_decode
+};
+
 // one generate call, described once by llm_generate: the caller's descriptors, the decode mode, the column sink, and the device state
-// of beam search (with its host table of length-penalty divisors) or of prompt lookup
+// of beam search (with its host table of length-penalty divisors) or of prompt lookup; or one admission into / decode segment of a
+// slot pool (`pool`; an admission's host slot list `slots`)
 struct GenerateCall {
   fo1_generate_desc* d;
   const fo1_prefix_desc* px;        // shared prefix (null: none)
@@ -479,6 +518,9 @@ struct GenerateCall {
   std::vector<float> lp_div;
   const fo1_lookup_desc* lkd;       // prompt lookup (null: none): `lookup`
   LookupArgs lookup;
+  SlotPool* pool;
+  const int* slots;
+  int exit_at;                      // the decode loop ends once at most this many sequences run (0: all stopped)
 };
 
 // the scratch buffers of a decoder layer over packed rows
@@ -551,6 +593,15 @@ static int llm_layer(Model* m, int li, const bf16* x_in, bf16* x_out, const Laye
   return FO1_OK;
 }
 
+// CTAs of the persistent decode kernel for B sequences, or 0 (the per-kernel path): the persistent kernel serves every batch it
+// supports (1..32 sequences; scripts/mega_prof.py times the two paths alternately).  FO1_MEGA_MAX_B lowers the threshold,
+// FO1_NO_MEGA disables the kernel.
+static int mega_grid_for(Model* m, int B) {
+  int mega_max_b = 32;
+  if (const char* e = getenv("FO1_MEGA_MAX_B")) mega_max_b = std::max(0, std::min(32, atoi(e)));
+  return m->llm.mega_ok && B <= mega_max_b && getenv("FO1_NO_MEGA") == nullptr ? decode_mega_grid() : 0;
+}
+
 // the buffers both decode paths use after the prefill, carved from the arena (the dry run sizes it)
 struct DecodeBufs {
   int mega_grid;                  // CTAs of the persistent kernel (0: the per-kernel path)
@@ -560,6 +611,31 @@ struct DecodeBufs {
   int *mg_amax_i, *mg_sync, *samp_tok;
   SampleRowParams* samp;
 };
+
+// the buffers of DecodeBufs every decode path reads: the layer buffers and the two residual streams for R rows, the per-row decode
+// scratch for RD rows, and the persistent kernel's per-CTA slots (g.mega_grid set) and barrier words for B sequences
+static void decode_bufs_alloc(Model* m, DecodeBufs& g, int R, int RD, int B) {
+  const fo1_model_config& c = m->cfg;
+  Arena& A = m->arena;
+  const int H = c.llm_hidden, hd = c.llm_head_dim, QD = c.llm_heads * hd, KD = c.llm_kv_heads * hd;
+  const int Ip = (c.llm_inter + 31) / 32 * 32;
+  LayerBuf& buf = g.layer;
+  g.xa = A.alloc<bf16>((size_t)R * H);
+  g.xb = A.alloc<bf16>((size_t)R * H);
+  buf.xn = A.alloc<bf16>((size_t)R * H);
+  buf.qkv = A.alloc<bf16>((size_t)R * (QD + 2 * KD));
+  buf.att = A.alloc<bf16>((size_t)R * QD);
+  buf.x_mid = A.alloc<bf16>((size_t)R * H);
+  buf.h = A.alloc<bf16>((size_t)R * Ip);
+  g.cs_dec = A.alloc<float>((size_t)RD * hd);
+  buf.dec_part = A.alloc<float>((size_t)RD * c.llm_heads * kDecSplits * (128 + 4));
+  g.lastn = A.alloc<bf16>((size_t)RD * H);
+  g.logits = A.alloc<float>((size_t)RD * c.llm_vocab);
+  g.mg_ssq = A.alloc<float>((size_t)2 * std::max(g.mega_grid, 1) * 32);
+  g.mg_amax_v = A.alloc<float>((size_t)std::max(g.mega_grid, 1) * 32);
+  g.mg_amax_i = A.alloc<int>((size_t)std::max(g.mega_grid, 1) * 32);
+  g.mg_sync = A.alloc<int>((size_t)B * c.llm_kv_heads + 8);
+}
 
 // the tokens of the current output column into new_tok (scored: also the column's scores), then their recording; every kernel reads
 // the column from *st.step, as the captured decode step does.  `advance`: the column came from a decode step (not the prefill)
@@ -572,13 +648,32 @@ static int decode_column(const GenerateCall& q, const DecodeBufs& g, int B, int 
     FO1_TRY(score_rows(g.logits, V, B, V, g.samp, st.step, st.new_tok, true, st.finished, k.max_new, sc->logprobs, k.max_new, sc->scores,
                        sc->logits, V, s));
   } else if (q.mode == DEC_SAMPLED) {
-    FO1_TRY(sample_rows(g.logits, V, B, V, g.samp, st.step, 0, st.new_tok, s));       // the Philox step is read from *st.step
+    // the Philox step is read from *st.step, or (slot pool) from each slot's own column
+    FO1_TRY(sample_rows(g.logits, V, B, V, g.samp, k.col != nullptr ? k.col : st.step, k.col != nullptr ? 1 : 0, st.new_tok, s));
   } else {
     launch_k(argmax_kernel, dim3(B), dim3(1024), 0, s, g.logits, V, st.new_tok);
     FO1_LAUNCH_CHECK();
   }
   const int threads = std::min(1024, std::max(32, (B + 31) / 32 * 32));
   launch_k(k.stream.progress != nullptr ? decode_update_kernel<true> : decode_update_kernel<false>, dim3(1), dim3(threads), 0, s, k, B, advance);
+  FO1_LAUNCH_CHECK();
+  return FO1_OK;
+}
+
+// slot pool admission, after the prefill of its n sequences: column 0 from the prefill's last rows (the Philox step is 0), then the
+// admitted slots' state (slots_admit_kernel).  The slot list and limits were uploaded to the pool's admission ints by slots_admit.
+static int slots_admit_column(const GenerateCall& q, const DecodeBufs& g, int V, const int* d_lens, const int* d_deltas, cudaStream_t s) {
+  const SlotPool& p = *q.pool;
+  const int n = q.d->n_seqs, N = p.n_slots;
+  const int* adm = p.ints + 2 * N;        // slots [N], max_new [N], 0
+  if (p.mode == DEC_SAMPLED) {
+    FO1_TRY(sample_rows(g.logits, V, n, V, g.samp, adm + 2 * N, 0, p.k.st.new_tok, s));
+  } else {
+    launch_k(argmax_kernel, dim3(n), dim3(1024), 0, s, (const float*)g.logits, V, p.k.st.new_tok);
+    FO1_LAUNCH_CHECK();
+  }
+  slots_admit_kernel<<<1, 256, 0, s>>>(p.k, N, n, adm, adm + N, d_lens, d_deltas, p.k.st.new_tok,
+                                       p.mode == DEC_SAMPLED ? g.samp : nullptr, p.prm);
   FO1_LAUNCH_CHECK();
   return FO1_OK;
 }
@@ -610,12 +705,13 @@ static int prefill_plan(Model* m, const GenerateCall& q, const LayerBuf& b, int 
   for (int i = 0; i < B; ++i) {
     pre[i] = prefix_of(px, i); own[i] = d->seq_lens[i] - pre[i];
     for (int t = 0; t < own[i]; ++t) { row_gt.push_back(G + i); row_gt.push_back(pre[i] + t); }
-    for (int j = 0; j < N; ++j) members.push_back(i * N + j);
+    for (int j = 0; j < N; ++j) members.push_back(q.slots ? q.slots[i] : i * N + j);
     grp_off.push_back((int)members.size());
     r += own[i];
     last.push_back(r - 1);
     if (!px) cu.push_back(r);
     key += "/" + std::to_string(px ? px->seq_group[i] : -1) + ":" + std::to_string(d->seq_lens[i]);
+    if (q.slots) key += "@" + std::to_string(q.slots[i]);
   }
   const int* gt = nullptr;
   FO1_TRY(cached_ints(m, key + ":gt", row_gt, &gt, s));
@@ -666,8 +762,7 @@ static int llm_prefill(Model* m, GenerateCall& q, cudaStream_t s, bool dry, Deco
   const fo1_prefix_desc* px = q.px;
   const bool beam = q.bmd != nullptr, lookup = q.lkd != nullptr;
   const int B = d->n_seqs, H = c.llm_hidden, hd = c.llm_head_dim, V = c.llm_vocab;
-  const int QD = c.llm_heads * hd, KD = c.llm_kv_heads * hd, ldq = QD + 2 * KD;
-  const int Ip = (c.llm_inter + 31) / 32 * 32;
+  const int KD = c.llm_kv_heads * hd;
   long long T = 0;      // packed rows through the layers: every sequence's rows, or (px) the prefix rows then the own rows
   int n_pre = 0;
   for (int b = 0; b < B; ++b) T += d->seq_lens[b] - prefix_of(px, b);
@@ -678,34 +773,16 @@ static int llm_prefill(Model* m, GenerateCall& q, cudaStream_t s, bool dry, Deco
 
   g = DecodeBufs();
   LayerBuf& buf = g.layer;
-  g.xa = A.alloc<bf16>((size_t)R * H);
-  g.xb = A.alloc<bf16>((size_t)R * H);
-  buf.xn = A.alloc<bf16>((size_t)R * H);
-  buf.qkv = A.alloc<bf16>((size_t)R * ldq);
-  buf.att = A.alloc<bf16>((size_t)R * QD);
-  buf.x_mid = A.alloc<bf16>((size_t)R * H);
-  buf.h = A.alloc<bf16>((size_t)R * Ip);
+  // persistent decode kernel (decode_mega.cu): per-CTA slots + the grid barrier
+  g.mega_grid = !beam && !lookup ? mega_grid_for(m, B) : 0;
+  decode_bufs_alloc(m, g, R, RD, B);
   float* cs_pre = A.alloc<float>((size_t)R * hd);
-  g.cs_dec = A.alloc<float>((size_t)RD * hd);
-  buf.dec_part = A.alloc<float>((size_t)RD * c.llm_heads * kDecSplits * (128 + 4));
   buf.rowseg = A.alloc<int>((size_t)R * 2);
   bf16* last = A.alloc<bf16>((size_t)B * H);
-  g.lastn = A.alloc<bf16>((size_t)RD * H);
-  g.logits = A.alloc<float>((size_t)RD * V);
   bf16* alln = d->all_logits ? A.alloc<bf16>((size_t)T * H) : nullptr;
   int* d_lens = A.alloc<int>(B);
   int* d_deltas = A.alloc<int>(B);
   int* pos_all = px ? A.alloc<int>((size_t)3 * T) : nullptr;      // prefix positions, then the own rows'
-  // persistent decode kernel (decode_mega.cu): per-CTA slots + the grid barrier
-  // the persistent kernel serves every batch it supports (1..32 sequences; scripts/mega_prof.py times the two paths alternately).
-  // FO1_MEGA_MAX_B lowers the threshold, FO1_NO_MEGA disables the kernel.
-  int mega_max_b = 32;
-  if (const char* e = getenv("FO1_MEGA_MAX_B")) mega_max_b = std::max(0, std::min(32, atoi(e)));
-  g.mega_grid = (m->llm.mega_ok && !beam && !lookup && B <= mega_max_b && getenv("FO1_NO_MEGA") == nullptr) ? decode_mega_grid() : 0;
-  g.mg_ssq = A.alloc<float>((size_t)2 * std::max(g.mega_grid, 1) * 32);
-  g.mg_amax_v = A.alloc<float>((size_t)std::max(g.mega_grid, 1) * 32);
-  g.mg_amax_i = A.alloc<int>((size_t)std::max(g.mega_grid, 1) * 32);
-  g.mg_sync = A.alloc<int>((size_t)B * c.llm_kv_heads + 8);
   // sampled or scored decoding: the per-sequence parameters and the tokens the persistent kernel's CTA b drew
   g.samp = q.mode == DEC_SAMPLED || q.mode == DEC_SCORED ? A.alloc<SampleRowParams>(B) : nullptr;
   g.samp_tok = q.mode == DEC_SAMPLED || q.mode == DEC_SCORED ? A.alloc<int>(B) : nullptr;
@@ -772,6 +849,7 @@ static int llm_prefill(Model* m, GenerateCall& q, cudaStream_t s, bool dry, Deco
     FO1_RUN(linear(g.lastn, H, m->llm.lm_head, H, g.logits, V, FO1_F32, B, V, H, nullptr, 0, FO1_EPI_NONE, nullptr, 0, 0, s));
   }
   if (dry) return FO1_OK;
+  if (q.pool) return slots_admit_column(q, g, V, d_lens, d_deltas, s);
   if (d->prefill_logits) FO1_CUDA(cudaMemcpyAsync(d->prefill_logits, g.logits, (size_t)B * V * sizeof(float), cudaMemcpyDeviceToDevice, s));
   if (beam) {
     FO1_TRY(beam_init(q.beam, q.k.st, d_lens, d_deltas, s));
@@ -801,7 +879,7 @@ static int decode_persistent(Model* m, const GenerateCall& q, const DecodeBufs& 
   a.amax_val = g.mg_amax_v; a.amax_idx = g.mg_amax_i; a.sink = q.k;
   a.logits = g.logits; a.samp = g.samp; a.samp_tok = g.samp_tok;
   if (q.sc) { a.sc_logprobs = q.sc->logprobs; a.sc_scores = q.sc->scores; a.sc_logits = q.sc->logits; }
-  a.n_steps = d->max_new_tokens - 1; a.bar = reinterpret_cast<unsigned*>(g.mg_sync);
+  a.n_steps = d->max_new_tokens - 1; a.exit_at = q.exit_at; a.bar = reinterpret_cast<unsigned*>(g.mg_sync);
   const int pairs = B * c.llm_kv_heads;
   a.n_splits = std::max(1, std::min(kMgMaxSplits, g.mega_grid / std::max(1, pairs)));
   FO1_CUDA(cudaMemsetAsync(g.mg_sync, 0, ((size_t)pairs + 8) * sizeof(int), s));
@@ -923,7 +1001,7 @@ static int decode_per_kernel(Model* m, const GenerateCall& q, const DecodeBufs& 
       if (cudaMemcpyAsync(ls->h_flag, k.st.n_active, sizeof(int), cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess) {
         set_error("early-exit poll failed"); rc = FO1_ERR_CUDA; break;
       }
-      if (*ls->h_flag <= 0) break;  // every sequence has emitted a stop id; the tail is already pad_id
+      if (*ls->h_flag <= q.exit_at) break;  // (exit_at 0: every sequence has emitted a stop id; the tail is already pad_id)
     }
   }
   if (gexec != nullptr) {
@@ -984,6 +1062,7 @@ int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, co
   if (sp) FO1_TRY(sampling_check(sp, d->n_seqs, sc ? "fo1_llm_generate_scored" : "fo1_llm_generate_sampled"));
   if (sc) FO1_TRY(raw_rows_check(sp, sc->raw_rows, d->n_seqs, "fo1_llm_generate_scored"));
   FO1_CHECK_ARG(m->llm.ok, "fo1_llm_generate: model not finalized (LLM weights unresolved)");
+  FO1_CHECK_ARG(m->slot_pool == nullptr, "fo1_llm_generate: a slot pool is open on this model (it owns the K/V cache); fo1_slots_close first");
   const fo1_model_config& c = m->cfg;
   FO1_CHECK_ARG(d->n_seqs > 0 && d->seq_lens && d->inputs_embeds && d->position_ids && (d->rope_deltas || d->rope_deltas_device),
                 "fo1_llm_generate: null argument");
@@ -1051,6 +1130,158 @@ int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, co
   if (g.mega_grid > 0 && d->max_new_tokens > 1) return decode_persistent(m, q, g, s);
   FO1_TRY(decode_per_kernel(m, q, g, s));
   return bmd ? beam_finalize(q.beam, s) : FO1_OK;
+}
+
+// -------------------------------------------------------------------------------- slot pool
+static void slots_free(Model* m) {
+  SlotPool* p = static_cast<SlotPool*>(m->slot_pool);
+  if (!p) return;
+  if (p->ints) cudaFree(p->ints);
+  if (p->prm) cudaFree(p->prm);
+  delete p;
+  m->slot_pool = nullptr;
+}
+
+// the device state of a freshly registered pool (its caller frees the pool if this fails)
+static int slots_init(SlotPool* p, const fo1_slots_desc* o, const DecodeState& st, cudaStream_t s) {
+  const int N = o->n_slots;
+  p->n_slots = N; p->interval = o->early_exit_interval; p->mode = o->sampled ? DEC_SAMPLED : DEC_GREEDY;
+  p->busy.assign(N, 0);
+  ColumnSink& k = p->k;
+  k = ColumnSink();
+  k.st = st;
+  k.st.finished = o->finished;
+  k.n_stop = o->n_stop_ids; k.pad_id = o->pad_id; k.max_new = o->max_new_tokens;
+  k.out_tokens = o->out_tokens; k.out_lens = o->out_lens;
+  if (cudaMalloc(reinterpret_cast<void**>(&p->ints), ((size_t)4 * N + 1) * sizeof(int)) != cudaSuccess ||
+      cudaMalloc(reinterpret_cast<void**>(&p->prm), (size_t)N * sizeof(SampleRowParams)) != cudaSuccess) {
+    cudaGetLastError();
+    set_error("fo1_slots_open: out of device memory for %d slots", N);
+    return FO1_ERR_CUDA;
+  }
+  k.col = p->ints; k.max_new_row = p->ints + N;
+  // every slot starts idle (finished, nothing running): an idle slot's rows still run in each step, so its state must be valid
+  FO1_CUDA(cudaMemsetAsync(p->ints, 0, ((size_t)4 * N + 1) * sizeof(int), s));
+  FO1_CUDA(cudaMemsetAsync(st.cache_len, 0, (size_t)N * sizeof(int), s));
+  for (int a = 0; a < 3; ++a) FO1_CUDA(cudaMemsetAsync(st.pos3 + (size_t)a * N, 0, (size_t)N * sizeof(int), s));
+  FO1_CUDA(cudaMemsetAsync(st.cur_tok, 0, (size_t)N * sizeof(int), s));
+  FO1_CUDA(cudaMemsetAsync(st.n_active, 0, sizeof(int), s));
+  FO1_CUDA(cudaMemsetAsync(st.step, 0, sizeof(int), s));
+  FO1_CUDA(cudaMemsetAsync(o->out_lens, 0, (size_t)N * sizeof(int), s));
+  fill_int_kernel<<<ceil_div(N, 256), 256, 0, s>>>(o->finished, 1, N);
+  FO1_LAUNCH_CHECK();
+  if (o->n_stop_ids > 0) FO1_CUDA(cudaMemcpyAsync(st.stop_ids, o->stop_ids, o->n_stop_ids * sizeof(int), cudaMemcpyHostToDevice, s));
+  const std::vector<SampleRowParams> greedy(N, SampleRowParams{1.0f, 1.0f, 1, 0, 0ull});
+  FO1_CUDA(cudaMemcpyAsync(p->prm, greedy.data(), greedy.size() * sizeof(SampleRowParams), cudaMemcpyHostToDevice, s));
+  return cudaStreamSynchronize(s) == cudaSuccess ? FO1_OK : (set_error("fo1_slots_open: %s", cudaGetErrorString(cudaGetLastError())), FO1_ERR_CUDA);
+}
+
+static int slots_open(Model* m, const fo1_slots_desc* o, cudaStream_t s) {
+  FO1_CHECK_ARG(m->llm.ok, "fo1_slots_open: model not finalized (LLM weights unresolved)");
+  FO1_CHECK_ARG(m->slot_pool == nullptr, "fo1_slots_open: a slot pool is already open on this model");
+  FO1_CHECK_ARG(m->cfg.llm_head_dim == 128, "fo1_slots_open: head_dim %d unsupported (128)", m->cfg.llm_head_dim);
+  FO1_CHECK_ARG(o->n_slots >= 1 && o->n_slots <= 65535, "fo1_slots_open: n_slots %d out of range [1, 65535]", o->n_slots);
+  FO1_CHECK_ARG(o->max_new_tokens >= 1 && o->cap > o->max_new_tokens, "fo1_slots_open: max_new_tokens %d / cap %d (1 <= max_new_tokens < cap)",
+                o->max_new_tokens, o->cap);
+  FO1_CHECK_ARG(o->early_exit_interval >= 1, "fo1_slots_open: early_exit_interval %d must be >= 1", o->early_exit_interval);
+  FO1_CHECK_ARG(o->n_stop_ids >= 0 && (o->n_stop_ids == 0 || o->stop_ids), "fo1_slots_open: null stop_ids");
+  FO1_CHECK_ARG(o->out_tokens && o->out_lens && o->finished, "fo1_slots_open: null outputs");
+  const int N = o->n_slots;
+  DecodeState st;
+  FO1_TRY(ensure_state(m, N, o->n_stop_ids, &st));
+  FO1_TRY(ensure_kv(m, N, o->cap));
+  SlotPool* p = new SlotPool();
+  m->slot_pool = p;
+  const int rc = slots_init(p, o, st, s);
+  if (rc != FO1_OK) slots_free(m);      // a pool that failed to open is not left registered: generate calls stay possible
+  return rc;
+}
+
+static int slots_admit(Model* m, const fo1_slots_admit_desc* a, cudaStream_t s) {
+  SlotPool* p = static_cast<SlotPool*>(m->slot_pool);
+  FO1_CHECK_ARG(p != nullptr, "fo1_slots_admit: no slot pool is open");
+  const int N = p->n_slots, n = a->n;
+  FO1_CHECK_ARG(n >= 1 && n <= N, "fo1_slots_admit: %d sequences for %d slots", n, N);
+  FO1_CHECK_ARG(a->slots && a->seq_lens && a->max_new_tokens && a->inputs_embeds && a->position_ids && a->rope_deltas_device,
+                "fo1_slots_admit: null argument");
+  if (a->sampling) {
+    FO1_CHECK_ARG(p->mode == DEC_SAMPLED, "fo1_slots_admit: sampling parameters for a pool opened without sampling");
+    FO1_TRY(sampling_check(a->sampling, n, "fo1_slots_admit"));
+  }
+  std::vector<char> seen(N, 0);
+  for (int i = 0; i < n; ++i) {
+    const int b = a->slots[i];
+    FO1_CHECK_ARG(b >= 0 && b < N, "fo1_slots_admit: sequence %d: slot %d out of range [0, %d)", i, b, N);
+    FO1_CHECK_ARG(!p->busy[b] && !seen[b], "fo1_slots_admit: sequence %d: slot %d is occupied", i, b);
+    seen[b] = 1;
+    FO1_CHECK_ARG(a->max_new_tokens[i] >= 1 && a->max_new_tokens[i] <= p->k.max_new,
+                  "fo1_slots_admit: sequence %d: max_new_tokens %d out of range [1, %d]", i, a->max_new_tokens[i], p->k.max_new);
+    FO1_CHECK_ARG(a->seq_lens[i] >= 1 && a->seq_lens[i] + a->max_new_tokens[i] <= m->kv_cap,
+                  "fo1_slots_admit: sequence %d: %d prompt rows + %d new tokens exceed the slot capacity %d", i, a->seq_lens[i],
+                  a->max_new_tokens[i], m->kv_cap);
+  }
+  fo1_generate_desc d{};
+  d.n_seqs = n; d.seq_lens = a->seq_lens; d.inputs_embeds = a->inputs_embeds; d.position_ids = a->position_ids;
+  d.rope_deltas_device = a->rope_deltas_device; d.max_new_tokens = 1; d.pad_id = p->k.pad_id;
+  GenerateCall q{};
+  q.d = &d; q.sp = a->sampling; q.mode = p->mode; q.k = p->k; q.pool = p; q.slots = a->slots;
+  FO1_TRY(int_cache_trim(m));
+  FO1_CUDA(cudaMemcpyAsync(p->ints + 2 * N, a->slots, n * sizeof(int), cudaMemcpyHostToDevice, s));
+  FO1_CUDA(cudaMemcpyAsync(p->ints + 3 * N, a->max_new_tokens, n * sizeof(int), cudaMemcpyHostToDevice, s));
+  m->arena.reset(true);
+  DecodeBufs g;
+  FO1_TRY(llm_prefill(m, q, s, true, g));
+  FO1_TRY(arena_ensure(m, m->arena.peak));
+  m->arena.reset(false);
+  FO1_TRY(llm_prefill(m, q, s, false, g));
+  for (int i = 0; i < n; ++i) p->busy[a->slots[i]] = 1;
+  return FO1_OK;
+}
+
+// the decode buffers of n_slots rows: only per-step scratch, so each segment carves them anew
+static void slots_decode_bufs(Model* m, const SlotPool& p, DecodeBufs& g) {
+  g = DecodeBufs();
+  g.mega_grid = mega_grid_for(m, p.n_slots);
+  decode_bufs_alloc(m, g, p.n_slots, p.n_slots, p.n_slots);
+  g.samp = p.mode == DEC_SAMPLED ? p.prm : nullptr;
+  g.samp_tok = m->arena.alloc<int>(p.n_slots);
+}
+
+static int slots_decode(Model* m, int exit_at, int* steps_run, cudaStream_t s) {
+  SlotPool* p = static_cast<SlotPool*>(m->slot_pool);
+  FO1_CHECK_ARG(p != nullptr, "fo1_slots_decode: no slot pool is open");
+  FO1_CHECK_ARG(exit_at >= 0, "fo1_slots_decode: exit_at %d must be >= 0", exit_at);
+  LlmState* ls = static_cast<LlmState*>(m->llm_state);
+  const DecodeState& st = p->k.st;
+  const int N = p->n_slots;
+  // h_flag: [0] n_active, [1] the step counter before the segment, [2] after it
+  FO1_CUDA(cudaMemcpyAsync(ls->h_flag, st.n_active, sizeof(int), cudaMemcpyDeviceToHost, s));
+  FO1_CUDA(cudaMemcpyAsync(ls->h_flag + 1, st.step, sizeof(int), cudaMemcpyDeviceToHost, s));
+  FO1_CUDA(cudaStreamSynchronize(s));
+  const int step0 = ls->h_flag[1];
+  if (ls->h_flag[0] > exit_at) {
+    // a running slot finishes within max_new steps (its own limit), so a segment needs at most that many
+    fo1_generate_desc d{};
+    d.n_seqs = N; d.max_new_tokens = p->k.max_new + 1; d.early_exit_interval = p->interval; d.pad_id = p->k.pad_id;
+    GenerateCall q{};
+    q.d = &d; q.mode = p->mode; q.k = p->k; q.pool = p; q.exit_at = exit_at;
+    DecodeBufs g;
+    m->arena.reset(true);
+    slots_decode_bufs(m, *p, g);
+    FO1_TRY(arena_ensure(m, m->arena.peak));
+    m->arena.reset(false);
+    slots_decode_bufs(m, *p, g);
+    if (g.mega_grid > 0) FO1_TRY(decode_persistent(m, q, g, s));
+    else FO1_TRY(decode_per_kernel(m, q, g, s));
+  }
+  std::vector<int> fin(N);
+  FO1_CUDA(cudaMemcpyAsync(ls->h_flag + 2, st.step, sizeof(int), cudaMemcpyDeviceToHost, s));
+  FO1_CUDA(cudaMemcpyAsync(fin.data(), st.finished, (size_t)N * sizeof(int), cudaMemcpyDeviceToHost, s));
+  FO1_CUDA(cudaStreamSynchronize(s));
+  for (int b = 0; b < N; ++b)
+    if (fin[b]) p->busy[b] = 0;
+  *steps_run = ls->h_flag[2] - step0;
+  return FO1_OK;
 }
 
 // -------------------------------------------------------------------------------- splice plan (host, integer)
@@ -1208,6 +1439,29 @@ extern "C" int fo1_llm_generate_lookup(fo1_model* m, fo1_generate_desc* d, const
   FO1_TRY(lookup_check(d, lk));
   if (px) FO1_TRY(prefix_check(d, px));
   return llm_generate(m, d, sp, sc, nullptr, static_cast<cudaStream_t>(stream), px, nullptr, lk);
+}
+
+extern "C" int fo1_slots_open(fo1_model* m, const fo1_slots_desc* o, void* stream) {
+  FO1_CHECK_ARG(m && o, "fo1_slots_open: null argument");
+  return slots_open(m, o, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int fo1_slots_admit(fo1_model* m, const fo1_slots_admit_desc* a, void* stream) {
+  FO1_CHECK_ARG(m && a, "fo1_slots_admit: null argument");
+  return slots_admit(m, a, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int fo1_slots_decode(fo1_model* m, int32_t exit_at, int32_t* steps_run, void* stream) {
+  FO1_CHECK_ARG(m && steps_run, "fo1_slots_decode: null argument");
+  return slots_decode(m, exit_at, steps_run, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int fo1_slots_close(fo1_model* m) {
+  FO1_CHECK_ARG(m, "fo1_slots_close: null argument");
+  FO1_CHECK_ARG(m->slot_pool != nullptr, "fo1_slots_close: no slot pool is open");
+  FO1_CUDA(cudaDeviceSynchronize());
+  slots_free(m);
+  return FO1_OK;
 }
 
 extern "C" int32_t fo1_stream_progress(const int32_t* progress) { return __atomic_load_n(progress, __ATOMIC_ACQUIRE); }

@@ -516,6 +516,62 @@ def _engine_generate_beam(self, inputs_embeds, position_ids, seq_lens, rope_delt
     return out
 
 
+class SlotPool:
+    """In-flight batching over the engine (include/fo1.h, fo1_slots_*): ``n_slots`` K/V cache slots of ``cap`` rows and their decode
+    state live across calls.  ``admit`` prefills requests into free slots, ``decode(exit_at)`` decodes every slot until at most
+    ``exit_at`` requests still run, and a finished slot's row of ``tokens`` int32 [n_slots, max_new_tokens] / ``lens`` /
+    ``finished`` (device) stays valid until the slot is admitted again.  Each request's tokens and length equal those of a static
+    Engine.generate of ``n_slots`` sequences on the same decode path.  While the pool is open, Engine.generate raises."""
+
+    def __init__(self, engine: Engine, n_slots: int, cap: int, max_new_tokens: int, stop_ids: Sequence[int], pad_id: int,
+                 sampled: bool = False, early_exit_interval: int = 8):
+        dev = engine.device
+        self.eng, self.n_slots, self.cap, self.max_new_tokens = engine, int(n_slots), int(cap), int(max_new_tokens)
+        self.tokens = torch.empty((self.n_slots, self.max_new_tokens), dtype=torch.int32, device=dev)
+        self.lens = torch.zeros((self.n_slots,), dtype=torch.int32, device=dev)
+        self.finished = torch.ones((self.n_slots,), dtype=torch.int32, device=dev)
+        st = (C.c_int32 * max(len(stop_ids), 1))(*[int(x) for x in stop_ids])
+        d = _lib.SlotsDesc(self.n_slots, self.cap, self.max_new_tokens, st, len(stop_ids), int(pad_id), int(bool(sampled)),
+                           int(early_exit_interval), self.tokens.data_ptr(), self.lens.data_ptr(), self.finished.data_ptr())
+        check(lib().fo1_slots_open(engine._h, C.byref(d), _stream()), "fo1_slots_open")
+        self.open = True
+
+    def admit(self, slots: Sequence[int], inputs_embeds: torch.Tensor, position_ids: torch.Tensor, seq_lens: Sequence[int],
+              rope_deltas: torch.Tensor, max_new_tokens: Sequence[int], sampling: Optional[Sampling] = None) -> None:
+        """Prefill len(slots) requests (packed bf16 embeddings [sum L, hidden], int32 positions [3, sum L], device int32 rope deltas
+        [n]) into ``slots`` and record their column 0; ``max_new_tokens`` and ``sampling`` per request."""
+        n = len(slots)
+        emb = inputs_embeds.contiguous()
+        pos = position_ids.to(self.eng.device, torch.int32).contiguous()
+        rd = rope_deltas.to(self.eng.device, torch.int32).contiguous()
+        assert emb.dtype == torch.bfloat16 and emb.shape == (int(sum(seq_lens)), self.eng.cfg.llm["hidden_size"])
+        assert pos.shape == (3, emb.shape[0]) and rd.numel() == n and len(seq_lens) == n and len(max_new_tokens) == n
+        sd = keep = None
+        if sampling is not None:
+            sd, keep = _lib.sampling_desc(sampling.temperature, sampling.top_p, sampling.top_k, sampling.seed)
+        a = _lib.SlotsAdmitDesc(n, (C.c_int32 * n)(*[int(x) for x in slots]), (C.c_int32 * n)(*[int(x) for x in seq_lens]), emb.data_ptr(),
+                                pos.data_ptr(), rd.data_ptr(), (C.c_int32 * n)(*[int(x) for x in max_new_tokens]),
+                                C.pointer(sd) if sd is not None else None)
+        check(lib().fo1_slots_admit(self.eng._h, C.byref(a), _stream()), "fo1_slots_admit")
+
+    def decode(self, exit_at: int) -> int:
+        """Decode until at most ``exit_at`` requests run; -> the decode steps run (synchronises)."""
+        steps = C.c_int32()
+        check(lib().fo1_slots_decode(self.eng._h, int(exit_at), C.byref(steps), _stream()), "fo1_slots_decode")
+        return steps.value
+
+    def close(self) -> None:
+        if self.open:
+            self.open = False
+            check(lib().fo1_slots_close(self.eng._h), "fo1_slots_close")
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+
 def prefix_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, prefix_lens: Sequence[int], own_lens: Sequence[int],
                      q_heads: int, kv_heads: int, scale: float) -> torch.Tensor:
     """fo1_prefix_attention: own rows q bf16 [sum own, q_heads * 128] (pitch = row stride) against the caches bf16 [n, cap, kv_heads * 128]:

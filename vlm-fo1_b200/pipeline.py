@@ -8,14 +8,15 @@
 One image per sample (what every caller in the reference does).  torch is the memory / stream plumbing."""
 from __future__ import annotations
 
+from collections import deque
 from dataclasses import dataclass
-from typing import Dict, List, Optional, Sequence, Tuple
+from typing import Callable, Dict, Iterator, List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
 
 from . import hfre as HF
-from .engine import Engine, Prefix, splice_plan, splice_plan_batch
+from .engine import Engine, Prefix, Sampling, SlotPool, splice_plan, splice_plan_batch
 
 
 @dataclass
@@ -92,6 +93,42 @@ def shared_prefix_groups(prompts: Sequence[Sequence[int]], rep: Sequence[int], i
         if P >= 1:
             out.append((mem, P))
     return out
+
+
+def refill_need(n_slots: int, n_waiting: int) -> int:
+    """Free slots at which a slot pool is refilled: a quarter of the pool, or the whole queue when it is shorter, so that the last
+    requests are admitted as soon as there is room for them instead of waiting for a quarter of the pool to drain (0: empty queue)."""
+    return min(max(1, n_slots // 4), n_waiting)
+
+
+def run_slots(n_items: int, n_slots: int, admit: Callable[[List[int], List[int]], List[int]], decode: Callable[[int], int],
+              poll: Callable[[], Tuple[Sequence[int], Sequence[int]]]) -> Iterator[Tuple[int, int, int]]:
+    """The host loop of in-flight batching over a slot pool, items in queue order 0 .. n_items - 1, free slots lowest first.
+    ``admit(items, slots)`` prefills the items into the slots and returns the items it admitted (a refused one is skipped and
+    frees its slot); ``decode(exit_at)`` decodes until at most exit_at requests run; ``poll()`` -> (finished flag, length) per
+    slot.  Yields (item, slot, length) in completion order (slot order within one segment); the slot's outputs are valid until the
+    generator is resumed."""
+    waiting = deque(range(n_items))
+    free = list(range(n_slots))
+    running: Dict[int, int] = {}
+    while waiting or running:
+        if waiting and len(free) >= refill_need(n_slots, len(waiting)):
+            k = min(len(free), len(waiting))
+            items, slots = [waiting.popleft() for _ in range(k)], free[:k]
+            done = set(admit(items, slots))
+            for it, b in zip(items, slots):
+                if it in done:
+                    running[b] = it
+            free = sorted(set(free) - set(running))
+            if not running:
+                continue
+        decode(n_slots - refill_need(n_slots, len(waiting)) if waiting else 0)
+        fin, lens = poll()
+        for b in sorted(running):
+            if fin[b]:
+                yield running.pop(b), b, int(lens[b])
+                free.append(b)
+        free.sort()
 
 
 class Fo1Pipeline:
@@ -339,3 +376,83 @@ class Fo1Pipeline:
         self._mark("llm_prefill_decode")
         out["prompt_lens"] = lens
         return out
+
+    # ---- in-flight batching ---------------------------------------------------------------------------------
+    def prompt_rows(self, s: SampleInputs, image_placeholder: int = -200) -> int:
+        """Prompt rows of a sample after the splice: exact for processor outputs, and for a uint8 image the rows of the largest image the
+        processors produce (2048 x 2048 px)."""
+        v = self.eng.cfg.vit
+        unit = v["spatial_merge_size"] ** 2
+        n_ph = sum(1 for t in s.input_ids if t == image_placeholder)
+        if s.grid_hw is not None:
+            rows = s.grid_hw[0] * s.grid_hw[1] // unit
+        else:
+            side = 2048 // (v["patch_size"] * v["spatial_merge_size"])
+            rows = side * side
+        return len(s.input_ids) - n_ph + min(n_ph, 1) * rows
+
+    def generate_continuous(self, samples: Sequence[SampleInputs], n_slots: int, max_new_tokens, stop_ids: Sequence[int],
+                            pad_id: int = 151643, sampling: Optional[Sampling] = None, early_exit_interval: int = 8,
+                            on_error: Optional[Callable[[int, BaseException], None]] = None) -> Iterator[Tuple[int, torch.Tensor, int]]:
+        """Every sample through a slot pool of ``n_slots`` slots (engine.SlotPool): a finished request hands its slot to the next
+        waiting one.  ``max_new_tokens``: one int, or one per sample; ``sampling``: None (greedy) or one parameter set per sample.
+        Yields (index, tokens int32 [n] on the device, n) in completion order.  Each request's tokens and length equal those of a
+        static generate() of ``n_slots`` samples on the same decode path (at most 8 slots on the persistent kernel, or 16 on the
+        per-kernel path of a 132-SM H100: those of generate() alone).  Admission groups are encoded together (equal images share the
+        towers); a group that fails is retried request by request, and a request that still fails is passed to ``on_error(index,
+        exception)`` and skipped (without ``on_error`` the exception propagates)."""
+        B = len(samples)
+        if B == 0:
+            return
+        mnt = [int(max_new_tokens)] * B if isinstance(max_new_tokens, int) else [int(x) for x in max_new_tokens]
+        assert len(mnt) == B and min(mnt) >= 1, "one max_new_tokens >= 1 per sample"
+        assert sampling is None or len(sampling.temperature) == B, "one sampling parameter set per sample"
+        T = max(mnt)
+        cap = max(self.prompt_rows(s) + m for s, m in zip(samples, mnt))
+        eng, dev = self.eng, self.eng.device
+        merge = eng.cfg.vit["spatial_merge_size"]
+        pool = SlotPool(eng, n_slots, cap, T, stop_ids, pad_id, sampled=sampling is not None, early_exit_interval=early_exit_interval)
+
+        def admit_group(items, slots):
+            group = self.preprocess([samples[i] for i in items])
+            rep = encoder_groups(group) if self._share_inputs and len(group) > 1 else list(range(len(group)))
+            own = [b for b in range(len(group)) if rep[b] == b]
+            slot_of = {b: i for i, b in enumerate(own)}
+            feats, _, region_tokens, _ = self.encode([group[b] for b in own])
+            grids = [group[rep[b]].grid_hw for b in range(len(group))]
+            plan = splice_plan_batch([s.input_ids for s in group], [[g] for g in grids],
+                                     [region_tokens[slot_of[rep[b]]].shape[0] for b in range(len(group))], dev, merge=merge,
+                                     row_src=rep, **self.ids)
+            st = plan["status"].cpu().tolist()
+            if any(st):
+                raise ValueError(f"fo1_splice_plan_batch: per-sample status {st} (placeholders and features disagree)")
+            embeds = eng.build_embeds(plan["kind"], plan["index"], feats, torch.cat(region_tokens, 0))
+            sp = None
+            if sampling is not None:
+                sp = Sampling(*([list(f)[i] for i in items] for f in (sampling.temperature, sampling.top_p, sampling.top_k, sampling.seed)))
+            pool.admit(slots, embeds, plan["position_ids"], plan["lens"], plan["rope_delta"], [mnt[i] for i in items], sampling=sp)
+
+        def admit(items, slots):
+            try:
+                admit_group(items, slots)
+                return items
+            except Exception:
+                if on_error is None:
+                    raise
+            done = []
+            for it, b in zip(items, slots):        # the group failed: each request alone, the failing ones reported and skipped
+                try:
+                    admit_group([it], [b])
+                    done.append(it)
+                except Exception as exc:  # noqa: BLE001 -- handed to the caller's on_error
+                    on_error(it, exc)
+            return done
+
+        def poll():
+            return pool.finished.cpu().tolist(), pool.lens.cpu().tolist()
+
+        try:
+            for it, b, n in run_slots(B, n_slots, admit, pool.decode, poll):
+                yield it, pool.tokens[b, :n].clone(), n
+        finally:
+            pool.close()

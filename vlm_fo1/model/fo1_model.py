@@ -334,6 +334,41 @@ class Fo1ForCausalLM:
             res.append((r, out["logprobs"][b:b + 1, :out["lens"][b]]) if output_logprobs else r)
         return res
 
+    @torch.no_grad()
+    def generate_iter(self, kwargs_iterable, batch_size=16, on_error=None):
+        """In-flight batching: the dicts ``prepare_inputs`` returns (as ``generate_batch`` takes them) through ``batch_size`` decode
+        slots; a finished sample hands its slot to the next one.  Yields (i, LongTensor [1, P_i + T_i]) in completion order, each
+        honouring its own ``max_new_tokens`` as ``generate(**kw)`` does, and equal to that sample's row in a static batch of
+        ``batch_size`` samples on the same decode path (at most 8 slots on the persistent kernel: ``generate(**kw)`` alone).  Seeds
+        are drawn from torch's generator in sample order.  ``on_error(i, exception)``: a sample whose admission fails is reported
+        there and skipped (without it the exception propagates).  Scores, streaming, beams, prompt lookup and
+        num_return_sequences > 1 are refused with NotImplementedError."""
+        batch = list(kwargs_iterable)
+        if not batch:
+            return
+        for kw in batch:
+            if self._outputs(kw) is not None:
+                raise NotImplementedError("return_dict_in_generate is not supported by generate_iter (it returns token ids)")
+            if kw.get("streamer") is not None:
+                raise NotImplementedError("streamer is not supported by generate_iter")
+            if self._beams(kw.get("do_sample", False), kw) is not None or int(kw.get("num_beams") or 1) > 1:
+                raise NotImplementedError("num_beams > 1 is not supported by generate_iter")
+            if self._lookup(kw) is not None:
+                raise NotImplementedError("prompt_lookup_num_tokens is not supported by generate_iter")
+            if self._num_return_sequences(kw) != 1:
+                raise NotImplementedError("num_return_sequences > 1 is not supported by generate_iter")
+        keys = ("inputs", "images", "images_aux", "image_grid_thws", "bbox_list", "do_sample", "temperature", "stopping_criteria", "top_p",
+                "top_k") + tuple(n for n, _ in _UNSUPPORTED_PROCESSORS)
+        samples, stops, samps = zip(*(self._sample(**{k: v for k, v in kw.items() if k in keys}) for kw in batch))
+        stop = sorted(set(x for s in stops for x in s))
+        pads = [kw.get("pad_token_id") for kw in batch]
+        pad = pads[0] if pads[0] is not None else (stop[0] if stop else 0)
+        mnt = [int(kw.get("max_new_tokens", 512)) for kw in batch]
+        for i, tokens, n in self.pipeline.generate_continuous(list(samples), int(batch_size), mnt, stop, pad_id=int(pad), early_exit_interval=8,
+                                                             sampling=self._sampling(samps), on_error=on_error):
+            inputs = batch[i]["inputs"]
+            yield i, torch.cat([inputs[0].to(tokens.device), tokens.to(torch.long)]).unsqueeze(0)
+
     def _generate_batch_beams(self, batch, beams, wants, max_new_tokens, output_logprobs):
         """generate_batch of beam-search samples: one packed engine call when every sample asks for the same beam setting.  With
         ``output_logprobs`` each element carries fp32 [num_return, T], the returned tokens' log-probabilities gathered along their
