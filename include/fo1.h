@@ -569,6 +569,58 @@ int fo1_lookup_drafts(const int32_t* corpus, int64_t ld, const int32_t* lens, in
                       int32_t* n_draft, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Logits processors (HF generate's sequence_bias, no_repeat_ngram_size, bad_words_ids, min_length, min_new_tokens, suppress_tokens
+ * and begin_suppress_tokens: transformers' GenerationMixin._get_logits_processor).  Before a column's token is chosen, the row of a
+ * sequence with a processor set is edited in place, in HF's order
+ *   SequenceBias -> NoRepeatNGram -> NoBadWords -> MinLength -> MinNewTokensLength -> SuppressTokens -> SuppressTokensAtBegin,
+ * over HF's input_ids: the sequence's prompt ids as the caller passes them (placeholders included), then the tokens it has emitted.
+ *   sequence_bias: a sequence of length 1 always adds its bias to its token; a longer one adds it to its last token when the history
+ *                  ends with the others.  A token's biases are summed in fp32 from 0, the length-1 bias first, then the longer
+ *                  sequences in their given order, and the sum is added once.
+ *   bad words:     the same match; the last token becomes -inf.
+ *   no_repeat_ngram_size n: with L history ids and L + 1 >= n, every earlier n-gram whose first n - 1 ids equal the last n - 1
+ *                  history ids bans its last id (-inf; a negative prompt id bans vocab + id, as torch indexing wraps it).
+ *   min_length:    the eos ids are -inf while L < min_length (the prompt counts).  min_new_tokens: while the column < min_new_tokens.
+ *   suppress:      always -inf.  begin_suppress: -inf at column 0.
+ * Column 0, drawn from the prefill's last row, is processed too.  A row without a set is never edited: its outputs are bit-identical
+ * to the same call without processors.  Scores: `logits` stays the raw row, `scores` is the processed one (then the sampler's cut),
+ * and the log-probabilities are those of the processed row.  A row that ends up all -inf (every token banned) draws token 0, the
+ * arg-max rule, on every path, greedy or sampled; nothing is kept, so its log-probability is -inf.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct {
+  int32_t n_sets;                          /* >= 1 processor sets, each used by any number of sequences */
+  const int32_t* seq_set;                  /* HOST [n_seqs]: the sequence's set, or -1 (no processors) */
+  const int32_t* prompt;                   /* HOST: the sequences' prompt ids packed, each in [-vocab, vocab) */
+  const int32_t* prompt_offsets;           /* HOST [n_seqs + 1]: prompt b is prompt[offsets[b] .. offsets[b + 1]), offsets[0] == 0 */
+  const int32_t* no_repeat_ngram_size;     /* HOST [n_sets]: >= 0 (0: off) */
+  const int32_t* min_length;               /* HOST [n_sets]: >= 0 (0: off) */
+  const int32_t* min_new_tokens;           /* HOST [n_sets]: >= 0 (0: off) */
+  /* id lists of set s: ids[offsets[s] .. offsets[s + 1]), each offsets array HOST [n_sets + 1], non-decreasing, <= n_ids */
+  const int32_t* eos_offsets;              /* the eos ids MinLength / MinNewTokens mask (HF's eos_token_id, not the stop list) */
+  const int32_t* suppress_offsets;
+  const int32_t* begin_suppress_offsets;
+  /* token sequences of set s: sequences [offsets[s] .. offsets[s + 1]), each offsets array HOST [n_sets + 1], non-decreasing,
+   * <= n_sequences; sequence k is ids[seq_offsets[k] .. seq_offsets[k + 1]) (non-empty) */
+  const int32_t* bias_offsets;             /* sequence_bias, in its given order */
+  const int32_t* bad_offsets;              /* bad_words_ids */
+  int32_t n_sequences;
+  const int32_t* seq_offsets;              /* HOST [n_sequences + 1], non-decreasing, <= n_ids */
+  const float* bias;                       /* HOST [n_sequences]: the bias of each sequence_bias sequence, finite (bad words: unread) */
+  int32_t n_ids;
+  const int32_t* ids;                      /* HOST [n_ids]: token ids in [0, vocab) */
+} fo1_processor_desc;
+/* fo1_llm_generate_prefixed with logits processors; pr == NULL, or no sequence with a set, is exactly fo1_llm_generate_prefixed.
+ * Checked on the host before any launch: the ranges above.  A greedy call with processors chooses through the sampler with top_k 1
+ * (bit-identical to the arg-max), on the persistent kernel too.  Beam search and prompt lookup take no processors. */
+int fo1_llm_generate_processed(fo1_model* m, fo1_generate_desc* d, const fo1_prefix_desc* px /* NULL */, const fo1_sampling_desc* sp /* NULL: greedy */,
+                               const fo1_score_desc* sc /* NULL: unscored */, const fo1_stream_desc* st /* NULL: not streamed */,
+                               const fo1_processor_desc* pr /* NULL: none */, void* stream);
+/* The row routine alone: rows [n_rows] of fp32 logits (DEVICE, pitch ld) edited in place; row r is sequence r of pr at output column
+ * cols[r] (HOST), its emitted tokens outputs[r][0 .. cols[r]) (DEVICE, pitch ld_out; may be NULL when every column is 0). */
+int fo1_logits_process(float* logits, int64_t ld, int32_t n_rows, int32_t vocab, const fo1_processor_desc* pr, const int32_t* outputs,
+                       int64_t ld_out, const int32_t* cols, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Slot pool: in-flight batching of many requests (replaces the reference callers' one-image-at-a-time generate loop,
  * eval_coco.py:36-88 / eval_countbench.py:30-60, for a whole request list).  n_slots K/V cache slots and decode-state rows live
  * across calls; the host repeats: admit waiting requests into free slots (fo1_slots_admit), decode every slot until at most exit_at
@@ -605,6 +657,8 @@ typedef struct {
   const int32_t* rope_deltas_device;     /* DEVICE int32 [n] (what fo1_splice_plan_batch wrote) */
   const int32_t* max_new_tokens;         /* HOST [n]: each request's own limit, 1 .. the pool's max_new_tokens */
   const fo1_sampling_desc* sampling;     /* NULL: greedy; else per request (a pool opened with sampled = 1) */
+  const fo1_processor_desc* processors;  /* NULL: none; else per request, checked as fo1_llm_generate_processed checks it.  The
+                                            pool keeps each admitted request's set and prompt ids until its slot is admitted again. */
 } fo1_slots_admit_desc;
 /* Prefills the n requests into their slots (the prefill of fo1_llm_generate with the slots as the cache-write members) and records
  * column 0.  Checked on the host before any launch: slot in range, slot free (never admitted, or seen finished by the last

@@ -115,11 +115,21 @@ class SlotsDesc(C.Structure):
                 ("out_tokens", C.c_void_p), ("out_lens", C.c_void_p), ("finished", C.c_void_p)]
 
 
+class ProcessorDesc(C.Structure):
+    """fo1_processor_desc: every array HOST; per sequence its set (-1: none) and prompt ids, per set its settings and id lists."""
+    _fields_ = [("n_sets", C.c_int32), ("seq_set", C.POINTER(C.c_int32)), ("prompt", C.POINTER(C.c_int32)),
+                ("prompt_offsets", C.POINTER(C.c_int32)), ("no_repeat_ngram_size", C.POINTER(C.c_int32)), ("min_length", C.POINTER(C.c_int32)),
+                ("min_new_tokens", C.POINTER(C.c_int32)), ("eos_offsets", C.POINTER(C.c_int32)), ("suppress_offsets", C.POINTER(C.c_int32)),
+                ("begin_suppress_offsets", C.POINTER(C.c_int32)), ("bias_offsets", C.POINTER(C.c_int32)), ("bad_offsets", C.POINTER(C.c_int32)),
+                ("n_sequences", C.c_int32), ("seq_offsets", C.POINTER(C.c_int32)), ("bias", C.POINTER(C.c_float)), ("n_ids", C.c_int32),
+                ("ids", C.POINTER(C.c_int32))]
+
+
 class SlotsAdmitDesc(C.Structure):
     """fo1_slots_admit_desc: HOST slots / seq_lens / max_new_tokens [n]; DEVICE embeddings, positions [3][sum L], rope deltas [n]."""
     _fields_ = [("n", C.c_int32), ("slots", C.POINTER(C.c_int32)), ("seq_lens", C.POINTER(C.c_int32)), ("inputs_embeds", C.c_void_p),
                 ("position_ids", C.c_void_p), ("rope_deltas_device", C.c_void_p), ("max_new_tokens", C.POINTER(C.c_int32)),
-                ("sampling", C.POINTER(SamplingDesc))]
+                ("sampling", C.POINTER(SamplingDesc)), ("processors", C.POINTER(ProcessorDesc))]
 
 
 FO1_STREAM_DONE = 1 << 30
@@ -170,6 +180,12 @@ def lib() -> C.CDLL:
     L.fo1_llm_generate_prefixed.restype = C.c_int
     L.fo1_llm_generate_prefixed.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(PrefixDesc), C.POINTER(SamplingDesc), C.POINTER(ScoreDesc),
                                             C.POINTER(StreamDesc), C.c_void_p]
+    L.fo1_llm_generate_processed.restype = C.c_int
+    L.fo1_llm_generate_processed.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(PrefixDesc), C.POINTER(SamplingDesc), C.POINTER(ScoreDesc),
+                                             C.POINTER(StreamDesc), C.POINTER(ProcessorDesc), C.c_void_p]
+    L.fo1_logits_process.restype = C.c_int
+    L.fo1_logits_process.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.POINTER(ProcessorDesc), C.c_void_p, C.c_int64,
+                                     C.POINTER(C.c_int32), C.c_void_p]
     L.fo1_llm_generate_beam.restype = C.c_int
     L.fo1_llm_generate_beam.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(BeamDesc), C.c_void_p]
     L.fo1_llm_generate_lookup.restype = C.c_int

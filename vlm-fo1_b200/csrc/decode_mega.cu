@@ -592,9 +592,11 @@ __device__ __forceinline__ void mg_attention_phase(const MegaArgs& a, uint8_t* s
 // MODE (DecodeMode) DEC_GREEDY: the greedy loop.  DEC_SAMPLED: the head stores its logits, CTA b < B draws sequence b's token with
 // the row routine of sampling.cuh (one more grid barrier per step), CTA 0 records the drawn tokens.  DEC_SCORED: CTA b also scores
 // row b in the same phase -- one more pass over the row for Z_kept, the log-probability and the optional scores / logits rows (a
-// scored greedy call runs here with top_k = 1, which draws the arg-max).  STREAM: CTA 0 also mirrors each recorded column into the
+// scored greedy call runs here with top_k = 1, which draws the arg-max).  PROC (logits processors, a.proc): CTA b first edits row b
+// (processors.cuh), in both modes; a greedy call with processors runs DEC_SAMPLED with top_k = 1.  PROC is a template parameter so
+// that the calls without processors keep the registers and spills of the plain instantiations.  STREAM: CTA 0 also mirrors each recorded column into the
 // caller's mapped host buffers and publishes it (a.sink.stream), and honours the host's cancel flag.
-template <int MT, int MODE, bool STREAM>
+template <int MT, int MODE, bool STREAM, bool PROC>
 __global__ void __launch_bounds__(kMgThreads, 1) decode_mega_kernel(const MegaArgs a) {
   using Lay = MgLay<MT>;
   extern __shared__ __align__(128) uint8_t mg_smem[];
@@ -710,6 +712,12 @@ __global__ void __launch_bounds__(kMgThreads, 1) decode_mega_kernel(const MegaAr
         mg_wait<0>();
         SampleSmem<kMgThreads>& sm = *reinterpret_cast<SampleSmem<kMgThreads>*>(mg_smem);
         const int b = blockIdx.x;
+        if constexpr (PROC) {    // the logits processors on the row CTA b owns (nothing past the sequence's stop)
+          const int col = a.sink.col != nullptr ? __ldcg(a.sink.col + b) : __ldcg(a.sink.st.step);
+          if (col < a.sink.max_new && !__ldcg(a.sink.st.finished + b))
+            process_row<kMgThreads>(a.proc, b, col, a.logits + (long long)b * a.V, a.V, a.sink.out_tokens + (long long)b * a.sink.max_new,
+                                    MODE == DEC_SCORED && a.sc_logits != nullptr ? a.sc_logits + ((long long)col * a.B + b) * a.V : nullptr);
+        }
         if constexpr (MODE == DEC_SCORED) {
           const float* row = a.logits + (long long)b * a.V;
           const int step = __ldcg(a.sink.st.step);
@@ -718,7 +726,7 @@ __global__ void __launch_bounds__(kMgThreads, 1) decode_mega_kernel(const MegaAr
           if (step < a.sink.max_new && !__ldcg(a.sink.st.finished + b)) {       // past the sequence's stop nothing is recorded
             const long long o = ((long long)step * a.B + b) * a.V;
             const float lp = score_row<kMgThreads>(row, a.V, a.samp[b].temperature, tok, sm, a.sc_scores ? a.sc_scores + o : nullptr,
-                                                   a.sc_logits ? a.sc_logits + o : nullptr);
+                                                   a.sc_logits && !PROC ? a.sc_logits + o : nullptr);
             if (threadIdx.x == 0 && a.sc_logprobs != nullptr) a.sc_logprobs[(long long)b * a.sink.max_new + step] = lp;
           }
         } else {
@@ -780,10 +788,15 @@ __global__ void __launch_bounds__(kMgThreads, 1) decode_mega_kernel(const MegaAr
 namespace fo1 {
 
 // every instantiation, [MT - 1][DecodeMode][STREAM]
-#define MG_KERNELS(MT, MODE) {reinterpret_cast<void*>(decode_mega_kernel<MT, MODE, false>), reinterpret_cast<void*>(decode_mega_kernel<MT, MODE, true>)}
-static void* const kMgKernels[2][3][2] = {{MG_KERNELS(1, DEC_GREEDY), MG_KERNELS(1, DEC_SAMPLED), MG_KERNELS(1, DEC_SCORED)},
-                                          {MG_KERNELS(2, DEC_GREEDY), MG_KERNELS(2, DEC_SAMPLED), MG_KERNELS(2, DEC_SCORED)}};
+// every instantiation, [MT - 1][DecodeMode][STREAM][PROC]; a greedy call with processors runs DEC_SAMPLED, so the greedy loop has
+// no PROC instantiation (its slot repeats the plain one)
+#define MG_PAIR(MT, MODE, STREAM, P) {reinterpret_cast<void*>(decode_mega_kernel<MT, MODE, STREAM, false>), \
+                                      reinterpret_cast<void*>(decode_mega_kernel<MT, MODE, STREAM, P>)}
+#define MG_KERNELS(MT, MODE, P) {MG_PAIR(MT, MODE, false, P), MG_PAIR(MT, MODE, true, P)}
+static void* const kMgKernels[2][3][2][2] = {{MG_KERNELS(1, DEC_GREEDY, false), MG_KERNELS(1, DEC_SAMPLED, true), MG_KERNELS(1, DEC_SCORED, true)},
+                                             {MG_KERNELS(2, DEC_GREEDY, false), MG_KERNELS(2, DEC_SAMPLED, true), MG_KERNELS(2, DEC_SCORED, true)}};
 #undef MG_KERNELS
+#undef MG_PAIR
 
 int decode_mega_grid() {
   static int grid = -1;
@@ -793,7 +806,8 @@ int decode_mega_grid() {
     bool ok = cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev) == cudaSuccess && coop;
     for (const auto& per_mt : kMgKernels)
       for (const auto& per_mode : per_mt)
-        for (void* fn : per_mode)
+        for (const auto& per_stream : per_mode)
+          for (void* fn : per_stream)
           ok = ok && cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kMgSmemBytes) == cudaSuccess &&
                cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kMgThreads, kMgSmemBytes) == cudaSuccess && per_sm >= 1;
     if (ok)
@@ -876,6 +890,7 @@ int decode_mega_run(MegaArgs a, DecodeMode mode, cudaStream_t s) {
   FO1_CHECK_ARG(mode != DEC_SCORED || a.samp != nullptr, "decode_mega: scoring needs the per-row sampling parameters");
   FO1_CHECK_ARG(mode == DEC_GREEDY || (a.samp != nullptr && a.logits != nullptr && a.samp_tok != nullptr && (a.V & 1) == 0),
                 "decode_mega: sampling buffers missing");
+  FO1_CHECK_ARG(mode != DEC_GREEDY || a.proc.tab == nullptr, "decode_mega: logits processors run in the sampled or scored loop");
   const StreamArgs& sa = a.sink.stream;
   FO1_CHECK_ARG(sa.progress == nullptr || (sa.tokens != nullptr && sa.lens != nullptr), "decode_mega: stream buffers missing");
   const bool prof = getenv("FO1_MEGA_PROF") != nullptr;
@@ -890,7 +905,7 @@ int decode_mega_run(MegaArgs a, DecodeMode mode, cudaStream_t s) {
   {
     void* params[] = {&a};
     ProfScope ps("decode_mega", 0.0, 0.0, s);
-    FO1_CUDA(cudaLaunchCooperativeKernel(kMgKernels[a.B <= 16 ? 0 : 1][mode][sa.progress != nullptr], dim3(grid), dim3(kMgThreads), params,
+    FO1_CUDA(cudaLaunchCooperativeKernel(kMgKernels[a.B <= 16 ? 0 : 1][mode][sa.progress != nullptr][a.proc.tab != nullptr], dim3(grid), dim3(kMgThreads), params,
                                          kMgSmemBytes, s));
     count_launch();
   }

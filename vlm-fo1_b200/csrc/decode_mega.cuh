@@ -2,6 +2,7 @@
 #pragma once
 #include "engine.cuh"
 #include "decode_loop.cuh"
+#include "processors.cuh"
 #include "sampling.cuh"
 
 namespace fo1 {
@@ -40,6 +41,9 @@ struct MegaArgs {
   int* samp_tok;                    // [B] the token CTA b drew for sequence b
   // scored decoding (MODE DEC_SCORED; any may be nullptr): logprobs [B][max_new], scores / logits [max_new][B][V]
   float *sc_logprobs, *sc_scores, *sc_logits;
+  // logits processors (MODE DEC_SAMPLED or DEC_SCORED; proc.tab == nullptr: none): CTA b edits row b before it draws, and stores the
+  // raw row in sc_logits first
+  ProcArgs proc;
 };
 
 

@@ -500,7 +500,21 @@ struct SlotPool {
   int* ints = nullptr;              // col, max_new_row, then the admission's slots / max_new / 0 (n_slots each, + 1)
   SampleRowParams* prm = nullptr;   // [n_slots]
   std::vector<int> busy;            // host: admitted and not seen finished by the last fo1_slots_decode
+  // logits processors: the distinct sets the running requests use (host; an admission that brings a new set drops the ones no
+  // running slot uses, so they number at most n_slots + the admitted requests), their device table, and per slot its set, prompt
+  // length and prompt ids (proc.set_of / plen / prompt: `proc_ints`, [n_slots] + [n_slots] + [n_slots][cap]; slot_set mirrors
+  // set_of).  proc.tab stays nullptr until an admission brings a set; from then on a greedy pool decodes through the sampler with
+  // top_k 1 (bit-identical)
+  ProcArgs proc{};
+  int* proc_ints = nullptr;
+  std::vector<ProcSet> proc_sets;
+  std::map<std::vector<int>, int> proc_index;
+  std::vector<int> slot_set;
+  size_t proc_tab_cap = 0, proc_bias_cap = 0;
 };
+
+// the decode mode of a pool: a greedy pool with logits processors draws with top_k 1 from its stored logits rows
+static DecodeMode pool_mode(const SlotPool& p) { return p.mode == DEC_GREEDY && p.proc.tab != nullptr ? DEC_SAMPLED : p.mode; }
 
 // one generate call, described once by llm_generate: the caller's descriptors, the decode mode, the column sink, and the device state
 // of beam search (with its host table of length-penalty divisors) or of prompt lookup; or one admission into / decode segment of a
@@ -521,6 +535,11 @@ struct GenerateCall {
   SlotPool* pool;
   const int* slots;
   int exit_at;                      // the decode loop ends once at most this many sequences run (0: all stopped)
+  const fo1_processor_desc* pr;     // logits processors (null: none): `proc` on the device, uploaded from proc_ints / proc_bias
+  ProcArgs proc;
+  std::vector<int> proc_ints;       // the table, then set_of [B], plen [B], prompts [B][proc.ld]
+  std::vector<float> proc_bias;
+  size_t proc_tab_n;
 };
 
 // the scratch buffers of a decoder layer over packed rows
@@ -644,9 +663,16 @@ static int decode_column(const GenerateCall& q, const DecodeBufs& g, int B, int 
   const DecodeState& st = k.st;
   const fo1_score_desc* sc = q.sc;
   if (q.mode == DEC_BEAM) return beam_column(q.beam, g.logits, st, advance, s);
+  // the logits processors edit the rows first (scored: after storing the raw rows, which score_rows then leaves alone)
+  float* raw_out = q.mode == DEC_SCORED ? sc->logits : nullptr;
+  if (q.proc.tab != nullptr) {
+    FO1_TRY(logits_process(q.proc, g.logits, B, V, k.col != nullptr ? k.col : st.step, k.col != nullptr ? 1 : 0, nullptr, st.finished, k.max_new,
+                           k.out_tokens, raw_out, s));
+    raw_out = nullptr;
+  }
   if (q.mode == DEC_SCORED) {
     FO1_TRY(score_rows(g.logits, V, B, V, g.samp, st.step, st.new_tok, true, st.finished, k.max_new, sc->logprobs, k.max_new, sc->scores,
-                       sc->logits, V, s));
+                       raw_out, V, s));
   } else if (q.mode == DEC_SAMPLED) {
     // the Philox step is read from *st.step, or (slot pool) from each slot's own column
     FO1_TRY(sample_rows(g.logits, V, B, V, g.samp, k.col != nullptr ? k.col : st.step, k.col != nullptr ? 1 : 0, st.new_tok, s));
@@ -666,6 +692,7 @@ static int slots_admit_column(const GenerateCall& q, const DecodeBufs& g, int V,
   const SlotPool& p = *q.pool;
   const int n = q.d->n_seqs, N = p.n_slots;
   const int* adm = p.ints + 2 * N;        // slots [N], max_new [N], 0
+  if (q.pr != nullptr) FO1_TRY(logits_process(p.proc, g.logits, n, V, adm + 2 * N, 0, adm, nullptr, p.k.max_new, p.k.out_tokens, nullptr, s));
   if (p.mode == DEC_SAMPLED) {
     FO1_TRY(sample_rows(g.logits, V, n, V, g.samp, adm + 2 * N, 0, p.k.st.new_tok, s));
   } else {
@@ -788,6 +815,11 @@ static int llm_prefill(Model* m, GenerateCall& q, cudaStream_t s, bool dry, Deco
   g.samp_tok = q.mode == DEC_SAMPLED || q.mode == DEC_SCORED ? A.alloc<int>(B) : nullptr;
   if (beam) beam_alloc(A, q.beam);   // beam search: its state and scratch (sized by the dry run like everything else)
   if (lookup) lookup_alloc(A, q.lookup, q.lkd);
+  if (q.pr != nullptr && !q.pool) {
+    int* pi = A.alloc<int>(q.proc_ints.size());
+    q.proc.tab = pi; q.proc.set_of = pi + q.proc_tab_n; q.proc.plen = pi + q.proc_tab_n + B; q.proc.prompt = pi + q.proc_tab_n + 2 * B;
+    q.proc.bias = A.alloc<float>(q.proc_bias.size());
+  }
 
   // ---- integer tables and inputs ----
   PrefillAttn pa = {};
@@ -803,6 +835,10 @@ static int llm_prefill(Model* m, GenerateCall& q, cudaStream_t s, bool dry, Deco
       FO1_CUDA(cudaMemcpyAsync(const_cast<float*>(q.beam.lp_div), q.lp_div.data(), q.lp_div.size() * sizeof(float), cudaMemcpyHostToDevice, s));
     }
     if (lookup) FO1_TRY(lookup_upload(q.lookup, q.lkd, s));
+    if (q.pr != nullptr && !q.pool) {    // (pageable sources: each copy returns once staged)
+      FO1_CUDA(cudaMemcpyAsync(const_cast<int*>(q.proc.tab), q.proc_ints.data(), q.proc_ints.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+      FO1_CUDA(cudaMemcpyAsync(const_cast<float*>(q.proc.bias), q.proc_bias.data(), q.proc_bias.size() * sizeof(float), cudaMemcpyHostToDevice, s));
+    }
     if (q.mode == DEC_SAMPLED || q.mode == DEC_SCORED) {
       // a scored greedy call samples with top_k 1 (bit-identical to greedy) so that both paths score in the sampler's per-row pass
       std::vector<SampleRowParams> h(B);
@@ -879,6 +915,7 @@ static int decode_persistent(Model* m, const GenerateCall& q, const DecodeBufs& 
   a.amax_val = g.mg_amax_v; a.amax_idx = g.mg_amax_i; a.sink = q.k;
   a.logits = g.logits; a.samp = g.samp; a.samp_tok = g.samp_tok;
   if (q.sc) { a.sc_logprobs = q.sc->logprobs; a.sc_scores = q.sc->scores; a.sc_logits = q.sc->logits; }
+  a.proc = q.proc;
   a.n_steps = d->max_new_tokens - 1; a.exit_at = q.exit_at; a.bar = reinterpret_cast<unsigned*>(g.mg_sync);
   const int pairs = B * c.llm_kv_heads;
   a.n_splits = std::max(1, std::min(kMgMaxSplits, g.mega_grid / std::max(1, pairs)));
@@ -959,7 +996,7 @@ static int decode_per_kernel(Model* m, const GenerateCall& q, const DecodeBufs& 
   for (int step = 1; step < d->max_new_tokens; ++step) {
     if (gexec != nullptr) {
       if (cudaGraphLaunch(gexec, s) != cudaSuccess) { set_error("cudaGraphLaunch failed: %s", cudaGetErrorString(cudaGetLastError())); rc = FO1_ERR_CUDA; break; }
-      count_launch((uint64_t)c.llm_layers * 9 + (lookup ? 8 : 6));
+      count_launch((uint64_t)c.llm_layers * 9 + (lookup ? 8 : 6) + (q.proc.tab != nullptr ? 1 : 0));
     } else if (want_graph && step == 2) {
       cudaGraph_t graph = nullptr;
       if (cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
@@ -1056,8 +1093,15 @@ static int prefix_check(const fo1_generate_desc* d, const fo1_prefix_desc* px) {
 
 int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, const fo1_score_desc* sc, const fo1_stream_desc* stm,
                  cudaStream_t s, const fo1_prefix_desc* px = nullptr, const fo1_beam_desc* bmd = nullptr,
-                 const fo1_lookup_desc* lkd = nullptr) {
+                 const fo1_lookup_desc* lkd = nullptr, const fo1_processor_desc* pr = nullptr) {
   if (sc != nullptr && sc->logprobs == nullptr && sc->scores == nullptr && sc->logits == nullptr) sc = nullptr;   // nothing to score
+  if (pr) {       // no sequence with a set: the call without processors
+    FO1_CHECK_ARG(pr->seq_set != nullptr, "fo1_llm_generate_processed: null seq_set");
+    bool any = false;
+    for (int b = 0; b < d->n_seqs; ++b) any |= pr->seq_set[b] >= 0;
+    if (!any) pr = nullptr;
+  }
+  if (pr) FO1_TRY(proc_check(pr, d->n_seqs, m->cfg.llm_vocab, "fo1_llm_generate_processed"));
   // the per-sequence host arrays first: they are the caller's, and need neither the model nor the device
   if (sp) FO1_TRY(sampling_check(sp, d->n_seqs, sc ? "fo1_llm_generate_scored" : "fo1_llm_generate_sampled"));
   if (sc) FO1_TRY(raw_rows_check(sp, sc->raw_rows, d->n_seqs, "fo1_llm_generate_scored"));
@@ -1074,7 +1118,7 @@ int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, co
     max_len = std::max(max_len, d->seq_lens[b]);
   }
   GenerateCall q{};
-  q.d = d; q.px = px; q.sp = sp; q.sc = sc; q.stm = stm; q.bmd = bmd; q.lkd = lkd;
+  q.d = d; q.px = px; q.sp = sp; q.sc = sc; q.stm = stm; q.bmd = bmd; q.lkd = lkd; q.pr = pr;
   ColumnSink& k = q.k;
   if (stm) {
     FO1_TRY(stream_resolve(stm, &k.stream));
@@ -1084,7 +1128,25 @@ int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, co
   FO1_TRY(ensure_state(m, rows, d->n_stop_ids, &k.st));
   k.n_stop = d->n_stop_ids; k.pad_id = d->pad_id; k.max_new = d->max_new_tokens;
   k.out_tokens = d->out_tokens; k.out_lens = d->out_lens;
-  q.mode = bmd ? DEC_BEAM : sc ? DEC_SCORED : sp ? DEC_SAMPLED : DEC_GREEDY;
+  // a greedy call with logits processors draws with top_k 1 (bit-identical to the arg-max) from the stored, processed rows
+  q.mode = bmd ? DEC_BEAM : sc ? DEC_SCORED : sp || pr ? DEC_SAMPLED : DEC_GREEDY;
+  if (pr) {
+    std::vector<int> tab;
+    proc_table(proc_sets(pr), tab, q.proc_bias);
+    const int B = d->n_seqs;
+    long long ld = 1;
+    for (int b = 0; b < B; ++b) ld = std::max<long long>(ld, pr->prompt_offsets[b + 1] - pr->prompt_offsets[b]);
+    q.proc_tab_n = tab.size();
+    q.proc_ints = std::move(tab);
+    q.proc_ints.resize(q.proc_tab_n + 2 * B + (size_t)B * ld, 0);
+    for (int b = 0; b < B; ++b) {
+      const int o = pr->prompt_offsets[b], n = pr->prompt_offsets[b + 1] - o;
+      q.proc_ints[q.proc_tab_n + b] = pr->seq_set[b];
+      q.proc_ints[q.proc_tab_n + B + b] = n;
+      std::copy(pr->prompt + o, pr->prompt + o + n, q.proc_ints.begin() + q.proc_tab_n + 2 * B + (size_t)b * ld);
+    }
+    q.proc.ld = ld;
+  }
   // a shared-prefix call rounds the slot up to 64 rows: the cache-reading attention's last key tile stays inside the slot; a lookup
   // call's verify rows write up to K rows past the sequence's last position
   const int n_drafts = lkd ? std::min(lkd->num_tokens, kLookupMaxDrafts) : 0;
@@ -1138,6 +1200,9 @@ static void slots_free(Model* m) {
   if (!p) return;
   if (p->ints) cudaFree(p->ints);
   if (p->prm) cudaFree(p->prm);
+  if (p->proc_ints) cudaFree(p->proc_ints);
+  if (p->proc.tab) cudaFree(const_cast<int*>(p->proc.tab));
+  if (p->proc.bias) cudaFree(const_cast<float*>(p->proc.bias));
   delete p;
   m->slot_pool = nullptr;
 }
@@ -1197,6 +1262,91 @@ static int slots_open(Model* m, const fo1_slots_desc* o, cudaStream_t s) {
   return rc;
 }
 
+// an admission's processors: its sets join the pool's distinct sets (the device table is rebuilt when one is new), and each admitted
+// slot gets its set and prompt ids
+static int slots_proc_admit(SlotPool* p, const fo1_processor_desc* pr, const int* slots, int n, int cap, cudaStream_t s) {
+  const int N = p->n_slots;
+  if (p->proc_ints == nullptr) {
+    if (cudaMalloc(reinterpret_cast<void**>(&p->proc_ints), ((size_t)2 * N + (size_t)N * cap) * sizeof(int)) != cudaSuccess) {
+      cudaGetLastError();
+      set_error("fo1_slots_admit: out of device memory for the processors' prompt rows");
+      return FO1_ERR_CUDA;
+    }
+    p->slot_set.assign(N, -1);
+    p->proc.set_of = p->proc_ints; p->proc.plen = p->proc_ints + N; p->proc.prompt = p->proc_ints + 2 * N; p->proc.ld = cap;
+  }
+  const std::vector<ProcSet> sets = proc_sets(pr);
+  std::vector<std::vector<int>> keys;
+  bool fresh = p->proc.tab == nullptr;
+  for (const ProcSet& ps : sets) {
+    keys.push_back(ps.key());
+    fresh |= p->proc_index.count(keys.back()) == 0;
+  }
+  for (int i = 0; i < n; ++i) p->slot_set[slots[i]] = -1;
+  if (fresh) {
+    // keep the sets of the running slots (renumbered), then add the new ones
+    std::vector<int> remap(p->proc_sets.size(), -1);
+    std::vector<ProcSet> kept;
+    std::map<std::vector<int>, int> index;
+    for (int b = 0; b < N; ++b) {
+      int& g = p->slot_set[b];
+      if (g < 0 || !p->busy[b]) { g = -1; continue; }
+      if (remap[g] < 0) {
+        remap[g] = (int)kept.size();
+        index.emplace(p->proc_sets[g].key(), remap[g]);
+        kept.push_back(p->proc_sets[g]);
+      }
+      g = remap[g];
+    }
+    p->proc_sets = std::move(kept);
+    p->proc_index = std::move(index);
+  }
+  std::vector<int> global(sets.size());
+  for (size_t i = 0; i < sets.size(); ++i) {
+    auto it = p->proc_index.emplace(keys[i], (int)p->proc_sets.size());
+    if (it.second) p->proc_sets.push_back(sets[i]);
+    global[i] = it.first->second;
+  }
+  if (fresh) {
+    std::vector<int> tab;
+    std::vector<float> bias;
+    proc_table(p->proc_sets, tab, bias);
+    if (tab.size() > p->proc_tab_cap || bias.size() > p->proc_bias_cap) {
+      FO1_CUDA(cudaStreamSynchronize(s));       // an earlier admission's launches may still read the old table
+      if (p->proc.tab) cudaFree(const_cast<int*>(p->proc.tab));
+      if (p->proc.bias) cudaFree(const_cast<float*>(p->proc.bias));
+      p->proc.tab = nullptr; p->proc.bias = nullptr;
+      p->proc_tab_cap = std::max(tab.size(), 2 * p->proc_tab_cap);
+      p->proc_bias_cap = std::max(bias.size(), 2 * p->proc_bias_cap);
+      int* t = nullptr;
+      float* bb = nullptr;
+      FO1_CUDA(cudaMalloc(reinterpret_cast<void**>(&t), p->proc_tab_cap * sizeof(int)));
+      p->proc.tab = t;
+      FO1_CUDA(cudaMalloc(reinterpret_cast<void**>(&bb), p->proc_bias_cap * sizeof(float)));
+      p->proc.bias = bb;
+    }
+    FO1_CUDA(cudaMemcpyAsync(const_cast<int*>(p->proc.tab), tab.data(), tab.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    FO1_CUDA(cudaMemcpyAsync(const_cast<float*>(p->proc.bias), bias.data(), bias.size() * sizeof(float), cudaMemcpyHostToDevice, s));
+  }
+  for (int i = 0; i < n; ++i) {
+    const int b = slots[i], o = pr->prompt_offsets[i], len = pr->prompt_offsets[i + 1] - o;
+    p->slot_set[b] = pr->seq_set[i] >= 0 ? global[pr->seq_set[i]] : -1;
+    FO1_CUDA(cudaMemcpyAsync(const_cast<int*>(p->proc.plen) + b, &len, sizeof(int), cudaMemcpyHostToDevice, s));
+    if (len > 0)
+      FO1_CUDA(cudaMemcpyAsync(const_cast<int*>(p->proc.prompt) + (size_t)b * cap, pr->prompt + o, len * sizeof(int), cudaMemcpyHostToDevice, s));
+  }
+  // (pageable source: the copy returns once staged)
+  FO1_CUDA(cudaMemcpyAsync(const_cast<int*>(p->proc.set_of), p->slot_set.data(), N * sizeof(int), cudaMemcpyHostToDevice, s));
+  return FO1_OK;
+}
+
+// an admission without processors into a pool that has them: its slots get no set
+static int slots_proc_clear(SlotPool* p, const int* slots, int n, cudaStream_t s) {
+  for (int i = 0; i < n; ++i) p->slot_set[slots[i]] = -1;
+  FO1_CUDA(cudaMemcpyAsync(const_cast<int*>(p->proc.set_of), p->slot_set.data(), p->n_slots * sizeof(int), cudaMemcpyHostToDevice, s));
+  return FO1_OK;
+}
+
 static int slots_admit(Model* m, const fo1_slots_admit_desc* a, cudaStream_t s) {
   SlotPool* p = static_cast<SlotPool*>(m->slot_pool);
   FO1_CHECK_ARG(p != nullptr, "fo1_slots_admit: no slot pool is open");
@@ -1220,11 +1370,21 @@ static int slots_admit(Model* m, const fo1_slots_admit_desc* a, cudaStream_t s) 
                   "fo1_slots_admit: sequence %d: %d prompt rows + %d new tokens exceed the slot capacity %d", i, a->seq_lens[i],
                   a->max_new_tokens[i], m->kv_cap);
   }
+  const fo1_processor_desc* pr = a->processors;
+  if (pr) {
+    FO1_TRY(proc_check(pr, n, m->cfg.llm_vocab, "fo1_slots_admit"));
+    for (int i = 0; i < n; ++i)
+      FO1_CHECK_ARG(pr->prompt_offsets[i + 1] - pr->prompt_offsets[i] <= m->kv_cap, "fo1_slots_admit: sequence %d: %d prompt ids exceed the slot "
+                    "capacity %d", i, pr->prompt_offsets[i + 1] - pr->prompt_offsets[i], m->kv_cap);
+    FO1_TRY(slots_proc_admit(p, pr, a->slots, n, m->kv_cap, s));
+  } else if (p->proc.tab != nullptr) {
+    FO1_TRY(slots_proc_clear(p, a->slots, n, s));
+  }
   fo1_generate_desc d{};
   d.n_seqs = n; d.seq_lens = a->seq_lens; d.inputs_embeds = a->inputs_embeds; d.position_ids = a->position_ids;
   d.rope_deltas_device = a->rope_deltas_device; d.max_new_tokens = 1; d.pad_id = p->k.pad_id;
   GenerateCall q{};
-  q.d = &d; q.sp = a->sampling; q.mode = p->mode; q.k = p->k; q.pool = p; q.slots = a->slots;
+  q.d = &d; q.sp = a->sampling; q.mode = p->mode; q.k = p->k; q.pool = p; q.slots = a->slots; q.pr = pr;
   FO1_TRY(int_cache_trim(m));
   FO1_CUDA(cudaMemcpyAsync(p->ints + 2 * N, a->slots, n * sizeof(int), cudaMemcpyHostToDevice, s));
   FO1_CUDA(cudaMemcpyAsync(p->ints + 3 * N, a->max_new_tokens, n * sizeof(int), cudaMemcpyHostToDevice, s));
@@ -1243,7 +1403,7 @@ static void slots_decode_bufs(Model* m, const SlotPool& p, DecodeBufs& g) {
   g = DecodeBufs();
   g.mega_grid = mega_grid_for(m, p.n_slots);
   decode_bufs_alloc(m, g, p.n_slots, p.n_slots, p.n_slots);
-  g.samp = p.mode == DEC_SAMPLED ? p.prm : nullptr;
+  g.samp = pool_mode(p) == DEC_SAMPLED ? p.prm : nullptr;
   g.samp_tok = m->arena.alloc<int>(p.n_slots);
 }
 
@@ -1264,7 +1424,7 @@ static int slots_decode(Model* m, int exit_at, int* steps_run, cudaStream_t s) {
     fo1_generate_desc d{};
     d.n_seqs = N; d.max_new_tokens = p->k.max_new + 1; d.early_exit_interval = p->interval; d.pad_id = p->k.pad_id;
     GenerateCall q{};
-    q.d = &d; q.mode = p->mode; q.k = p->k; q.pool = p; q.exit_at = exit_at;
+    q.d = &d; q.mode = pool_mode(*p); q.k = p->k; q.pool = p; q.exit_at = exit_at; q.proc = p->proc;
     DecodeBufs g;
     m->arena.reset(true);
     slots_decode_bufs(m, *p, g);
@@ -1424,6 +1584,16 @@ extern "C" int fo1_llm_generate_prefixed(fo1_model* m, fo1_generate_desc* d, con
                 "progress are required; cancel may be NULL)");
   if (px) FO1_TRY(prefix_check(d, px));
   return llm_generate(m, d, sp, sc, st, static_cast<cudaStream_t>(stream), px);
+}
+
+extern "C" int fo1_llm_generate_processed(fo1_model* m, fo1_generate_desc* d, const fo1_prefix_desc* px, const fo1_sampling_desc* sp,
+                                          const fo1_score_desc* sc, const fo1_stream_desc* st, const fo1_processor_desc* pr, void* stream) {
+  if (px != nullptr && px->n_groups == 0) px = nullptr;
+  FO1_CHECK_ARG(m && d, "fo1_llm_generate_processed: null argument");
+  FO1_CHECK_ARG(st == nullptr || (st->tokens && st->lens && st->progress), "fo1_llm_generate_processed: null stream buffer (tokens, lens and "
+                "progress are required; cancel may be NULL)");
+  if (px) FO1_TRY(prefix_check(d, px));
+  return llm_generate(m, d, sp, sc, st, static_cast<cudaStream_t>(stream), px, nullptr, nullptr, pr);
 }
 
 extern "C" int fo1_llm_generate_beam(fo1_model* m, fo1_generate_desc* d, const fo1_beam_desc* bm, void* stream) {

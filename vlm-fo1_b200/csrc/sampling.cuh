@@ -24,6 +24,7 @@
 //   scores row: x where kept, -inf elsewhere (a raw row: the logits unchanged).
 //   logprob of token t: (x_t - x_max) - ln(Z_kept * 2^-40), Z_kept the order-free fixed-point sum of exp(x - x_max) over the kept
 //     set; -inf for a token outside it.  Like the token, it depends on (row, T, p, k, t) alone.
+//   A row of -inf only (the logits processors banned every token) draws token 0 and keeps nothing (log-probability -inf).
 // sample_row<NT, SMP_DRAW> is the sampler; SMP_DRAW_KEPT also leaves the kept set in SampleSmem (the draw is unchanged) and
 // SMP_KEPT stops before the draw; score_row then makes one pass over the row.
 #pragma once
@@ -250,6 +251,13 @@ __device__ int sample_row(const float* __restrict__ row, int V, const SampleRowP
   for (int w = 1; w < NT / 32; ++w)
     if (sm.maxv[w] > bv || (sm.maxv[w] == bv && sm.maxi[w] < bi)) { bv = sm.maxv[w]; bi = sm.maxi[w]; }
   __syncthreads();
+  if (bv == -INFINITY) {     // every token banned by the logits processors: token 0 (the arg-max rule), nothing kept
+    if constexpr (MODE != SMP_DRAW) {
+      if (tid == 0) { sm.kept_key = 0xffffffffu; sm.kept_idx = -1; sm.kept_max = bv; }
+      __syncthreads();
+    }
+    return bi;
+  }
   if constexpr (MODE == SMP_DRAW) {
     if (prm.top_k == 1) return bi;
   }

@@ -297,6 +297,81 @@ class Lookup:
     corpus: Optional[Sequence[Sequence[int]]] = None
 
 
+@dataclass(frozen=True)
+class ProcessorSet:
+    """One sequence's logits processors (include/fo1.h, fo1_processor_desc), HF's semantics and order.  0 / empty: off.
+    ``eos_token_ids``: the ids MinLength and MinNewTokens mask (HF's eos_token_id, not the stop list).  ``sequence_bias``: ((ids,
+    bias), ...) in HF's dict order; ``bad_words_ids``: (ids, ...) with HF's eos filtering already applied."""
+    no_repeat_ngram_size: int = 0
+    min_length: int = 0
+    min_new_tokens: int = 0
+    eos_token_ids: Tuple[int, ...] = ()
+    suppress_tokens: Tuple[int, ...] = ()
+    begin_suppress_tokens: Tuple[int, ...] = ()
+    sequence_bias: Tuple[Tuple[Tuple[int, ...], float], ...] = ()
+    bad_words_ids: Tuple[Tuple[int, ...], ...] = ()
+
+
+@dataclass
+class Processors:
+    """Logits processors of a generate call: ``sets[b]``, sequence b's ProcessorSet or None (its rows are never edited), and
+    ``prompts[b]``, its prompt ids as the caller passes them (placeholders included; None: the pipeline fills in each sample's
+    ``input_ids``).  Equal sets are packed once."""
+    sets: Sequence[Optional[ProcessorSet]]
+    prompts: Optional[Sequence[Sequence[int]]] = None
+
+
+def _processor_desc(pr: Processors, B: int):
+    """(ProcessorDesc, keep-alive) of a call with B sequences; the sets deduplicated."""
+    if len(pr.sets) != B or pr.prompts is None or len(pr.prompts) != B:
+        raise ValueError(f"processors: {len(pr.sets)} sets / {None if pr.prompts is None else len(pr.prompts)} prompts for {B} sequences")
+    uniq, seq_set = {}, []
+    for s in pr.sets:
+        seq_set.append(-1 if s is None else uniq.setdefault(s, len(uniq)))
+    sets = list(uniq)
+    ids, bias = [], []
+    offs = {}
+    for key, get in (("eos", lambda s: s.eos_token_ids), ("sup", lambda s: s.suppress_tokens), ("bsup", lambda s: s.begin_suppress_tokens)):
+        offs[key] = [len(ids)]
+        for s in sets:
+            ids.extend(int(t) for t in get(s))
+            offs[key].append(len(ids))
+    # the sequence list: every set's bias sequences, then every set's bad words
+    seq_offsets = [len(ids)]
+    for key, get in (("bias", lambda s: s.sequence_bias), ("bad", lambda s: [(w, 0.0) for w in s.bad_words_ids])):
+        offs[key] = [len(bias)]
+        for s in sets:
+            for w, v in get(s):
+                ids.extend(int(t) for t in w)
+                seq_offsets.append(len(ids))
+                bias.append(float(v))
+            offs[key].append(len(bias))
+    flat = [int(t) for p in pr.prompts for t in p]
+    poff = [0]
+    for p in pr.prompts:
+        poff.append(poff[-1] + len(p))
+    i32 = lambda v: (C.c_int32 * max(len(v), 1))(*v)
+    S = len(sets)
+    keep = dict(seq_set=i32(seq_set), prompt=i32(flat), poff=i32(poff), ng=i32([s.no_repeat_ngram_size for s in sets]),
+                ml=i32([s.min_length for s in sets]), mn=i32([s.min_new_tokens for s in sets]), eos=i32(offs["eos"]), sup=i32(offs["sup"]),
+                bsup=i32(offs["bsup"]), bias_off=i32(offs["bias"]), bad_off=i32(offs["bad"]), seq_off=i32(seq_offsets),
+                bias=(C.c_float * max(len(bias), 1))(*bias), ids=i32(ids))
+    desc = _lib.ProcessorDesc(S, keep["seq_set"], keep["prompt"], keep["poff"], keep["ng"], keep["ml"], keep["mn"], keep["eos"], keep["sup"],
+                              keep["bsup"], keep["bias_off"], keep["bad_off"], len(bias), keep["seq_off"], keep["bias"], len(ids), keep["ids"])
+    return desc, keep
+
+
+def logits_process(logits: torch.Tensor, processors: Processors, outputs: Optional[torch.Tensor], cols: Sequence[int]) -> None:
+    """fo1_logits_process: the row routine alone.  ``logits`` fp32 [n, V] on the device, edited in place; row r is sequence r of
+    ``processors`` at output column ``cols[r]`` with emitted tokens ``outputs[r, :cols[r]]`` (int32 [n, >= max cols], device)."""
+    n, V = logits.shape
+    desc, _keep = _processor_desc(processors, n)
+    out = outputs.to(logits.device, torch.int32).contiguous() if outputs is not None else None
+    check(lib().fo1_logits_process(logits.data_ptr(), logits.stride(0), n, V, C.byref(desc), out.data_ptr() if out is not None else None,
+                                   out.stride(0) if out is not None else 0, (C.c_int32 * n)(*[int(c) for c in cols]), _stream()),
+          "fo1_logits_process")
+
+
 def _lookup_desc(lookup: Lookup, B: int, dev):
     """(LookupDesc, keep-alive, steps, accepted) of a call with B sequences."""
     corpus = lookup.corpus if lookup.corpus is not None else [[] for _ in range(B)]
@@ -337,7 +412,8 @@ def _engine_generate(self, inputs_embeds: torch.Tensor, position_ids: torch.Tens
                      sampling: Optional[Sampling] = None, want_logprobs: bool = False, want_scores: bool = False,
                      want_logits: bool = False, raw_rows: Optional[Sequence[int]] = None,
                      on_tokens: Optional[Callable[[int, int, "np.ndarray", "np.ndarray"], Optional[bool]]] = None,
-                     prefix: Optional[Prefix] = None, beams: Optional[Beams] = None, lookup: Optional[Lookup] = None):
+                     prefix: Optional[Prefix] = None, beams: Optional[Beams] = None, lookup: Optional[Lookup] = None,
+                     processors: Optional[Processors] = None):
     """Prefill + decode of a packed batch: greedy, or sampled per sequence when ``sampling`` is given.  position_ids int32
     [3, sum L].  Returns a dict of device tensors.
 
@@ -368,7 +444,13 @@ def _engine_generate(self, inputs_embeds: torch.Tensor, position_ids: torch.Tens
     length are bit-identical to the same call on the per-kernel path without lookup (FO1_NO_MEGA=1); against the persistent
     kernel (B <= 32 by default) they agree as any two decode paths do (DESIGN.md §2).  ``steps_run`` counts verify steps; added
     are ``lookup_steps`` / ``lookup_accepted`` int32 [B] (verify steps each sequence took part in, drafts it accepted).
-    Streaming and beams are refused."""
+    Streaming and beams are refused.
+
+    Logits processors (include/fo1.h, fo1_processor_desc): with ``processors``, each sequence's rows are edited by its ProcessorSet
+    before its token is chosen; a sequence without one is bit-identical to the call without processors.  ``logits`` stays raw,
+    ``scores`` and ``logprobs`` follow the processed rows.  Beams and lookup are refused."""
+    if processors is not None and (beams is not None or lookup is not None):
+        raise ValueError("logits processors do not combine with `beams` or `lookup`")
     if lookup is not None and (beams is not None or on_tokens is not None):
         raise ValueError("prompt lookup does not take `beams` or `on_tokens`")
     if beams is not None:
@@ -433,6 +515,11 @@ def _engine_generate(self, inputs_embeds: torch.Tensor, position_ids: torch.Tens
                              (C.c_int32 * B)(*[int(g) for g in prefix.seq_group]))
         px_arg = C.byref(px)
 
+    pr_arg = None
+    if processors is not None and any(x is not None for x in processors.sets):
+        prd, _pr_keep = _processor_desc(processors, B)
+        pr_arg = C.byref(prd)
+
     lk_out = None
     if lookup is not None:
         lk, _lk_keep, lk_steps, lk_acc = _lookup_desc(lookup, B, self.device)
@@ -442,6 +529,8 @@ def _engine_generate(self, inputs_embeds: torch.Tensor, position_ids: torch.Tens
         sa = C.byref(st) if st is not None else None
         if lookup is not None:
             check(L.fo1_llm_generate_lookup(self._h, C.byref(d), C.byref(lk), px_arg, sp_arg, sc_arg, stream), "fo1_llm_generate_lookup")
+        elif pr_arg is not None:
+            check(L.fo1_llm_generate_processed(self._h, C.byref(d), px_arg, sp_arg, sc_arg, sa, pr_arg, stream), "fo1_llm_generate_processed")
         elif px_arg is None:
             check(L.fo1_llm_generate_streamed(self._h, C.byref(d), sp_arg, sc_arg, sa, stream), "fo1_llm_generate_streamed")
         else:
@@ -537,9 +626,10 @@ class SlotPool:
         self.open = True
 
     def admit(self, slots: Sequence[int], inputs_embeds: torch.Tensor, position_ids: torch.Tensor, seq_lens: Sequence[int],
-              rope_deltas: torch.Tensor, max_new_tokens: Sequence[int], sampling: Optional[Sampling] = None) -> None:
+              rope_deltas: torch.Tensor, max_new_tokens: Sequence[int], sampling: Optional[Sampling] = None,
+              processors: Optional[Processors] = None) -> None:
         """Prefill len(slots) requests (packed bf16 embeddings [sum L, hidden], int32 positions [3, sum L], device int32 rope deltas
-        [n]) into ``slots`` and record their column 0; ``max_new_tokens`` and ``sampling`` per request."""
+        [n]) into ``slots`` and record their column 0; ``max_new_tokens``, ``sampling`` and ``processors`` per request."""
         n = len(slots)
         emb = inputs_embeds.contiguous()
         pos = position_ids.to(self.eng.device, torch.int32).contiguous()
@@ -552,6 +642,9 @@ class SlotPool:
         a = _lib.SlotsAdmitDesc(n, (C.c_int32 * n)(*[int(x) for x in slots]), (C.c_int32 * n)(*[int(x) for x in seq_lens]), emb.data_ptr(),
                                 pos.data_ptr(), rd.data_ptr(), (C.c_int32 * n)(*[int(x) for x in max_new_tokens]),
                                 C.pointer(sd) if sd is not None else None)
+        if processors is not None and any(x is not None for x in processors.sets):
+            prd, keep2 = _processor_desc(processors, n)
+            a.processors = C.pointer(prd)
         check(lib().fo1_slots_admit(self.eng._h, C.byref(a), _stream()), "fo1_slots_admit")
 
     def decode(self, exit_at: int) -> int:

@@ -16,7 +16,7 @@ import numpy as np
 import torch
 
 from . import hfre as HF
-from .engine import Engine, Prefix, Sampling, SlotPool, splice_plan, splice_plan_batch
+from .engine import Engine, Prefix, Processors, Sampling, SlotPool, splice_plan, splice_plan_batch
 
 
 @dataclass
@@ -288,19 +288,24 @@ class Fo1Pipeline:
     # ---- language side -----------------------------------------------------------------------------------
     def generate(self, samples: Sequence[SampleInputs], max_new_tokens: int, stop_ids: Sequence[int], pad_id: int = 151643,
                  early_exit_interval: int = 8, want_prefill_logits: bool = False, sampling=None, want_logprobs: bool = False,
-                 want_scores: bool = False, want_logits: bool = False, raw_rows=None, on_tokens=None, beams=None, lookup=None):
+                 want_scores: bool = False, want_logits: bool = False, raw_rows=None, on_tokens=None, beams=None, lookup=None,
+                 processors=None):
         """``sampling``: None (greedy) or an engine.Sampling with one parameter set per sample.  ``want_logprobs`` / ``want_scores`` /
         ``want_logits`` / ``raw_rows``: per-token scores, as Engine.generate.  ``on_tokens``: the streaming callback of
         Engine.generate (columns of the whole batch, in sample order).  ``beams``: an engine.Beams, beam search for every sample
         (Engine.generate's outputs); the towers still run once per unique image, but each prompt is prefilled in full.  ``lookup``: an
-        engine.Lookup, prompt-lookup decoding; without a corpus of its own, each sample's ``input_ids`` is its corpus (HF's)."""
+        engine.Lookup, prompt-lookup decoding; without a corpus of its own, each sample's ``input_ids`` is its corpus (HF's).
+        ``processors``: an engine.Processors, one ProcessorSet or None per sample; without prompts of its own, each sample's
+        ``input_ids`` is its history's prompt (HF's input_ids)."""
+        from dataclasses import replace
+        if processors is not None and processors.prompts is None:
+            processors = replace(processors, prompts=[list(s.input_ids) for s in samples])
         if lookup is not None and lookup.corpus is None:
-            from dataclasses import replace
             lookup = replace(lookup, corpus=[list(s.input_ids) for s in samples])
         eng, dev = self.eng, self.eng.device
         kw = dict(max_new_tokens=max_new_tokens, stop_ids=stop_ids, pad_id=pad_id, early_exit_interval=early_exit_interval,
                   want_prefill_logits=want_prefill_logits, sampling=sampling, want_logprobs=want_logprobs, want_scores=want_scores,
-                  want_logits=want_logits, raw_rows=raw_rows, on_tokens=on_tokens, beams=beams, lookup=lookup)
+                  want_logits=want_logits, raw_rows=raw_rows, on_tokens=on_tokens, beams=beams, lookup=lookup, processors=processors)
         if self._share_inputs and len(samples) > 1:
             rep = encoder_groups(samples)
             if any(r != b for b, r in enumerate(rep)):
@@ -323,13 +328,13 @@ class Fo1Pipeline:
         self._mark("splice")
         out = eng.generate(embeds, pos, lens, deltas, max_new_tokens, stop_ids, pad_id, want_prefill_logits=want_prefill_logits,
                            early_exit_interval=early_exit_interval, sampling=sampling, want_logprobs=want_logprobs, want_scores=want_scores,
-                           want_logits=want_logits, raw_rows=raw_rows, on_tokens=on_tokens, beams=beams, lookup=lookup)
+                           want_logits=want_logits, raw_rows=raw_rows, on_tokens=on_tokens, beams=beams, lookup=lookup, processors=processors)
         self._mark("llm_prefill_decode")
         out["prompt_lens"] = lens
         return out
 
     def _generate_shared(self, samples, rep, max_new_tokens, stop_ids, pad_id, early_exit_interval, want_prefill_logits, sampling,
-                         want_logprobs, want_scores, want_logits, raw_rows, on_tokens, beams, lookup):
+                         want_logprobs, want_scores, want_logits, raw_rows, on_tokens, beams, lookup, processors):
         """generate() of a batch in which some samples have equal encoder inputs: the towers run once per unique image, and each set's
         common prompt prefix is prefilled once (Engine.generate's ``prefix``).  Bit-identical to the unshared path."""
         eng, dev = self.eng, self.eng.device
@@ -372,7 +377,8 @@ class Fo1Pipeline:
         self._mark("splice")
         out = eng.generate(embeds, pos, lens, plan["rope_delta"], max_new_tokens, stop_ids, pad_id, want_prefill_logits=want_prefill_logits,
                            early_exit_interval=early_exit_interval, sampling=sampling, want_logprobs=want_logprobs, want_scores=want_scores,
-                           want_logits=want_logits, raw_rows=raw_rows, on_tokens=on_tokens, prefix=prefix, beams=beams, lookup=lookup)
+                           want_logits=want_logits, raw_rows=raw_rows, on_tokens=on_tokens, prefix=prefix, beams=beams, lookup=lookup,
+                           processors=processors)
         self._mark("llm_prefill_decode")
         out["prompt_lens"] = lens
         return out
@@ -393,14 +399,16 @@ class Fo1Pipeline:
 
     def generate_continuous(self, samples: Sequence[SampleInputs], n_slots: int, max_new_tokens, stop_ids: Sequence[int],
                             pad_id: int = 151643, sampling: Optional[Sampling] = None, early_exit_interval: int = 8,
-                            on_error: Optional[Callable[[int, BaseException], None]] = None) -> Iterator[Tuple[int, torch.Tensor, int]]:
+                            on_error: Optional[Callable[[int, BaseException], None]] = None,
+                            processors: Optional[Processors] = None) -> Iterator[Tuple[int, torch.Tensor, int]]:
         """Every sample through a slot pool of ``n_slots`` slots (engine.SlotPool): a finished request hands its slot to the next
         waiting one.  ``max_new_tokens``: one int, or one per sample; ``sampling``: None (greedy) or one parameter set per sample.
         Yields (index, tokens int32 [n] on the device, n) in completion order.  Each request's tokens and length equal those of a
         static generate() of ``n_slots`` samples on the same decode path (at most 8 slots on the persistent kernel, or 16 on the
         per-kernel path of a 132-SM H100: those of generate() alone).  Admission groups are encoded together (equal images share the
         towers); a group that fails is retried request by request, and a request that still fails is passed to ``on_error(index,
-        exception)`` and skipped (without ``on_error`` the exception propagates)."""
+        exception)`` and skipped (without ``on_error`` the exception propagates).  ``processors``: None or an engine.Processors with
+        one ProcessorSet or None per sample (prompts: each sample's ``input_ids`` unless given)."""
         B = len(samples)
         if B == 0:
             return
@@ -430,7 +438,12 @@ class Fo1Pipeline:
             sp = None
             if sampling is not None:
                 sp = Sampling(*([list(f)[i] for i in items] for f in (sampling.temperature, sampling.top_p, sampling.top_k, sampling.seed)))
-            pool.admit(slots, embeds, plan["position_ids"], plan["lens"], plan["rope_delta"], [mnt[i] for i in items], sampling=sp)
+            pr = None
+            if processors is not None:
+                prompts = processors.prompts if processors.prompts is not None else [s.input_ids for s in samples]
+                pr = Processors([processors.sets[i] for i in items], [list(prompts[i]) for i in items])
+            pool.admit(slots, embeds, plan["position_ids"], plan["lens"], plan["rope_delta"], [mnt[i] for i in items], sampling=sp,
+                       **({"processors": pr} if pr is not None else {}))
 
         def admit(items, slots):
             try:

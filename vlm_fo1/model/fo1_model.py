@@ -16,7 +16,12 @@ import torch
 # generation_config.json fields of logits processors the engine does not implement, with HF GenerationConfig's neutral defaults.
 # On the sampled path a non-neutral value is refused (honour or refuse, never ignore); greedy decoding does not read them.
 _UNSUPPORTED_PROCESSORS = (("repetition_penalty", 1.0), ("min_p", None), ("typical_p", 1.0), ("epsilon_cutoff", 0.0),
-                           ("eta_cutoff", 0.0), ("no_repeat_ngram_size", 0), ("num_beams", 1))
+                           ("eta_cutoff", 0.0), ("num_beams", 1))
+
+# HF logits processors the engine does not implement, with their neutral values: a non-neutral value is refused on every path
+_UNIMPLEMENTED_PROCESSORS = (("forced_bos_token_id", None), ("forced_eos_token_id", None), ("exponential_decay_length_penalty", None),
+                             ("guidance_scale", 1.0), ("prefix_allowed_tokens_fn", None), ("remove_invalid_values", False),
+                             ("renormalize_logits", False), ("watermarking_config", None), ("top_h", None))
 
 
 class Fo1ForCausalLM:
@@ -63,6 +68,70 @@ class Fo1ForCausalLM:
         if k < 0:
             raise ValueError(f"`top_k` has to be a non-negative integer, but is {top_k}")
         return T, p, k
+
+    def _processors(self, kwargs):
+        """None (no logits processor: today's path) or the engine.ProcessorSet of a call: sequence_bias, no_repeat_ngram_size,
+        bad_words_ids, min_length, min_new_tokens, suppress_tokens and begin_suppress_tokens from the call's kwargs, else
+        generation_config.json, validated by transformers' own processor classes (their ValueErrors).  As in HF's generate, a
+        min_new_tokens (even 0) overrides min_length: HF sets min_length = prompt length + min_new_tokens.  The eos ids MinLength and
+        MinNewTokens mask are HF's: eos_token_id, else the model's default stop ids.  Ids outside the vocabulary in the suppress and
+        eos lists are dropped, as HF's isin masks drop them.  HF processors the engine does not implement raise NotImplementedError
+        when non-neutral."""
+        gc = self.generation_config
+        get = lambda name: kwargs[name] if kwargs.get(name) is not None else gc.get(name)
+        for name, neutral in _UNIMPLEMENTED_PROCESSORS:
+            v = get(name)
+            if v is not None and v != neutral:
+                raise NotImplementedError(f"{name}={v!r} is not supported by the fo1-b200 engine (its logits processors are sequence_bias, "
+                                          "no_repeat_ngram_size, bad_words_ids, min_length, min_new_tokens, suppress_tokens and "
+                                          "begin_suppress_tokens)")
+        if kwargs.get("logits_processor"):
+            raise NotImplementedError("a custom logits_processor list is not supported by the fo1-b200 engine (its processors run on the device)")
+        from transformers.generation import logits_process as LP
+        E = import_module("vlm-fo1_b200.engine")
+        V = self._vocab()
+        in_vocab = lambda ids: tuple(int(t) for t in ids if V is None or 0 <= int(t) < V)
+        eos = kwargs.get("eos_token_id")
+        eos = gc.get("eos_token_id", self.default_stop_ids) if eos is None else eos
+        eos = [] if eos is None else ([int(eos)] if isinstance(eos, int) else [int(t) for t in eos])
+
+        def vocab_check(seqs):
+            bad = [t for w in seqs for t in w if V is not None and t >= V]
+            if bad:
+                raise ValueError(f"The model vocabulary size is {V}, but the following tokens were being biased: {bad}")
+        f = {}
+        ng = get("no_repeat_ngram_size")
+        if ng is not None and ng > 0:
+            f["no_repeat_ngram_size"] = LP.NoRepeatNGramLogitsProcessor(ng).ngram_size
+        sb = get("sequence_bias")
+        if sb is not None:
+            d = LP.SequenceBiasLogitsProcessor(sequence_bias=sb).sequence_bias
+            vocab_check(d)
+            f["sequence_bias"] = tuple((tuple(int(t) for t in k), float(v)) for k, v in d.items())
+        bw = get("bad_words_ids")
+        if bw is not None:
+            d = LP.NoBadWordsLogitsProcessor(bw, eos or None).sequence_bias
+            vocab_check(d)
+            if d:
+                f["bad_words_ids"] = tuple(tuple(int(t) for t in k) for k in d)
+        ml, mn = get("min_length"), get("min_new_tokens")
+        if mn is not None:      # HF's _prepare_generated_length: min_new_tokens takes precedence, min_length becomes P + min_new_tokens
+            ml = None
+        if ml is not None and eos and ml > 0:
+            f["min_length"] = LP.MinLengthLogitsProcessor(ml, eos).min_length
+        if mn is not None and eos and mn > 0:
+            f["min_new_tokens"] = LP.MinNewTokensLengthLogitsProcessor(0, mn, eos).min_new_tokens
+        if "min_length" in f or "min_new_tokens" in f:
+            f["eos_token_ids"] = in_vocab(eos)
+        for name in ("suppress_tokens", "begin_suppress_tokens"):
+            v = get(name)
+            if v is not None and in_vocab(v):
+                f[name] = in_vocab(v)
+        return E.ProcessorSet(**f) if f else None
+
+    def _vocab(self):
+        eng = getattr(self, "engine", None)
+        return eng.cfg.llm["vocab_size"] if eng is not None else None
 
     def _outputs(self, kwargs):
         """None (a bare LongTensor, as today) or (output_scores, output_logits) of a return_dict_in_generate call.  Like HF, the
@@ -243,8 +312,14 @@ class Fo1ForCausalLM:
         want = self._outputs(kwargs)
         beams = self._beams(do_sample, kwargs)
         lookup = self._lookup(kwargs)       # (with beams HF only warns and runs beam search; a streamed call runs without lookup)
+        procs = self._processors(kwargs)
         n = self._num_return_sequences(kwargs)
         kwargs.pop("num_return_sequences", None)
+        if procs is not None and (beams is not None or lookup is not None):
+            raise NotImplementedError("logits processors with num_beams > 1 or prompt_lookup_num_tokens are not supported by the fo1-b200 "
+                                      "engine (they run on its sampling and greedy paths)")
+        E = import_module("vlm-fo1_b200.engine")
+        pkw = lambda k: {"processors": E.Processors([procs] * k)} if procs is not None else {}
         if beams is not None:
             if streamer is not None:
                 raise ValueError("`streamer` cannot be used with beam search (yet!). Make sure that `num_beams` is set to 1.")
@@ -268,7 +343,7 @@ class Fo1ForCausalLM:
             # n copies of the sample share the whole prompt but its last row (the pipeline prefills it once); one seed each
             out = self.pipeline.generate([sample] * n, int(max_new_tokens), sorted(set(stop)), pad_id=int(pad), early_exit_interval=8,
                                          sampling=self._sampling([samp] * n), want_scores=bool(want and want[0]),
-                                         want_logits=bool(want and want[1]))
+                                         want_logits=bool(want and want[1]), **pkw(n))
             return self._results(out, inputs[0], want)
         on_tokens = None
         if streamer is not None:
@@ -282,7 +357,7 @@ class Fo1ForCausalLM:
                     streamer.put(torch.tensor([int(toks[0, t - lo])], dtype=torch.long))
         out = self.pipeline.generate([sample], int(max_new_tokens), sorted(set(stop)), pad_id=int(pad), early_exit_interval=8,
                                      sampling=self._sampling([samp]), want_scores=bool(want and want[0]), want_logits=bool(want and want[1]),
-                                     on_tokens=on_tokens, **({"lookup": lookup} if lookup is not None and streamer is None else {}))
+                                     on_tokens=on_tokens, **({"lookup": lookup} if lookup is not None and streamer is None else {}), **pkw(1))
         res = self._result(out, 0, inputs, want)
         if streamer is not None:
             streamer.end()
@@ -305,6 +380,10 @@ class Fo1ForCausalLM:
             return []
         wants = [self._outputs(kw) for kw in batch]
         beams = [self._beams(kw.get("do_sample", False), kw) for kw in batch]
+        procs = [self._processors(kw) for kw in batch]
+        if any(p is not None for p in procs) and (any(b is not None for b in beams) or any(self._lookup(kw) is not None for kw in batch)):
+            raise NotImplementedError("logits processors with num_beams > 1 or prompt_lookup_num_tokens are not supported by the fo1-b200 "
+                                      "engine (they run on its sampling and greedy paths)")
         if any(b is not None for b in beams):
             return self._generate_batch_beams(batch, beams, wants, max_new_tokens, output_logprobs)
         if any(self._num_return_sequences(kw) != 1 for kw in batch):
@@ -326,7 +405,9 @@ class Fo1ForCausalLM:
         out = self.pipeline.generate(list(samples), T, stop, pad_id=int(pad), early_exit_interval=8, sampling=sampling,
                                      want_logprobs=bool(output_logprobs), want_scores=any(w is not None and w[0] for w in wants),
                                      want_logits=any(w is not None and w[1] for w in wants), raw_rows=raw,
-                                     **({"lookup": lookups[0]} if lookups[0] is not None else {}))
+                                     **({"lookup": lookups[0]} if lookups[0] is not None else {}),
+                                     **({"processors": import_module("vlm-fo1_b200.engine").Processors(procs)}
+                                        if any(p is not None for p in procs) else {}))
         out["lens"] = out["lens"].cpu().tolist()
         res = []
         for b, kw in enumerate(batch):
@@ -341,8 +422,8 @@ class Fo1ForCausalLM:
         honouring its own ``max_new_tokens`` as ``generate(**kw)`` does, and equal to that sample's row in a static batch of
         ``batch_size`` samples on the same decode path (at most 8 slots on the persistent kernel: ``generate(**kw)`` alone).  Seeds
         are drawn from torch's generator in sample order.  ``on_error(i, exception)``: a sample whose admission fails is reported
-        there and skipped (without it the exception propagates).  Scores, streaming, beams, prompt lookup and
-        num_return_sequences > 1 are refused with NotImplementedError."""
+        there and skipped (without it the exception propagates).  Logits processors are honoured per sample.  Scores, streaming,
+        beams, prompt lookup and num_return_sequences > 1 are refused with NotImplementedError."""
         batch = list(kwargs_iterable)
         if not batch:
             return
@@ -357,6 +438,7 @@ class Fo1ForCausalLM:
                 raise NotImplementedError("prompt_lookup_num_tokens is not supported by generate_iter")
             if self._num_return_sequences(kw) != 1:
                 raise NotImplementedError("num_return_sequences > 1 is not supported by generate_iter")
+        procs = [self._processors(kw) for kw in batch]
         keys = ("inputs", "images", "images_aux", "image_grid_thws", "bbox_list", "do_sample", "temperature", "stopping_criteria", "top_p",
                 "top_k") + tuple(n for n, _ in _UNSUPPORTED_PROCESSORS)
         samples, stops, samps = zip(*(self._sample(**{k: v for k, v in kw.items() if k in keys}) for kw in batch))
@@ -365,7 +447,9 @@ class Fo1ForCausalLM:
         pad = pads[0] if pads[0] is not None else (stop[0] if stop else 0)
         mnt = [int(kw.get("max_new_tokens", 512)) for kw in batch]
         for i, tokens, n in self.pipeline.generate_continuous(list(samples), int(batch_size), mnt, stop, pad_id=int(pad), early_exit_interval=8,
-                                                             sampling=self._sampling(samps), on_error=on_error):
+                                                             sampling=self._sampling(samps), on_error=on_error,
+                                                             **({"processors": import_module("vlm-fo1_b200.engine").Processors(procs)}
+                                                                if any(p is not None for p in procs) else {})):
             inputs = batch[i]["inputs"]
             yield i, torch.cat([inputs[0].to(tokens.device), tokens.to(torch.long)]).unsqueeze(0)
 
