@@ -21,7 +21,7 @@
 extern "C" {
 #endif
 
-#define FO1_ABI_VERSION 3
+#define FO1_ABI_VERSION 4
 
 typedef enum {
   FO1_OK = 0,
@@ -188,7 +188,7 @@ typedef struct {
 size_t fo1_decode_attention_workspace_bytes(int32_t n_seqs, int32_t q_heads);
 int fo1_decode_attention(const fo1_decode_attn_desc* d, void* stream);
 
-/* Causal attention of a sequence's own rows against its K/V cache, the attention of fo1_llm_generate_prefixed: own row i of
+/* Causal attention of a sequence's own rows against its K/V cache, the attention of fo1_llm_generate with d.prefix: own row i of
  * sequence b (query row own_off_b + i of q, own rows of the sequences packed in order) attends the cache keys 0 .. P_b + i of b.
  * Its own K/V must already sit in the cache at row P_b + i.  Key tiles start at key 0 of the sequence, as in the full-sequence
  * prefill, so each row's output is bit-identical to what fo1_attention_varlen (causal) gives that row over the whole sequence.
@@ -358,6 +358,14 @@ int fo1_parse_predictions(const int32_t* tokens, int64_t ld, const int32_t* lens
 int fo1_llm_build_embeds(fo1_model* m, const int32_t* src_kind, const int32_t* src_index, int32_t n_rows,
                          const void* img_feats, const void* region_feats, void* inputs_embeds, void* stream);
 
+typedef struct fo1_sampling_desc fo1_sampling_desc;
+typedef struct fo1_score_desc fo1_score_desc;
+typedef struct fo1_stream_desc fo1_stream_desc;
+typedef struct fo1_prefix_desc fo1_prefix_desc;
+typedef struct fo1_processor_desc fo1_processor_desc;
+typedef struct fo1_lookup_desc fo1_lookup_desc;
+typedef struct fo1_beam_desc fo1_beam_desc;
+
 typedef struct {
   int32_t n_seqs;
   const int32_t* seq_lens;        /* host [n_seqs]: L_b, prompt length after the splice */
@@ -375,11 +383,32 @@ typedef struct {
   int32_t early_exit_interval;    /* host polls "all sequences stopped" every k decode steps (0 = never) */
   int32_t steps_run;              /* out: decode iterations actually executed */
   const int32_t* rope_deltas_device; /* optional DEVICE [n_seqs] (what fo1_splice_plan_batch wrote); overrides rope_deltas when set */
+  /* decoding options, each described in its section below; NULL: the option is off */
+  const fo1_sampling_desc* sampling;     /* per-sequence sampling (NULL: greedy) */
+  const fo1_score_desc* scores;          /* per-token scores */
+  const fo1_stream_desc* stream;         /* live token streaming */
+  const fo1_prefix_desc* prefix;         /* shared-prefix prefill */
+  const fo1_processor_desc* processors;  /* logits processors */
+  const fo1_lookup_desc* lookup;         /* prompt-lookup decoding */
+  const fo1_beam_desc* beam;             /* beam search */
 } fo1_generate_desc;
 
-/* Prefill + greedy decode (replaces OmChatQwen25VLForCausalLM.forward / HF generate's greedy loop /
+/* Prefill + decode (replaces OmChatQwen25VLForCausalLM.forward / HF generate's decoding loop /
  * DynamicCache for this path: omchat_qwen2_5_vl.py:466-532, modeling_qwen2_5_vl.py:1126-1242, 1848-1876).
- * The K/V cache and the decode loop state live on the device; the host only launches. */
+ * The K/V cache and the decode loop state live on the device; the host only launches.  With every option NULL (a
+ * zero-initialised descriptor plus the inputs and outputs) the call is greedy.
+ *
+ * An option that asks for nothing is the call without it: a `scores` whose three outputs are NULL, a `prefix` with
+ * n_groups == 0, and `processors` in which no sequence has a set (seq_set[b] == -1 for every b).
+ *
+ * Which options combine (any pair not listed combines):
+ *   beam        takes none of sampling, scores, stream, prefix, processors, lookup; refuses all_logits, allows prefill_logits
+ *   lookup      takes sampling, scores and prefix; refuses stream, processors and beam
+ *   prefix      refuses all_logits
+ *   processors  takes sampling, scores, stream and prefix
+ * A refused pair returns FO1_ERR_UNSUPPORTED, with a message that names both options, before any option's own checks and before
+ * the model is touched.  Every argument is checked on the host before anything is enqueued; a failed check of an option returns
+ * FO1_ERR_INVALID_ARG with the message "fo1_llm_generate: <option>: <rule>". */
 int fo1_llm_generate(fo1_model* m, fo1_generate_desc* d, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
@@ -391,20 +420,18 @@ int fo1_llm_generate(fo1_model* m, fo1_generate_desc* d, void* stream);
  * ascending.  top_k == 1 is greedy (lowest index among equal maxima).  A row's token depends only on its logits, its
  * parameters and its step.  The parameter arrays are validated on the host before any CUDA call.
  * ---------------------------------------------------------------------------------------------- */
-typedef struct {
+struct fo1_sampling_desc {
   const float* temperature;  /* HOST [n]: > 0 and finite; 1.0 = no scaling */
   const float* top_p;        /* HOST [n]: (0, 1]; 1.0 = off */
   const int32_t* top_k;      /* HOST [n]: >= 0; 0 or >= vocab = off */
   const uint64_t* seed;      /* HOST [n]: Philox key of each row / sequence */
-} fo1_sampling_desc;
+};
 size_t fo1_sample_tokens_workspace_bytes(int32_t n_rows);
 /* One token per row of fp32 logits [n_rows][ld] (device); step: DEVICE int32 [n_rows], the Philox counter of each row. */
 int fo1_sample_tokens(const float* logits, int64_t ld, int32_t n_rows, int32_t vocab, const fo1_sampling_desc* sp,
                       const int32_t* step /* DEVICE [n_rows] */, int32_t* out_tokens /* DEVICE [n_rows] */,
                       void* workspace, size_t workspace_bytes, void* stream);
-/* fo1_llm_generate with per-sequence sampling (the step of a sequence's token is its output column); sp == NULL is exactly
- * fo1_llm_generate (greedy). */
-int fo1_llm_generate_sampled(fo1_model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, void* stream);
+/* fo1_llm_generate with d.sampling samples each sequence with its parameters (the step of a sequence's token is its output column). */
 
 /* ------------------------------------------------------------------------------------------------
  * Per-token scores (HF generate's return_dict_in_generate with output_logits / output_scores, and the log-probability of each
@@ -424,18 +451,15 @@ int fo1_llm_generate_sampled(fo1_model* m, fo1_generate_desc* d, const fo1_sampl
  * Rows of scores / logits past a sequence's stop column, or of steps an early exit skipped, are unspecified.  Asking for any
  * of these never changes a token: the tokens are bit-identical to the same call without scoring.
  * ---------------------------------------------------------------------------------------------- */
-typedef struct {
+struct fo1_score_desc {
   float* logprobs;          /* optional DEVICE fp32 [n_seqs][max_new_tokens] */
   float* scores;            /* optional DEVICE fp32 [max_new_tokens][n_seqs][vocab] (HF output_scores) */
   float* logits;            /* optional DEVICE fp32 [max_new_tokens][n_seqs][vocab] (HF output_logits) */
   const int32_t* raw_rows;  /* optional HOST [n_seqs]: 1 = greedy sequence (top_k 1, temperature 1), scored on its raw logits.
-                               Ignored when sp == NULL: every sequence is then greedy and raw. */
-} fo1_score_desc;
-/* fo1_llm_generate_sampled with scoring; sc == NULL or all its outputs NULL is exactly fo1_llm_generate_sampled (sp == NULL:
- * greedy).  A greedy call with scoring samples with top_k 1, which is bit-identical to greedy. */
-int fo1_llm_generate_scored(fo1_model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp /* NULL: greedy */,
-                            const fo1_score_desc* sc, void* stream);
-/* The scoring of fo1_llm_generate_scored for arbitrary tokens: rows [n_rows] of fp32 logits (DEVICE, pitch ld) -> logprobs[r]
+                               Ignored without d.sampling: every sequence is then greedy and raw. */
+};
+/* fo1_llm_generate with d.scores: a greedy call with scoring samples with top_k 1, which is bit-identical to greedy.
+ * fo1_score_rows is that scoring for arbitrary tokens: rows [n_rows] of fp32 logits (DEVICE, pitch ld) -> logprobs[r]
  * of tokens[r] (-inf for a token outside the kept set) and, optionally, the processed rows scores[r] (pitch ld_scores).
  * sp == NULL or raw_rows[r] == 1: the row is scored raw (T = 1, nothing cut). */
 int fo1_score_rows(const float* logits, int64_t ld, int32_t n_rows, int32_t vocab, const fo1_sampling_desc* sp /* NULL: raw */,
@@ -464,16 +488,14 @@ int fo1_score_rows(const float* logits, int64_t ld, int32_t n_rows, int32_t voca
  * Streaming changes no token, score or logit: the outputs are bit-identical to the same call without it.
  * ---------------------------------------------------------------------------------------------- */
 #define FO1_STREAM_DONE (1 << 30)
-typedef struct {
+struct fo1_stream_desc {
   int32_t* tokens;          /* HOST mapped [n_seqs][max_new_tokens] */
   int32_t* lens;            /* HOST mapped [n_seqs] */
   int32_t* progress;        /* HOST mapped [1] */
   const int32_t* cancel;    /* HOST mapped [1], optional (NULL: the loop cannot be cancelled) */
-} fo1_stream_desc;
-/* fo1_llm_generate_scored with streaming; st == NULL is exactly fo1_llm_generate_scored.  The buffers are validated (non-NULL,
- * pinned and mapped) before anything is launched; the device uses their cudaHostGetDevicePointer aliases. */
-int fo1_llm_generate_streamed(fo1_model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp /* NULL: greedy */,
-                              const fo1_score_desc* sc /* NULL: unscored */, const fo1_stream_desc* st, void* stream);
+};
+/* fo1_llm_generate with d.stream: the buffers are validated (non-NULL, pinned and mapped) before anything is launched; the device
+ * uses their cudaHostGetDevicePointer aliases. */
 /* Acquire load of *progress and release store of 1 to *cancel: plain host code (no device, no model), for hosts whose language
  * cannot express the ordering (and for CPUs with a weaker memory model than x86). */
 int32_t fo1_stream_progress(const int32_t* progress);
@@ -485,22 +507,18 @@ void fo1_stream_cancel(int32_t* cancel);
  * through every layer, and their rotated K/V rows are written into the cache slot of every member at rows 0 .. P_g - 1.  The
  * remaining "own" rows of each sequence attend its cache (fo1_prefix_attention).  Decode is unchanged: each sequence owns a full
  * copy of its prefix K/V.  Every output (tokens, lengths, prefill logits, scores, logits, streamed columns) is bit-identical to
- * fo1_llm_generate_streamed on the full sequences.
+ * fo1_llm_generate without d.prefix on the full sequences.
  * ---------------------------------------------------------------------------------------------- */
-typedef struct {
+struct fo1_prefix_desc {
   int32_t n_groups;
   const int32_t* prefix_lens;          /* HOST [n_groups]: P_g >= 1 */
   const void* prefix_embeds;           /* DEVICE bf16 [sum P_g][llm_hidden], groups back to back */
   const int32_t* prefix_position_ids;  /* DEVICE int32 [3][sum P_g] */
   const int32_t* seq_group;            /* HOST [n_seqs]: the sequence's group, or -1 (no shared prefix) */
-} fo1_prefix_desc;
-/* fo1_llm_generate_streamed with shared prefixes.  In d, seq_lens stays the full length L_b; inputs_embeds / position_ids hold
- * only each sequence's own rows (L_b - P_g, or L_b without a group), packed in sequence order.  px == NULL or n_groups == 0 is
- * exactly fo1_llm_generate_streamed.  Checked on the host before any CUDA call: group indices in range, at least two members
- * per group, P_g < L_b for every member, non-NULL pointers, and no all_logits. */
-int fo1_llm_generate_prefixed(fo1_model* m, fo1_generate_desc* d, const fo1_prefix_desc* px, const fo1_sampling_desc* sp /* NULL: greedy */,
-                              const fo1_score_desc* sc /* NULL: unscored */, const fo1_stream_desc* st /* NULL: not streamed */,
-                              void* stream);
+};
+/* fo1_llm_generate with d.prefix: seq_lens stays the full length L_b; inputs_embeds / position_ids hold only each sequence's own
+ * rows (L_b - P_g, or L_b without a group), packed in sequence order.  Checked on the host before any CUDA call: group indices in
+ * range, at least two members per group, P_g < L_b for every member, non-NULL pointers, and no all_logits. */
 
 /* ------------------------------------------------------------------------------------------------
  * Beam search (HF generate with num_beams > 1 and do_sample=False: transformers' GenerationMixin._beam_search and its helpers).
@@ -517,7 +535,7 @@ int fo1_llm_generate_prefixed(fo1_model* m, fo1_generate_desc* d, const fo1_pref
  * best num_return hypotheses of each prompt, best first; all_logits is refused, prefill_logits is allowed; steps_run is the number
  * of decode iterations the loop ran.  Always the per-kernel decode path (fo1_last_decode_path() == 0).
  * ---------------------------------------------------------------------------------------------- */
-typedef struct {
+struct fo1_beam_desc {
   int32_t num_beams;         /* N: 2 .. 16 */
   int32_t n_keep;            /* K: HF's max(2, 1 + number of eos ids) * N; 2N <= K <= 128 and K <= vocab */
   double length_penalty;     /* finite; double, as HF's Python float: the divisors are (float)pow(len, length_penalty) */
@@ -530,10 +548,10 @@ typedef struct {
   float* logits;             /* optional DEVICE fp32 [max_new_tokens][n_seqs * N][vocab]: the raw rows (HF output_logits) */
   float* logprobs;           /* optional DEVICE fp32 [n_seqs * num_return][max_new_tokens]: each returned token's log-probability
                                 under its parent beam's row (HF's compute_transition_scores with beam_indices); 0 past the length */
-} fo1_beam_desc;
-/* Checked on the host before any CUDA call: 2 <= N <= 16, 1 <= num_return <= N, 2N <= n_keep <= min(128, vocab), a finite
- * length_penalty, early_stopping in {0, 1, 2}, max_new_tokens >= 1, the outputs non-NULL and no all_logits. */
-int fo1_llm_generate_beam(fo1_model* m, fo1_generate_desc* d, const fo1_beam_desc* bm, void* stream);
+};
+/* fo1_llm_generate with d.beam: checked on the host before any CUDA call: 2 <= N <= 16, 1 <= num_return <= N,
+ * 2N <= n_keep <= min(128, vocab), a finite length_penalty, early_stopping in {0, 1, 2}, max_new_tokens >= 1, the outputs non-NULL
+ * and no all_logits. */
 
 /* ------------------------------------------------------------------------------------------------
  * Prompt-lookup decoding (HF generate's prompt_lookup_num_tokens / max_matching_ngram_size).  Each sequence's corpus is its
@@ -548,19 +566,17 @@ int fo1_llm_generate_beam(fo1_model* m, fo1_generate_desc* d, const fo1_beam_des
  * early_exit_interval > 0 the loop polls after every verify step, one step behind (at most one step runs after the last sequence
  * ends); with 0 it never polls and runs max_new_tokens - 1 steps.
  * ---------------------------------------------------------------------------------------------- */
-typedef struct {
+struct fo1_lookup_desc {
   int32_t num_tokens;               /* K >= 1 (drafts per step; more than 16 proposes 16) */
   int32_t max_ngram;                /* >= 1 */
   const int32_t* corpus;            /* HOST int32, the n_seqs corpora packed */
   const int32_t* corpus_offsets;    /* HOST int32 [n_seqs + 1]: corpus b is corpus[offsets[b] .. offsets[b + 1]) */
   int32_t* steps;                   /* optional DEVICE int32 [n_seqs]: verify steps the sequence took part in */
   int32_t* accepted;                /* optional DEVICE int32 [n_seqs]: drafts accepted */
-} fo1_lookup_desc;
-/* Checked on the host before any CUDA call: num_tokens >= 1, max_ngram >= 1, corpus offsets present, starting at 0 and
- * non-decreasing, corpus present when non-empty; with px, the checks of fo1_llm_generate_prefixed.  sp / sc as in
- * fo1_llm_generate_scored; px as in fo1_llm_generate_prefixed (the prefill is unchanged). */
-int fo1_llm_generate_lookup(fo1_model* m, fo1_generate_desc* d, const fo1_lookup_desc* lk, const fo1_prefix_desc* px /* NULL */,
-                            const fo1_sampling_desc* sp /* NULL: greedy */, const fo1_score_desc* sc /* NULL: unscored */, void* stream);
+};
+/* fo1_llm_generate with d.lookup: checked on the host before any CUDA call: num_tokens >= 1, max_ngram >= 1, corpus offsets present,
+ * starting at 0 and non-decreasing, corpus present when non-empty.  d.sampling, d.scores and d.prefix work as without lookup (the
+ * prefill is unchanged). */
 /* The draft rule alone: corpora DEVICE int32 [n_seqs][ld] with lengths lens [n_seqs] -> drafts DEVICE int32 [n_seqs][num_tokens]
  * and n_draft [n_seqs].  stop_ids DEVICE [n_stop]; emitted (DEVICE [n_seqs], optional) with max_new_tokens caps the drafts at
  * max_new_tokens - emitted - 1.  1 <= num_tokens <= 16, max_ngram >= 1. */
@@ -587,7 +603,7 @@ int fo1_lookup_drafts(const int32_t* corpus, int64_t ld, const int32_t* lens, in
  * and the log-probabilities are those of the processed row.  A row that ends up all -inf (every token banned) draws token 0, the
  * arg-max rule, on every path, greedy or sampled; nothing is kept, so its log-probability is -inf.
  * ---------------------------------------------------------------------------------------------- */
-typedef struct {
+struct fo1_processor_desc {
   int32_t n_sets;                          /* >= 1 processor sets, each used by any number of sequences */
   const int32_t* seq_set;                  /* HOST [n_seqs]: the sequence's set, or -1 (no processors) */
   const int32_t* prompt;                   /* HOST: the sequences' prompt ids packed, each in [-vocab, vocab) */
@@ -608,13 +624,9 @@ typedef struct {
   const float* bias;                       /* HOST [n_sequences]: the bias of each sequence_bias sequence, finite (bad words: unread) */
   int32_t n_ids;
   const int32_t* ids;                      /* HOST [n_ids]: token ids in [0, vocab) */
-} fo1_processor_desc;
-/* fo1_llm_generate_prefixed with logits processors; pr == NULL, or no sequence with a set, is exactly fo1_llm_generate_prefixed.
- * Checked on the host before any launch: the ranges above.  A greedy call with processors chooses through the sampler with top_k 1
- * (bit-identical to the arg-max), on the persistent kernel too.  Beam search and prompt lookup take no processors. */
-int fo1_llm_generate_processed(fo1_model* m, fo1_generate_desc* d, const fo1_prefix_desc* px /* NULL */, const fo1_sampling_desc* sp /* NULL: greedy */,
-                               const fo1_score_desc* sc /* NULL: unscored */, const fo1_stream_desc* st /* NULL: not streamed */,
-                               const fo1_processor_desc* pr /* NULL: none */, void* stream);
+};
+/* fo1_llm_generate with d.processors: checked on the host before any launch: the ranges above.  A greedy call with processors chooses
+ * through the sampler with top_k 1 (bit-identical to the arg-max), on the persistent kernel too. */
 /* The row routine alone: rows [n_rows] of fp32 logits (DEVICE, pitch ld) edited in place; row r is sequence r of pr at output column
  * cols[r] (HOST), its emitted tokens outputs[r][0 .. cols[r]) (DEVICE, pitch ld_out; may be NULL when every column is 0). */
 int fo1_logits_process(float* logits, int64_t ld, int32_t n_rows, int32_t vocab, const fo1_processor_desc* pr, const int32_t* outputs,
@@ -628,9 +640,9 @@ int fo1_logits_process(float* logits, int64_t ld, int32_t n_rows, int32_t vocab,
  * output row, the Philox step of its sampler, and what is tested against its own max_new_tokens; a slot that reaches its limit or a
  * stop id finishes and stays idle (its cache stops growing) until it is admitted again.  Every step runs all n_slots rows, so the
  * decode attention's key split and the decode path follow n_slots for the life of the pool: each request's tokens and length equal
- * its tokens and length in a static fo1_llm_generate_sampled call of n_slots sequences on the same decode path, whatever its
+ * its tokens and length in a static fo1_llm_generate call of n_slots sequences (with d.sampling) on the same decode path, whatever its
  * companions and whenever it was admitted.  Greedy and sampled decoding; no scores, streaming, beams, lookup or shared prefixes.
- * While a pool is open it owns the model's K/V cache: every fo1_llm_generate* call is refused.
+ * While a pool is open it owns the model's K/V cache: every fo1_llm_generate call is refused.
  * ---------------------------------------------------------------------------------------------- */
 typedef struct {
   int32_t n_slots;              /* 1 .. 65535 */
@@ -657,7 +669,7 @@ typedef struct {
   const int32_t* rope_deltas_device;     /* DEVICE int32 [n] (what fo1_splice_plan_batch wrote) */
   const int32_t* max_new_tokens;         /* HOST [n]: each request's own limit, 1 .. the pool's max_new_tokens */
   const fo1_sampling_desc* sampling;     /* NULL: greedy; else per request (a pool opened with sampled = 1) */
-  const fo1_processor_desc* processors;  /* NULL: none; else per request, checked as fo1_llm_generate_processed checks it.  The
+  const fo1_processor_desc* processors;  /* NULL: none; else per request, checked as fo1_llm_generate checks d.processors.  The
                                             pool keeps each admitted request's set and prompt ids until its slot is admitted again. */
 } fo1_slots_admit_desc;
 /* Prefills the n requests into their slots (the prefill of fo1_llm_generate with the slots as the cache-write members) and records

@@ -2,8 +2,9 @@
 engine (before and after a change to the decoder) can be required to agree bit for bit.
 
 The set: greedy, sampled, scored and streamed calls at B = 1, 8, 17 and 33, on both decode paths (the default, and the per-kernel
-path with FO1_NO_MEGA=1); a shared-prefix batch (one group and loners); beam search with N = 4; prompt lookup with K = 4.  Every call
-asks for the prefill logits.  Random-init decoder (Qwen2.5-3B widths, 4 layers, 20000-token vocabulary) on the GPU.
+path with FO1_NO_MEGA=1); a shared-prefix batch (one group and loners); beam search with N = 4; prompt lookup with K = 4; logits
+processors (sets that differ per sequence, some sequences without one) on greedy, sampled, scored and streamed calls at B = 8 and 17
+on both decode paths, and with the shared prefix.  Every call asks for the prefill logits.  Random-init decoder (Qwen2.5-3B widths, 4 layers, 20000-token vocabulary) on the GPU.
 
     python scripts/ab_generate.py --out run.pt             # run the set, save every output
     python scripts/ab_generate.py --compare old.pt new.pt  # torch.equal on every output of every call
@@ -36,6 +37,19 @@ def _batch(make_seq, B, seed):
     seqs = [make_seq(30 + 9 * (b % 7), None, seed + b, vocab=VOCAB) for b in range(B)]
     return (torch.cat([s.emb for s in seqs]).cuda(), torch.cat([s.pos for s in seqs], 1).cuda(), [s.L for s in seqs],
             [s.delta for s in seqs])
+
+
+def _processors(E, B, seed):
+    """Processor sets for B sequences, cycling through four: a bias strong enough that the n-gram ban has to act, lists and min lengths
+    that hold back the stop ids, and None (a row that is never edited).  The prompts start with an image placeholder."""
+    S = E.ProcessorSet
+    sets = [S(no_repeat_ngram_size=2, sequence_bias=(((5,), 30.0),), min_new_tokens=3, eos_token_ids=(7, 11)),
+            None,
+            S(sequence_bias=(((9,), 2.5), ((9, 5), -1.0)), bad_words_ids=((13,), (4, 6)), suppress_tokens=(17,), begin_suppress_tokens=(19,)),
+            S(min_length=40, eos_token_ids=(7,), no_repeat_ngram_size=3)]
+    g = torch.Generator().manual_seed(seed)
+    prompts = [[-200] + torch.randint(0, VOCAB, (10 + b,), generator=g).tolist() for b in range(B)]
+    return E.Processors([sets[b % len(sets)] for b in range(B)], prompts)
 
 
 def run(out_path):
@@ -90,6 +104,25 @@ def run(out_path):
         call(f"prefix-greedy/{p}", no_mega, *xp, prefix=prefix)
         call(f"prefix-scored/{p}", no_mega, *xp, prefix=prefix, sampling=sampp, want_logprobs=True, want_scores=True, want_logits=True)
         call(f"prefix-streamed/{p}", no_mega, *xp, prefix=prefix, stream=True)
+
+    # logits processors: greedy, sampled, scored and streamed, on both decode paths, and with the shared prefix
+    for B in (8, 17):
+        x = _batch(make_seq, B, 9000 + B)
+        procs = _processors(E, B, 40 + B)
+        samp = E.Sampling([0.8] * B, [0.9] * B, [40] * B, [4000 + b for b in range(B)])
+        for no_mega in (False, True):
+            p = "pk" if no_mega else "default"
+            call(f"processed-greedy/B{B}/{p}", no_mega, *x, processors=procs)
+            call(f"processed-sampled/B{B}/{p}", no_mega, *x, sampling=samp, processors=procs)
+            call(f"processed-scored/B{B}/{p}", no_mega, *x, sampling=samp, want_logprobs=True, want_scores=True, want_logits=True,
+                 processors=procs)
+            call(f"processed-scored-greedy/B{B}/{p}", no_mega, *x, want_logprobs=True, want_scores=True, want_logits=True, processors=procs)
+            call(f"processed-streamed/B{B}/{p}", no_mega, *x, sampling=samp, stream=True, processors=procs)
+    procs_p = _processors(E, Bp, 60)
+    for no_mega in (False, True):
+        p = "pk" if no_mega else "default"
+        call(f"prefix-processed/{p}", no_mega, *xp, prefix=prefix, sampling=sampp, want_logprobs=True, want_scores=True, want_logits=True,
+             processors=procs_p)
 
     # beam search, N = 4
     for B in (1, 8):

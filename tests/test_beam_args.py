@@ -1,4 +1,4 @@
-"""CPU: the argument handling of beam search -- fo1_llm_generate_beam's host checks, which run before any CUDA call, and
+"""CPU: the argument handling of beam search -- fo1_llm_generate's host checks of d.beam, which run before any CUDA call, and
 Fo1ForCausalLM.generate / generate_batch's reading of num_beams, length_penalty, early_stopping and num_return_sequences, with
 HF's refusals.  The model tests record the pipeline call instead of running it."""
 import ctypes
@@ -36,7 +36,7 @@ BEAM_CASES = {  # case: (field overrides, expected text)
 
 
 @pytest.mark.parametrize("case", sorted(BEAM_CASES))
-def test_generate_beam_argument_validation_without_gpu(case):
+def test_generate_beam_desc_validation_without_gpu(case):
     F, L, E = _lib()
     over, text = BEAM_CASES[case]
     cfg = E.ModelConfigC()
@@ -53,20 +53,22 @@ def test_generate_beam_argument_validation_without_gpu(case):
              scores=None, logits=None, logprobs=None)
     f.update(over)
     bm = F.BeamDesc(**f)
-    rc = L.fo1_llm_generate_beam(m, ctypes.byref(d), ctypes.byref(bm), None)
+    d.beam = ctypes.pointer(bm)
+    rc = L.fo1_llm_generate(m, ctypes.byref(d), None)
     msg = L.fo1_last_error().decode()
     assert rc == -1, (case, rc, msg)
-    assert "fo1_llm_generate_beam" in msg and (text is None or text in msg), msg
+    assert "fo1_llm_generate: beam: " in msg and (text is None or text in msg), msg
     if case == "keep_above_vocab":
         assert "vocab 100" in msg
     L.fo1_model_destroy(m)
 
 
-def test_generate_beam_null_model():
+def test_generate_with_beam_null_model():
     F, L, E = _lib()
     d = E.GenerateDescC()
     bm = F.BeamDesc(num_beams=4, n_keep=8, num_return=1)
-    assert L.fo1_llm_generate_beam(None, ctypes.byref(d), ctypes.byref(bm), None) == -1
+    d.beam = ctypes.pointer(bm)
+    assert L.fo1_llm_generate(None, ctypes.byref(d), None) == -1
     assert "null argument" in L.fo1_last_error().decode()
 
 

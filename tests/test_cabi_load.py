@@ -2,12 +2,12 @@
 import ctypes
 
 
-def test_library_loads_and_exports_header_symbols():
+def test_library_loads_abi_4_and_exports_header_symbols():
     import __graft_entry__ as G
     G.build()
     import fo1_b200
     L = fo1_b200.lib()
-    assert L.fo1_abi_version() == 3
+    assert L.fo1_abi_version() == 4
     syms = fo1_b200._lib.exported_symbols()
     assert "fo1_hfre_forward" in syms and "fo1_gemm_bf16" in syms
     for s in syms:

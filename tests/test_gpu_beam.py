@@ -1,4 +1,4 @@
-"""-m gpu: beam search on the device (csrc/beam.cu, fo1_llm_generate_beam) at the 3B widths (2 decoder layers, vocabulary 20000,
+"""-m gpu: beam search on the device (csrc/beam.cu, fo1_llm_generate with d.beam) at the 3B widths (2 decoder layers, vocabulary 20000,
 non-unit norm gains and non-zero biases: tests/test_gpu_decode_parity.py's model).
 
   1. Selection is HF's, bit for bit: the engine's own per-step log-prob rows (`scores`) fed to oracle/beam.py (the restatement of

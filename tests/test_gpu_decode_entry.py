@@ -1,7 +1,6 @@
-"""-m gpu: the older generate entry points of the C ABI -- fo1_llm_generate, fo1_llm_generate_sampled and fo1_llm_generate_scored --
-called directly through ctypes.  Engine.generate calls fo1_llm_generate_streamed with NULL for whatever it does not use, which
-include/fo1.h documents as exactly each of these; every one must give Engine.generate's tokens, lengths, step count and scores bit
-for bit on both decode paths."""
+"""-m gpu: fo1_llm_generate called directly through ctypes with a descriptor filled by hand: every option NULL (greedy), d.sampling,
+and d.sampling with d.scores (greedy or sampled).  Each must give Engine.generate's tokens, lengths, step count and scores bit for bit
+on both decode paths."""
 import ctypes as C
 
 import pytest
@@ -24,7 +23,7 @@ def engine():
 
 
 def _direct(eng, mode, emb, pos, lens, T, stop, samp):
-    """One call of the entry point that `mode` names, with a descriptor filled as Engine.generate fills it."""
+    """One fo1_llm_generate call with the options `mode` names, in a descriptor filled as Engine.generate fills it."""
     F, E = _mods()
     B, V, dev = len(lens), eng.cfg.llm["vocab_size"], eng.device
     toks = torch.empty((B, T), dtype=torch.int32, device=dev)
@@ -38,28 +37,24 @@ def _direct(eng, mode, emb, pos, lens, T, stop, samp):
     d.max_new_tokens, d.pad_id, d.early_exit_interval = T, 0, 2
     d.out_tokens, d.out_lens = toks.data_ptr(), out_lens.data_ptr()
     L, stream = F.lib(), C.c_void_p(torch.cuda.current_stream().cuda_stream)
-    sd = None
     if samp is not None:
         sd, _keep = F.sampling_desc(samp.temperature, samp.top_p, samp.top_k, samp.seed)     # (the arrays must outlive the call)
-        sd = C.byref(sd)
+        d.sampling = C.pointer(sd)
     out = dict()
-    if mode == "greedy":
-        F.check(L.fo1_llm_generate(eng._h, C.byref(d), stream), "fo1_llm_generate")
-    elif mode == "sampled":
-        F.check(L.fo1_llm_generate_sampled(eng._h, C.byref(d), sd, stream), "fo1_llm_generate_sampled")
-    else:
+    if mode == "scored":
         out["logprobs"] = torch.empty((B, T), dtype=torch.float32, device=dev)
         out["scores"] = torch.empty((T, B, V), dtype=torch.float32, device=dev)
         out["logits"] = torch.empty((T, B, V), dtype=torch.float32, device=dev)
         desc = F.ScoreDesc(out["logprobs"].data_ptr(), out["scores"].data_ptr(), out["logits"].data_ptr(), None)
-        F.check(L.fo1_llm_generate_scored(eng._h, C.byref(d), sd, C.byref(desc), stream), "fo1_llm_generate_scored")
+        d.scores = C.pointer(desc)
+    F.check(L.fo1_llm_generate(eng._h, C.byref(d), stream), "fo1_llm_generate")
     torch.cuda.synchronize()
     return dict(out, tokens=toks, lens=out_lens, steps_run=d.steps_run)
 
 
 @pytest.mark.parametrize("no_mega", [False, True])
 @pytest.mark.parametrize("mode,sampled", [("greedy", False), ("sampled", True), ("scored", False), ("scored", True)])
-def test_older_entry_points_equal_generate(engine, mode, sampled, no_mega, monkeypatch):
+def test_hand_filled_descriptor_equals_generate(engine, mode, sampled, no_mega, monkeypatch):
     _, E = _mods()
     if no_mega:
         monkeypatch.setenv("FO1_NO_MEGA", "1")

@@ -115,7 +115,7 @@ def test_lookup_max_new_mid_step(eng, monkeypatch):
 
 
 def test_lookup_shared_prefix(eng, monkeypatch):
-    """A shared-prefix batch (fo1_llm_generate_prefixed's prefill) decodes with lookup as the same call without it."""
+    """A shared-prefix batch (the prefill of fo1_llm_generate with d.prefix) decodes with lookup as the same call without it."""
     E, _, _ = _mods()
     B, P = 6, 30
     s0 = make_seq(P + 10, None, 7, vocab=VOCAB)

@@ -1,4 +1,4 @@
-"""CPU: the argument handling of prompt-lookup decoding -- fo1_llm_generate_lookup's host checks, which run before any CUDA call,
+"""CPU: the argument handling of prompt-lookup decoding -- fo1_llm_generate's host checks of d.lookup, which run before any CUDA call,
 and Fo1ForCausalLM.generate / generate_batch's reading of prompt_lookup_num_tokens and max_matching_ngram_size.  The model tests
 record the pipeline call instead of running it (tests/test_beam_args.py)."""
 import ctypes
@@ -20,7 +20,7 @@ LOOKUP_CASES = {  # case: (num_tokens, max_ngram, offsets, corpus present, expec
 
 
 @pytest.mark.parametrize("case", sorted(LOOKUP_CASES))
-def test_generate_lookup_argument_validation_without_gpu(case):
+def test_generate_lookup_desc_validation_without_gpu(case):
     F, L, E = _lib()
     K, ng, offs, has_corpus, text = LOOKUP_CASES[case]
     cfg = E.ModelConfigC()
@@ -34,10 +34,11 @@ def test_generate_lookup_argument_validation_without_gpu(case):
     ids = (ctypes.c_int32 * 2)(5, 6)
     off = (ctypes.c_int32 * 3)(*offs) if offs is not None else None
     lk = F.LookupDesc(K, ng, ids if has_corpus else None, off, None, None)
-    rc = L.fo1_llm_generate_lookup(m, ctypes.byref(d), ctypes.byref(lk), None, None, None, None)
+    d.lookup = ctypes.pointer(lk)
+    rc = L.fo1_llm_generate(m, ctypes.byref(d), None)
     msg = L.fo1_last_error().decode()
     assert rc == -1, (case, rc, msg)
-    assert "fo1_llm_generate_lookup" in msg and text in msg, msg
+    assert "fo1_llm_generate: lookup: " in msg and text in msg, msg
     L.fo1_model_destroy(m)
 
 

@@ -1,6 +1,6 @@
 """CPU checks of the per-token scoring contract: tests/scores_oracle.py's processed / logprob against transformers' warper chain,
-Fo1ForCausalLM.compute_transition_scores against transformers' own, and the host-side argument validation of fo1_score_rows and
-fo1_llm_generate_scored."""
+Fo1ForCausalLM.compute_transition_scores against transformers' own, and the host-side argument validation of fo1_score_rows and of
+fo1_llm_generate with d.scores."""
 import ctypes
 from types import SimpleNamespace
 
@@ -146,8 +146,8 @@ def test_score_rows_argument_validation_without_gpu(case):
 
 
 @pytest.mark.parametrize("case", ["null_desc", "temp", "raw_value", "raw_not_greedy", "raw_temperature"])
-def test_generate_scored_argument_validation_without_gpu(case):
-    """fo1_llm_generate_scored checks the per-sequence host arrays before it touches the model or the device."""
+def test_generate_sampling_and_scores_validation_without_gpu(case):
+    """fo1_llm_generate checks the per-sequence host arrays of d.sampling and d.scores before it touches the model or the device."""
     F, L = _lib()
     E = __import__("importlib").import_module("vlm-fo1_b200.engine")
     d = E.GenerateDescC()
@@ -162,9 +162,11 @@ def test_generate_scored_argument_validation_without_gpu(case):
     sd, keep = _desc(T, 0.9, k, 2)
     raw = (ctypes.c_int32 * 2)(1, 3 if case == "raw_value" else 1)
     sc = F._lib.ScoreDesc(16, None, None, raw)
+    d.sampling, d.scores = ctypes.pointer(sd), ctypes.pointer(sc)
     if case == "null_desc":
-        rc = L.fo1_llm_generate_scored(None, None, ctypes.byref(sd), ctypes.byref(sc), None)
+        rc = L.fo1_llm_generate(None, None, None)
     else:
-        rc = L.fo1_llm_generate_scored(ctypes.c_void_p(16), ctypes.byref(d), ctypes.byref(sd), ctypes.byref(sc), None)
+        rc = L.fo1_llm_generate(ctypes.c_void_p(16), ctypes.byref(d), None)
     assert rc == -1
-    assert len(L.fo1_last_error()) > 0
+    msg = L.fo1_last_error().decode()
+    assert {"null_desc": "null argument", "temp": "sampling: "}.get(case, "scores: ") in msg, msg

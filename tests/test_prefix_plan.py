@@ -1,5 +1,5 @@
 """CPU checks of shared-prefix generation: the pipeline's grouping of samples by encoder-input content and its prefix planner (pure
-Python), and the host-side argument checks of fo1_llm_generate_prefixed, which run before the model or the device is touched."""
+Python), and fo1_llm_generate's host-side argument checks of d.prefix, which run before the model or the device is touched."""
 import ctypes
 from importlib import import_module
 
@@ -110,7 +110,7 @@ PREFIX_CASES = ["group_range", "group_below", "one_member", "prefix_too_long", "
 
 
 @pytest.mark.parametrize("case", PREFIX_CASES)
-def test_generate_prefixed_argument_validation_without_gpu(case):
+def test_generate_prefix_desc_validation_without_gpu(case):
     F, L, E = _lib()
     d = E.GenerateDescC()
     d.n_seqs = 3
@@ -132,11 +132,12 @@ def test_generate_prefixed_argument_validation_without_gpu(case):
         d.all_logits = 16
     px = F.PrefixDesc(1, None if case == "null_lens" else (ctypes.c_int32 * 1)(*plens), None if case == "null_embeds" else 16,
                       None if case == "null_pos" else 16, None if case == "null_groups" else (ctypes.c_int32 * 3)(*groups))
+    d.prefix = ctypes.pointer(px)
     model = None if case == "null_model" else ctypes.c_void_p(16)      # never dereferenced: the checks come first
-    rc = L.fo1_llm_generate_prefixed(model, ctypes.byref(d), ctypes.byref(px), None, None, None, None)
+    rc = L.fo1_llm_generate(model, ctypes.byref(d), None)
     assert rc == -1
     msg = L.fo1_last_error().decode()
-    assert "fo1_llm_generate_prefixed" in msg, msg
+    assert ("fo1_llm_generate: null argument" if case == "null_model" else "fo1_llm_generate: prefix: ") in msg, msg
 
 
 def test_prefix_attention_argument_validation_without_gpu():

@@ -1,6 +1,6 @@
 """CPU: the argument handling of the logits processors -- Fo1ForCausalLM._processors' reading of the call's kwargs, else
-generation_config.json, HF's ValueErrors, neutral values, the refusals, and fo1_llm_generate_processed's host checks (before any CUDA
-call).  The model tests record the pipeline call instead of running it (tests/test_beam_args.py)."""
+generation_config.json, HF's ValueErrors, neutral values, the refusals, and fo1_llm_generate's host checks of d.processors (before any
+CUDA call).  The model tests record the pipeline call instead of running it (tests/test_beam_args.py)."""
 import ctypes
 from types import SimpleNamespace
 
@@ -99,7 +99,7 @@ CHECKS = {  # case: (field edits, expected text)
 
 
 @pytest.mark.parametrize("case", sorted(CHECKS))
-def test_generate_processed_host_checks(case):
+def test_generate_processors_desc_host_checks(case):
     F, L, E = _lib()
     edits, text = CHECKS[case]
     cfg = E.ModelConfigC()
@@ -117,9 +117,10 @@ def test_generate_processed_host_checks(case):
     pr = F.ProcessorDesc(1, i32(f["seq_set"]), i32(f["prompt"]), i32(f["poff"]), i32(f["ng"]), i32(f["ml"]), i32(f["mn"]), i32(f["eos"]),
                          i32(f["sup"]), i32(f["bsup"]), i32(f["bias_off"]), i32(f["bad_off"]), len(f["bias"]), i32(f["seq_off"]),
                          (ctypes.c_float * 1)(*f["bias"]), len(f["ids"]), i32(f["ids"]))
-    rc = L.fo1_llm_generate_processed(m, ctypes.byref(d), None, None, None, None, ctypes.byref(pr), None)
+    d.processors = ctypes.pointer(pr)
+    rc = L.fo1_llm_generate(m, ctypes.byref(d), None)
     msg = L.fo1_last_error().decode()
-    assert rc == -1 and "fo1_llm_generate_processed" in msg and text in msg, (case, rc, msg)
+    assert rc == -1 and "fo1_llm_generate: processors: " in msg and text in msg, (case, rc, msg)
     L.fo1_model_destroy(m)
 
 

@@ -170,27 +170,11 @@ def lib() -> C.CDLL:
     L.fo1_sample_tokens.restype = C.c_int
     L.fo1_sample_tokens.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.POINTER(SamplingDesc), C.c_void_p, C.c_void_p,
                                     C.c_void_p, C.c_size_t, C.c_void_p]
-    L.fo1_llm_generate_sampled.restype = C.c_int
-    L.fo1_llm_generate_sampled.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(SamplingDesc), C.c_void_p]
-    L.fo1_llm_generate_scored.restype = C.c_int
-    L.fo1_llm_generate_scored.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(SamplingDesc), C.POINTER(ScoreDesc), C.c_void_p]
-    L.fo1_llm_generate_streamed.restype = C.c_int
-    L.fo1_llm_generate_streamed.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(SamplingDesc), C.POINTER(ScoreDesc), C.POINTER(StreamDesc),
-                                            C.c_void_p]
-    L.fo1_llm_generate_prefixed.restype = C.c_int
-    L.fo1_llm_generate_prefixed.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(PrefixDesc), C.POINTER(SamplingDesc), C.POINTER(ScoreDesc),
-                                            C.POINTER(StreamDesc), C.c_void_p]
-    L.fo1_llm_generate_processed.restype = C.c_int
-    L.fo1_llm_generate_processed.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(PrefixDesc), C.POINTER(SamplingDesc), C.POINTER(ScoreDesc),
-                                             C.POINTER(StreamDesc), C.POINTER(ProcessorDesc), C.c_void_p]
+    L.fo1_llm_generate.restype = C.c_int
+    L.fo1_llm_generate.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     L.fo1_logits_process.restype = C.c_int
     L.fo1_logits_process.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.POINTER(ProcessorDesc), C.c_void_p, C.c_int64,
                                      C.POINTER(C.c_int32), C.c_void_p]
-    L.fo1_llm_generate_beam.restype = C.c_int
-    L.fo1_llm_generate_beam.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(BeamDesc), C.c_void_p]
-    L.fo1_llm_generate_lookup.restype = C.c_int
-    L.fo1_llm_generate_lookup.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(LookupDesc), C.POINTER(PrefixDesc), C.POINTER(SamplingDesc),
-                                          C.POINTER(ScoreDesc), C.c_void_p]
     L.fo1_slots_open.restype = C.c_int
     L.fo1_slots_open.argtypes = [C.c_void_p, C.POINTER(SlotsDesc), C.c_void_p]
     L.fo1_slots_admit.restype = C.c_int

@@ -309,7 +309,7 @@ __global__ void beam_finalize_kernel(BeamArgs a) {
 
 // ------------------------------------------------------------------------------------------ host
 int beam_check(const fo1_generate_desc* d, const fo1_beam_desc* bm, int vocab) {
-  const char* fn = "fo1_llm_generate_beam";
+  const char* fn = "fo1_llm_generate: beam";
   const int N = bm->num_beams;
   FO1_CHECK_ARG(N >= 2 && N <= kBeamMaxBeams, "%s: num_beams %d must be in [2, %d]", fn, N, kBeamMaxBeams);
   FO1_CHECK_ARG(bm->num_return >= 1 && bm->num_return <= N, "%s: num_return %d must be in [1, num_beams = %d]", fn, bm->num_return, N);

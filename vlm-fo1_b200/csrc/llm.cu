@@ -516,9 +516,9 @@ struct SlotPool {
 // the decode mode of a pool: a greedy pool with logits processors draws with top_k 1 from its stored logits rows
 static DecodeMode pool_mode(const SlotPool& p) { return p.mode == DEC_GREEDY && p.proc.tab != nullptr ? DEC_SAMPLED : p.mode; }
 
-// one generate call, described once by llm_generate: the caller's descriptors, the decode mode, the column sink, and the device state
-// of beam search (with its host table of length-penalty divisors) or of prompt lookup; or one admission into / decode segment of a
-// slot pool (`pool`; an admission's host slot list `slots`)
+// one generate call, described once by llm_generate: the caller's descriptors (the options as generate_check normalised them), the
+// decode mode, the column sink, and the device state of beam search (with its host table of length-penalty divisors) or of prompt
+// lookup; or one admission into / decode segment of a slot pool (`pool`; an admission's host slot list `slots`)
 struct GenerateCall {
   fo1_generate_desc* d;
   const fo1_prefix_desc* px;        // shared prefix (null: none)
@@ -1061,7 +1061,7 @@ static int stream_resolve(const fo1_stream_desc* h, StreamArgs* sa) {
     const bool host = cudaPointerGetAttributes(&at, hp[i]) == cudaSuccess && at.type == cudaMemoryTypeHost;
     if (!host || cudaHostGetDevicePointer(&dp[i], const_cast<void*>(hp[i]), 0) != cudaSuccess || dp[i] == nullptr) {
       cudaGetLastError();
-      set_error("fo1_llm_generate_streamed: stream buffer `%s` is not pinned host memory mapped for the device (cudaHostAlloc, "
+      set_error("fo1_llm_generate: stream: stream buffer `%s` is not pinned host memory mapped for the device (cudaHostAlloc, "
                 "or cudaHostRegister with cudaHostRegisterMapped)", names[i]);
       return FO1_ERR_INVALID_ARG;
     }
@@ -1071,40 +1071,68 @@ static int stream_resolve(const fo1_stream_desc* h, StreamArgs* sa) {
   return FO1_OK;
 }
 
-// host checks of a shared-prefix call (fo1_llm_generate_prefixed): before the model or the device is touched
+// host checks of a shared-prefix call: before the model or the device is touched
 static int prefix_check(const fo1_generate_desc* d, const fo1_prefix_desc* px) {
   FO1_CHECK_ARG(px->n_groups > 0 && px->prefix_lens && px->prefix_embeds && px->prefix_position_ids && px->seq_group,
-                "fo1_llm_generate_prefixed: null prefix argument");
-  FO1_CHECK_ARG(d->n_seqs > 0 && d->seq_lens, "fo1_llm_generate_prefixed: null argument");
-  FO1_CHECK_ARG(d->all_logits == nullptr, "fo1_llm_generate_prefixed: all_logits is not available with a shared prefix");
+                "fo1_llm_generate: prefix: null prefix argument");
+  FO1_CHECK_ARG(d->n_seqs > 0 && d->seq_lens, "fo1_llm_generate: prefix: null argument");
+  FO1_CHECK_ARG(d->all_logits == nullptr, "fo1_llm_generate: prefix: all_logits is not available with a shared prefix");
   std::vector<int> members(px->n_groups, 0);
   for (int b = 0; b < d->n_seqs; ++b) {
     const int g = px->seq_group[b];
-    FO1_CHECK_ARG(g >= -1 && g < px->n_groups, "fo1_llm_generate_prefixed: sequence %d: group %d out of range [-1, %d)", b, g, px->n_groups);
+    FO1_CHECK_ARG(g >= -1 && g < px->n_groups, "fo1_llm_generate: prefix: sequence %d: group %d out of range [-1, %d)", b, g, px->n_groups);
     if (g < 0) continue;
     ++members[g];
     FO1_CHECK_ARG(px->prefix_lens[g] >= 1 && px->prefix_lens[g] < d->seq_lens[b],
-                  "fo1_llm_generate_prefixed: sequence %d: prefix %d rows, length %d (1 <= P < L)", b, px->prefix_lens[g], d->seq_lens[b]);
+                  "fo1_llm_generate: prefix: sequence %d: prefix %d rows, length %d (1 <= P < L)", b, px->prefix_lens[g], d->seq_lens[b]);
   }
   for (int g = 0; g < px->n_groups; ++g)
-    FO1_CHECK_ARG(members[g] >= 2, "fo1_llm_generate_prefixed: group %d has %d member(s) (at least 2)", g, members[g]);
+    FO1_CHECK_ARG(members[g] >= 2, "fo1_llm_generate: prefix: group %d has %d member(s) (at least 2)", g, members[g]);
   return FO1_OK;
 }
 
-int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, const fo1_score_desc* sc, const fo1_stream_desc* stm,
-                 cudaStream_t s, const fo1_prefix_desc* px = nullptr, const fo1_beam_desc* bmd = nullptr,
-                 const fo1_lookup_desc* lkd = nullptr, const fo1_processor_desc* pr = nullptr) {
-  if (sc != nullptr && sc->logprobs == nullptr && sc->scores == nullptr && sc->logits == nullptr) sc = nullptr;   // nothing to score
-  if (pr) {       // no sequence with a set: the call without processors
-    FO1_CHECK_ARG(pr->seq_set != nullptr, "fo1_llm_generate_processed: null seq_set");
+// the option pointers of d into q, normalised (an option that asks for nothing is the call without it), then the combination table
+// of include/fo1.h, then each option's checks: all before anything is enqueued.  Only the beam and processor checks read the model
+// (its vocabulary); the per-sequence host arrays are the caller's, and need neither the model nor the device.
+static int generate_check(Model* m, fo1_generate_desc* d, GenerateCall& q) {
+  q.d = d; q.sp = d->sampling; q.sc = d->scores; q.stm = d->stream; q.px = d->prefix; q.pr = d->processors; q.lkd = d->lookup;
+  q.bmd = d->beam;
+  if (q.sc != nullptr && q.sc->logprobs == nullptr && q.sc->scores == nullptr && q.sc->logits == nullptr) q.sc = nullptr;
+  if (q.px != nullptr && q.px->n_groups == 0) q.px = nullptr;
+  if (q.pr != nullptr) {
+    FO1_CHECK_ARG(q.pr->seq_set != nullptr, "fo1_llm_generate: processors: null seq_set");
     bool any = false;
-    for (int b = 0; b < d->n_seqs; ++b) any |= pr->seq_set[b] >= 0;
-    if (!any) pr = nullptr;
+    for (int b = 0; b < d->n_seqs; ++b) any |= q.pr->seq_set[b] >= 0;
+    if (!any) q.pr = nullptr;
   }
-  if (pr) FO1_TRY(proc_check(pr, d->n_seqs, m->cfg.llm_vocab, "fo1_llm_generate_processed"));
-  // the per-sequence host arrays first: they are the caller's, and need neither the model nor the device
-  if (sp) FO1_TRY(sampling_check(sp, d->n_seqs, sc ? "fo1_llm_generate_scored" : "fo1_llm_generate_sampled"));
-  if (sc) FO1_TRY(raw_rows_check(sp, sc->raw_rows, d->n_seqs, "fo1_llm_generate_scored"));
+  const struct { const void* a; const char* an; const void* b; const char* bn; } refused[] = {
+      {q.bmd, "beam", q.sp, "sampling"}, {q.bmd, "beam", q.sc, "scores"}, {q.bmd, "beam", q.stm, "stream"},
+      {q.bmd, "beam", q.px, "prefix"}, {q.bmd, "beam", q.pr, "processors"}, {q.bmd, "beam", q.lkd, "lookup"},
+      {q.lkd, "lookup", q.stm, "stream"}, {q.lkd, "lookup", q.pr, "processors"}};
+  for (const auto& r : refused)
+    if (r.a != nullptr && r.b != nullptr) {
+      set_error("fo1_llm_generate: %s does not combine with %s", r.an, r.bn);
+      return FO1_ERR_UNSUPPORTED;
+    }
+  FO1_CHECK_ARG(q.stm == nullptr || (q.stm->tokens && q.stm->lens && q.stm->progress), "fo1_llm_generate: stream: null stream buffer "
+                "(tokens, lens and progress are required; cancel may be NULL)");
+  if (q.lkd) FO1_TRY(lookup_check(d, q.lkd));
+  if (q.px) FO1_TRY(prefix_check(d, q.px));
+  if (q.bmd) FO1_TRY(beam_check(d, q.bmd, m->cfg.llm_vocab));
+  if (q.pr) FO1_TRY(proc_check(q.pr, d->n_seqs, m->cfg.llm_vocab, "fo1_llm_generate"));
+  if (q.sp) FO1_TRY(sampling_check(q.sp, d->n_seqs, "fo1_llm_generate: sampling"));
+  if (q.sc) FO1_TRY(raw_rows_check(q.sp, q.sc->raw_rows, d->n_seqs, "fo1_llm_generate: scores"));
+  return FO1_OK;
+}
+
+static int llm_generate(Model* m, fo1_generate_desc* d, cudaStream_t s) {
+  GenerateCall q{};
+  FO1_TRY(generate_check(m, d, q));
+  const fo1_stream_desc* stm = q.stm;
+  const fo1_beam_desc* bmd = q.bmd;
+  const fo1_lookup_desc* lkd = q.lkd;
+  const fo1_processor_desc* pr = q.pr;
+  const fo1_score_desc* sc = q.sc;
   FO1_CHECK_ARG(m->llm.ok, "fo1_llm_generate: model not finalized (LLM weights unresolved)");
   FO1_CHECK_ARG(m->slot_pool == nullptr, "fo1_llm_generate: a slot pool is open on this model (it owns the K/V cache); fo1_slots_close first");
   const fo1_model_config& c = m->cfg;
@@ -1117,8 +1145,6 @@ int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, co
     FO1_CHECK_ARG(d->seq_lens[b] > 0, "fo1_llm_generate: sequence %d is empty", b);
     max_len = std::max(max_len, d->seq_lens[b]);
   }
-  GenerateCall q{};
-  q.d = d; q.px = px; q.sp = sp; q.sc = sc; q.stm = stm; q.bmd = bmd; q.lkd = lkd; q.pr = pr;
   ColumnSink& k = q.k;
   if (stm) {
     FO1_TRY(stream_resolve(stm, &k.stream));
@@ -1129,7 +1155,7 @@ int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, co
   k.n_stop = d->n_stop_ids; k.pad_id = d->pad_id; k.max_new = d->max_new_tokens;
   k.out_tokens = d->out_tokens; k.out_lens = d->out_lens;
   // a greedy call with logits processors draws with top_k 1 (bit-identical to the arg-max) from the stored, processed rows
-  q.mode = bmd ? DEC_BEAM : sc ? DEC_SCORED : sp || pr ? DEC_SAMPLED : DEC_GREEDY;
+  q.mode = bmd ? DEC_BEAM : sc ? DEC_SCORED : q.sp || pr ? DEC_SAMPLED : DEC_GREEDY;
   if (pr) {
     std::vector<int> tab;
     proc_table(proc_sets(pr), tab, q.proc_bias);
@@ -1151,7 +1177,7 @@ int llm_generate(Model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, co
   // call's verify rows write up to K rows past the sequence's last position
   const int n_drafts = lkd ? std::min(lkd->num_tokens, kLookupMaxDrafts) : 0;
   const int cap = max_len + std::max(d->max_new_tokens, 1) + n_drafts;
-  FO1_TRY(ensure_kv(m, rows, px ? (cap + 63) / 64 * 64 : cap));
+  FO1_TRY(ensure_kv(m, rows, q.px ? (cap + 63) / 64 * 64 : cap));
   FO1_TRY(int_cache_trim(m));
   if (bmd) {
     BeamArgs& a = q.beam;
@@ -1554,61 +1580,7 @@ extern "C" int fo1_llm_build_embeds(fo1_model* m, const int32_t* src_kind, const
 
 extern "C" int fo1_llm_generate(fo1_model* m, fo1_generate_desc* d, void* stream) {
   FO1_CHECK_ARG(m && d, "fo1_llm_generate: null argument");
-  return llm_generate(m, d, nullptr, nullptr, nullptr, static_cast<cudaStream_t>(stream));
-}
-
-extern "C" int fo1_llm_generate_sampled(fo1_model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, void* stream) {
-  FO1_CHECK_ARG(m && d, "fo1_llm_generate_sampled: null argument");
-  return llm_generate(m, d, sp, nullptr, nullptr, static_cast<cudaStream_t>(stream));
-}
-
-extern "C" int fo1_llm_generate_scored(fo1_model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, const fo1_score_desc* sc,
-                                       void* stream) {
-  FO1_CHECK_ARG(m && d, "fo1_llm_generate_scored: null argument");
-  return llm_generate(m, d, sp, sc, nullptr, static_cast<cudaStream_t>(stream));
-}
-
-extern "C" int fo1_llm_generate_streamed(fo1_model* m, fo1_generate_desc* d, const fo1_sampling_desc* sp, const fo1_score_desc* sc,
-                                         const fo1_stream_desc* st, void* stream) {
-  FO1_CHECK_ARG(m && d, "fo1_llm_generate_streamed: null argument");
-  FO1_CHECK_ARG(st == nullptr || (st->tokens && st->lens && st->progress), "fo1_llm_generate_streamed: null stream buffer (tokens, lens and "
-                "progress are required; cancel may be NULL)");
-  return llm_generate(m, d, sp, sc, st, static_cast<cudaStream_t>(stream));
-}
-
-extern "C" int fo1_llm_generate_prefixed(fo1_model* m, fo1_generate_desc* d, const fo1_prefix_desc* px, const fo1_sampling_desc* sp,
-                                         const fo1_score_desc* sc, const fo1_stream_desc* st, void* stream) {
-  if (px != nullptr && px->n_groups == 0) px = nullptr;
-  FO1_CHECK_ARG(m && d, "fo1_llm_generate_prefixed: null argument");
-  FO1_CHECK_ARG(st == nullptr || (st->tokens && st->lens && st->progress), "fo1_llm_generate_prefixed: null stream buffer (tokens, lens and "
-                "progress are required; cancel may be NULL)");
-  if (px) FO1_TRY(prefix_check(d, px));
-  return llm_generate(m, d, sp, sc, st, static_cast<cudaStream_t>(stream), px);
-}
-
-extern "C" int fo1_llm_generate_processed(fo1_model* m, fo1_generate_desc* d, const fo1_prefix_desc* px, const fo1_sampling_desc* sp,
-                                          const fo1_score_desc* sc, const fo1_stream_desc* st, const fo1_processor_desc* pr, void* stream) {
-  if (px != nullptr && px->n_groups == 0) px = nullptr;
-  FO1_CHECK_ARG(m && d, "fo1_llm_generate_processed: null argument");
-  FO1_CHECK_ARG(st == nullptr || (st->tokens && st->lens && st->progress), "fo1_llm_generate_processed: null stream buffer (tokens, lens and "
-                "progress are required; cancel may be NULL)");
-  if (px) FO1_TRY(prefix_check(d, px));
-  return llm_generate(m, d, sp, sc, st, static_cast<cudaStream_t>(stream), px, nullptr, nullptr, pr);
-}
-
-extern "C" int fo1_llm_generate_beam(fo1_model* m, fo1_generate_desc* d, const fo1_beam_desc* bm, void* stream) {
-  FO1_CHECK_ARG(m && d && bm, "fo1_llm_generate_beam: null argument");
-  FO1_TRY(beam_check(d, bm, m->cfg.llm_vocab));
-  return llm_generate(m, d, nullptr, nullptr, nullptr, static_cast<cudaStream_t>(stream), nullptr, bm);
-}
-
-extern "C" int fo1_llm_generate_lookup(fo1_model* m, fo1_generate_desc* d, const fo1_lookup_desc* lk, const fo1_prefix_desc* px,
-                                       const fo1_sampling_desc* sp, const fo1_score_desc* sc, void* stream) {
-  if (px != nullptr && px->n_groups == 0) px = nullptr;
-  FO1_CHECK_ARG(m && d && lk, "fo1_llm_generate_lookup: null argument");
-  FO1_TRY(lookup_check(d, lk));
-  if (px) FO1_TRY(prefix_check(d, px));
-  return llm_generate(m, d, sp, sc, nullptr, static_cast<cudaStream_t>(stream), px, nullptr, lk);
+  return llm_generate(m, d, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int fo1_slots_open(fo1_model* m, const fo1_slots_desc* o, void* stream) {

@@ -108,14 +108,14 @@ __global__ void lookup_accept_kernel(LookupArgs a, ColumnSink k) {
 }
 
 int lookup_check(const fo1_generate_desc* d, const fo1_lookup_desc* lk) {
-  FO1_CHECK_ARG(lk->num_tokens >= 1, "fo1_llm_generate_lookup: num_tokens %d must be >= 1", lk->num_tokens);
-  FO1_CHECK_ARG(lk->max_ngram >= 1, "fo1_llm_generate_lookup: max_ngram %d must be >= 1", lk->max_ngram);
-  FO1_CHECK_ARG(d->n_seqs > 0 && d->seq_lens, "fo1_llm_generate_lookup: null argument");
-  FO1_CHECK_ARG(lk->corpus_offsets != nullptr, "fo1_llm_generate_lookup: null corpus_offsets");
-  FO1_CHECK_ARG(lk->corpus_offsets[0] == 0, "fo1_llm_generate_lookup: corpus_offsets[0] = %d must be 0", lk->corpus_offsets[0]);
+  FO1_CHECK_ARG(lk->num_tokens >= 1, "fo1_llm_generate: lookup: num_tokens %d must be >= 1", lk->num_tokens);
+  FO1_CHECK_ARG(lk->max_ngram >= 1, "fo1_llm_generate: lookup: max_ngram %d must be >= 1", lk->max_ngram);
+  FO1_CHECK_ARG(d->n_seqs > 0 && d->seq_lens, "fo1_llm_generate: lookup: null argument");
+  FO1_CHECK_ARG(lk->corpus_offsets != nullptr, "fo1_llm_generate: lookup: null corpus_offsets");
+  FO1_CHECK_ARG(lk->corpus_offsets[0] == 0, "fo1_llm_generate: lookup: corpus_offsets[0] = %d must be 0", lk->corpus_offsets[0]);
   for (int b = 0; b < d->n_seqs; ++b)
-    FO1_CHECK_ARG(lk->corpus_offsets[b + 1] >= lk->corpus_offsets[b], "fo1_llm_generate_lookup: corpus_offsets decrease at sequence %d", b);
-  FO1_CHECK_ARG(lk->corpus != nullptr || lk->corpus_offsets[d->n_seqs] == 0, "fo1_llm_generate_lookup: null corpus");
+    FO1_CHECK_ARG(lk->corpus_offsets[b + 1] >= lk->corpus_offsets[b], "fo1_llm_generate: lookup: corpus_offsets decrease at sequence %d", b);
+  FO1_CHECK_ARG(lk->corpus != nullptr || lk->corpus_offsets[d->n_seqs] == 0, "fo1_llm_generate: lookup: null corpus");
   return FO1_OK;
 }
 

@@ -36,7 +36,7 @@ struct LookupArgs {
   int* accepted;       // [B] drafts accepted
 };
 
-// host: the checks of fo1_llm_generate_lookup (no CUDA call)
+// host: the checks of fo1_llm_generate with d.lookup (no CUDA call)
 int lookup_check(const fo1_generate_desc* d, const fo1_lookup_desc* lk);
 // the arena carve-out (sized by the dry run like every other buffer)
 template <typename ArenaT>

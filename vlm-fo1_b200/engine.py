@@ -208,7 +208,10 @@ class GenerateDescC(C.Structure):
                 ("position_ids", C.c_void_p), ("rope_deltas", C.POINTER(C.c_int32)), ("max_new_tokens", C.c_int32),
                 ("stop_ids", C.POINTER(C.c_int32)), ("n_stop_ids", C.c_int32), ("pad_id", C.c_int32),
                 ("out_tokens", C.c_void_p), ("out_lens", C.c_void_p), ("prefill_logits", C.c_void_p),
-                ("all_logits", C.c_void_p), ("early_exit_interval", C.c_int32), ("steps_run", C.c_int32), ("rope_deltas_device", C.c_void_p)]
+                ("all_logits", C.c_void_p), ("early_exit_interval", C.c_int32), ("steps_run", C.c_int32), ("rope_deltas_device", C.c_void_p),
+                ("sampling", C.POINTER(_lib.SamplingDesc)), ("scores", C.POINTER(_lib.ScoreDesc)), ("stream", C.POINTER(_lib.StreamDesc)),
+                ("prefix", C.POINTER(_lib.PrefixDesc)), ("processors", C.POINTER(_lib.ProcessorDesc)), ("lookup", C.POINTER(_lib.LookupDesc)),
+                ("beam", C.POINTER(_lib.BeamDesc))]
 
 
 def splice_plan(input_ids: Sequence[int], image_grids: Sequence[Tuple[int, int]], n_regions: int,
@@ -436,27 +439,20 @@ def _engine_generate(self, inputs_embeds: torch.Tensor, position_ids: torch.Tens
     int32 [B * num_return, max_new] / ``lens`` [B * num_return] hold each prompt's best hypotheses, best first; added are
     ``sequence_scores`` fp32 [B * num_return], ``beam_indices`` int32 [B * num_return, max_new] (prompt * N + beam, -1 past the
     length) and ``beam_steps`` int32 [B] (the steps each prompt ran).  ``want_scores`` / ``want_logits`` give [max_new, B * N, V]
-    log-prob / raw rows; ``want_logprobs`` [B * num_return, max_new] the returned tokens' log-probabilities.  Sampling, streaming,
-    prefixes, ``raw_rows`` and ``want_all_logits`` are refused.
+    log-prob / raw rows; ``want_logprobs`` [B * num_return, max_new] the returned tokens' log-probabilities.  ``raw_rows`` is unread.
 
     Prompt lookup (include/fo1.h, fo1_lookup_desc): with ``lookup``, each step drafts tokens from the sequence's corpus and verifies
     them in one step of B * (K + 1) rows on the per-kernel decode path.  Tokens, lengths, logprobs and the score rows up to each
     length are bit-identical to the same call on the per-kernel path without lookup (FO1_NO_MEGA=1); against the persistent
     kernel (B <= 32 by default) they agree as any two decode paths do (DESIGN.md §2).  ``steps_run`` counts verify steps; added
     are ``lookup_steps`` / ``lookup_accepted`` int32 [B] (verify steps each sequence took part in, drafts it accepted).
-    Streaming and beams are refused.
 
     Logits processors (include/fo1.h, fo1_processor_desc): with ``processors``, each sequence's rows are edited by its ProcessorSet
     before its token is chosen; a sequence without one is bit-identical to the call without processors.  ``logits`` stays raw,
-    ``scores`` and ``logprobs`` follow the processed rows.  Beams and lookup are refused."""
-    if processors is not None and (beams is not None or lookup is not None):
-        raise ValueError("logits processors do not combine with `beams` or `lookup`")
-    if lookup is not None and (beams is not None or on_tokens is not None):
-        raise ValueError("prompt lookup does not take `beams` or `on_tokens`")
-    if beams is not None:
-        return self._generate_beam(inputs_embeds, position_ids, seq_lens, rope_deltas, max_new_tokens, stop_ids, pad_id, beams,
-                                   want_prefill_logits, early_exit_interval, want_logprobs, want_scores, want_logits, sampling, raw_rows,
-                                   on_tokens, prefix, want_all_logits)
+    ``scores`` and ``logprobs`` follow the processed rows.
+
+    Which options combine is the library's rule (include/fo1.h, fo1_llm_generate): a refused pair raises Fo1Error before anything
+    is enqueued."""
     B = len(seq_lens)
     V = self.cfg.llm["vocab_size"]
     pre = [0] * B
@@ -468,13 +464,15 @@ def _engine_generate(self, inputs_embeds: torch.Tensor, position_ids: torch.Tens
     inputs_embeds = inputs_embeds.contiguous()
     position_ids = position_ids.to(self.device, torch.int32).contiguous()
     assert position_ids.shape == (3, T)
-    toks = torch.empty((B, max(max_new_tokens, 1)), dtype=torch.int32, device=self.device)
-    lens = torch.zeros((B,), dtype=torch.int32, device=self.device)
+    # beam search returns num_return hypotheses per prompt and scores each of its N beam rows
+    R, S = (B * int(beams.num_return), B * int(beams.num_beams)) if beams is not None else (B, B)
+    toks = torch.empty((R, max(max_new_tokens, 1)), dtype=torch.int32, device=self.device)
+    lens = torch.zeros((R,), dtype=torch.int32, device=self.device)
     pl = torch.empty((B, V), dtype=torch.float32, device=self.device) if want_prefill_logits else None
     al = torch.empty((T, V), dtype=torch.float32, device=self.device) if want_all_logits else None
-    lp = torch.empty((B, max_new_tokens), dtype=torch.float32, device=self.device) if want_logprobs else None
-    sc = torch.empty((max_new_tokens, B, V), dtype=torch.float32, device=self.device) if want_scores else None
-    lg = torch.empty((max_new_tokens, B, V), dtype=torch.float32, device=self.device) if want_logits else None
+    lp = torch.empty((R, max_new_tokens), dtype=torch.float32, device=self.device) if want_logprobs else None
+    sc = torch.empty((max_new_tokens, S, V), dtype=torch.float32, device=self.device) if want_scores else None
+    lg = torch.empty((max_new_tokens, S, V), dtype=torch.float32, device=self.device) if want_logits else None
     d = GenerateDescC()
     d.n_seqs = B
     sl = (C.c_int32 * B)(*[int(x) for x in seq_lens])
@@ -491,20 +489,26 @@ def _engine_generate(self, inputs_embeds: torch.Tensor, position_ids: torch.Tens
     d.prefill_logits = pl.data_ptr() if pl is not None else None
     d.all_logits = al.data_ptr() if al is not None else None
     d.early_exit_interval = early_exit_interval
-    L = lib()
-    sp_arg = sc_arg = None      # NULL: greedy / unscored (fo1_llm_generate_streamed with NULL arguments is each older entry point)
+    ptr = lambda t: t.data_ptr() if t is not None else None
     if sampling is not None:
         sd, _keep = _lib.sampling_desc(sampling.temperature, sampling.top_p, sampling.top_k, sampling.seed)
         assert len(sampling.temperature) == B, "one sampling parameter set per sequence"
-        sp_arg = C.byref(sd)
-    if lp is not None or sc is not None or lg is not None:
-        ptr = lambda t: t.data_ptr() if t is not None else None
+        d.sampling = C.pointer(sd)
+    extra = {}
+    if beams is not None:
+        seq_scores = torch.empty((R,), dtype=torch.float32, device=self.device)
+        bidx = torch.empty((R, max(max_new_tokens, 1)), dtype=torch.int32, device=self.device)
+        steps = torch.zeros((B,), dtype=torch.int32, device=self.device)
+        bd = _lib.BeamDesc(int(beams.num_beams), int(beams.n_keep), float(beams.length_penalty), beams.code(), int(beams.num_return),
+                           seq_scores.data_ptr(), bidx.data_ptr(), steps.data_ptr(), ptr(sc), ptr(lg), ptr(lp))
+        d.beam = C.pointer(bd)
+        extra.update(sequence_scores=seq_scores, beam_indices=bidx, beam_steps=steps)
+    elif lp is not None or sc is not None or lg is not None:
         rr = (C.c_int32 * B)(*[int(x) for x in raw_rows]) if raw_rows is not None else None
         assert raw_rows is None or len(raw_rows) == B, "one raw_rows flag per sequence"
-        desc = _lib.ScoreDesc(ptr(lp), ptr(sc), ptr(lg), rr)
-        sc_arg = C.byref(desc)
+        scd = _lib.ScoreDesc(ptr(lp), ptr(sc), ptr(lg), rr)
+        d.scores = C.pointer(scd)
 
-    px_arg = None
     if prefix is not None:
         G = len(prefix.lens)
         pe = prefix.embeds.contiguous()
@@ -513,89 +517,26 @@ def _engine_generate(self, inputs_embeds: torch.Tensor, position_ids: torch.Tens
         assert pp.shape == (3, pe.shape[0])
         px = _lib.PrefixDesc(G, (C.c_int32 * max(G, 1))(*[int(x) for x in prefix.lens]), pe.data_ptr(), pp.data_ptr(),
                              (C.c_int32 * B)(*[int(g) for g in prefix.seq_group]))
-        px_arg = C.byref(px)
+        d.prefix = C.pointer(px)
 
-    pr_arg = None
     if processors is not None and any(x is not None for x in processors.sets):
         prd, _pr_keep = _processor_desc(processors, B)
-        pr_arg = C.byref(prd)
+        d.processors = C.pointer(prd)
 
-    lk_out = None
     if lookup is not None:
-        lk, _lk_keep, lk_steps, lk_acc = _lookup_desc(lookup, B, self.device)
-        lk_out = (lk_steps, lk_acc)
+        lk, _lk_keep, extra["lookup_steps"], extra["lookup_accepted"] = _lookup_desc(lookup, B, self.device)
+        d.lookup = C.pointer(lk)
+
+    L = lib()
 
     def launch(stream, st=None):
-        sa = C.byref(st) if st is not None else None
-        if lookup is not None:
-            check(L.fo1_llm_generate_lookup(self._h, C.byref(d), C.byref(lk), px_arg, sp_arg, sc_arg, stream), "fo1_llm_generate_lookup")
-        elif pr_arg is not None:
-            check(L.fo1_llm_generate_processed(self._h, C.byref(d), px_arg, sp_arg, sc_arg, sa, pr_arg, stream), "fo1_llm_generate_processed")
-        elif px_arg is None:
-            check(L.fo1_llm_generate_streamed(self._h, C.byref(d), sp_arg, sc_arg, sa, stream), "fo1_llm_generate_streamed")
-        else:
-            check(L.fo1_llm_generate_prefixed(self._h, C.byref(d), px_arg, sp_arg, sc_arg, sa, stream), "fo1_llm_generate_prefixed")
+        d.stream = C.pointer(st) if st is not None else None
+        check(L.fo1_llm_generate(self._h, C.byref(d), stream), "fo1_llm_generate")
     if on_tokens is None:
         launch(_stream())
     else:
         self._run_streamed(launch, B, max_new_tokens, on_tokens)
-    out = dict(tokens=toks, lens=lens, prefill_logits=pl, all_logits=al, steps_run=d.steps_run)
-    if lk_out is not None:
-        out["lookup_steps"], out["lookup_accepted"] = lk_out
-    if want_logprobs:
-        out["logprobs"] = lp
-    if want_scores:
-        out["scores"] = sc
-    if want_logits:
-        out["logits"] = lg
-    return out
-
-
-def _engine_generate_beam(self, inputs_embeds, position_ids, seq_lens, rope_deltas, max_new_tokens, stop_ids, pad_id, beams: Beams,
-                          want_prefill_logits, early_exit_interval, want_logprobs, want_scores, want_logits, sampling, raw_rows, on_tokens, prefix,
-                          want_all_logits):
-    """Engine.generate with ``beams`` (fo1_llm_generate_beam)."""
-    for name, v in (("sampling", sampling), ("raw_rows", raw_rows), ("on_tokens", on_tokens), ("prefix", prefix)):
-        if v is not None:
-            raise ValueError(f"beam search does not take `{name}`")
-    if want_all_logits:
-        raise ValueError("beam search does not take `want_all_logits`")
-    B, N, nr = len(seq_lens), int(beams.num_beams), int(beams.num_return)
-    V, T = self.cfg.llm["vocab_size"], max(int(max_new_tokens), 1)
-    assert inputs_embeds.shape == (int(sum(seq_lens)), self.cfg.llm["hidden_size"]) and inputs_embeds.dtype == torch.bfloat16
-    inputs_embeds = inputs_embeds.contiguous()
-    position_ids = position_ids.to(self.device, torch.int32).contiguous()
-    dev = self.device
-    toks = torch.empty((B * nr, T), dtype=torch.int32, device=dev)
-    lens = torch.zeros((B * nr,), dtype=torch.int32, device=dev)
-    seq_scores = torch.empty((B * nr,), dtype=torch.float32, device=dev)
-    bidx = torch.empty((B * nr, T), dtype=torch.int32, device=dev)
-    steps = torch.zeros((B,), dtype=torch.int32, device=dev)
-    pl = torch.empty((B, V), dtype=torch.float32, device=dev) if want_prefill_logits else None
-    sc = torch.empty((T, B * N, V), dtype=torch.float32, device=dev) if want_scores else None
-    lg = torch.empty((T, B * N, V), dtype=torch.float32, device=dev) if want_logits else None
-    lp = torch.empty((B * nr, T), dtype=torch.float32, device=dev) if want_logprobs else None
-    d = GenerateDescC()
-    d.n_seqs = B
-    sl = (C.c_int32 * B)(*[int(x) for x in seq_lens])
-    dev_deltas = rope_deltas if isinstance(rope_deltas, torch.Tensor) else None
-    rd = (C.c_int32 * B)(*([0] * B if dev_deltas is not None else [int(x) for x in rope_deltas]))
-    if dev_deltas is not None:
-        assert dev_deltas.is_cuda and dev_deltas.dtype == torch.int32 and dev_deltas.numel() == B
-        d.rope_deltas_device = dev_deltas.data_ptr()
-    st = (C.c_int32 * max(len(stop_ids), 1))(*[int(x) for x in stop_ids])
-    d.seq_lens, d.rope_deltas, d.stop_ids, d.n_stop_ids = sl, rd, st, len(stop_ids)
-    d.inputs_embeds, d.position_ids = inputs_embeds.data_ptr(), position_ids.data_ptr()
-    d.max_new_tokens, d.pad_id = max_new_tokens, pad_id
-    d.out_tokens, d.out_lens = toks.data_ptr(), lens.data_ptr()
-    d.prefill_logits = pl.data_ptr() if pl is not None else None
-    d.early_exit_interval = early_exit_interval
-    ptr = lambda t: t.data_ptr() if t is not None else None
-    bd = _lib.BeamDesc(N, int(beams.n_keep), float(beams.length_penalty), beams.code(), nr, seq_scores.data_ptr(), bidx.data_ptr(),
-                       steps.data_ptr(), ptr(sc), ptr(lg), ptr(lp))
-    check(lib().fo1_llm_generate_beam(self._h, C.byref(d), C.byref(bd), _stream()), "fo1_llm_generate_beam")
-    out = dict(tokens=toks, lens=lens, prefill_logits=pl, all_logits=None, steps_run=d.steps_run, sequence_scores=seq_scores,
-               beam_indices=bidx, beam_steps=steps)
+    out = dict(tokens=toks, lens=lens, prefill_logits=pl, all_logits=al, steps_run=d.steps_run, **extra)
     if want_logprobs:
         out["logprobs"] = lp
     if want_scores:
@@ -735,7 +676,7 @@ def _engine_stream_buffers(self, B: int, T: int):
 
 
 def _engine_run_streamed(self, launch, B: int, T: int, on_tokens) -> None:
-    """Run ``launch(stream, StreamDesc)`` (one fo1_llm_generate_streamed call) in a worker thread and deliver the published columns
+    """Run ``launch(stream, StreamDesc)`` (one streamed fo1_llm_generate call) in a worker thread and deliver the published columns
     to ``on_tokens`` from this thread.  The worker enqueues on this thread's current stream, on the engine's device (the library
     does not set the device), and records an event after the call; the per-kernel path's host loop blocks in that call, so it
     must not run where the polling does.  Polling ends on `done`, on the worker's failure (its Fo1Error is raised), or once the
@@ -791,7 +732,6 @@ def _engine_run_streamed(self, launch, B: int, T: int, on_tokens) -> None:
 
 Engine.build_embeds = _engine_build_embeds
 Engine.generate = _engine_generate
-Engine._generate_beam = _engine_generate_beam
 Engine._stream_buffers = _engine_stream_buffers
 Engine._run_streamed = _engine_run_streamed
 Engine.sample_tokens = staticmethod(sample_tokens)
