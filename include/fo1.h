@@ -521,6 +521,46 @@ struct fo1_prefix_desc {
  * range, at least two members per group, P_g < L_b for every member, non-NULL pointers, and no all_logits. */
 
 /* ------------------------------------------------------------------------------------------------
+ * Teacher-forced scoring (the reference's forward(labels=...): omchat_qwen2_5_vl.py:466-532 with HF's ForCausalLMLoss).  The prefill
+ * of fo1_llm_generate (same layers, same launches, optionally a shared prefix), then, instead of decoding, the log-likelihood of each
+ * scored row's target under the LM head: only the scored rows are gathered, normed (the kernel the all_logits output uses) and run
+ * through the LM-head GEMM with a log-likelihood epilogue; nothing vocabulary-sized is written unless all_logits is asked for.
+ *
+ * Rows are the packed rows of the FULL sequences (sum L_b, sequence b's rows back to back), with or without a prefix, as all_logits
+ * lays them out.  targets[r] is the id row r predicts (the labels already shifted by one), or -100: not scored.  Per scored row:
+ *   target_logit  the fp32 logit of the target, bit-identical to all_logits[r][target]
+ *   lse           log sum_v exp(logit_v), from per-128-column partials (max, sum of exp(x - max)) merged in column order
+ *   greedy        1 when the target is the lowest-index maximum of the row
+ *   logprobs[r]   target_logit - lse (0 where the row is not scored)
+ * and per sequence seq_logprob = the fp64 sum of its rows' logprobs in row order, seq_count = its scored rows.  Every reduction runs
+ * in an order that depends on the row alone: a sequence's outputs are bit-identical whatever else is in the call and with or
+ * without its prefix shared.
+ *
+ * Checked on the host before anything is enqueued, with the message "fo1_llm_loglik: <rule>": non-NULL inputs and outputs, targets
+ * in [0, vocab) or -100, no scored last row of a sequence (it has nothing to predict), no scored row inside a shared prefix (the
+ * row predicting the first own token is itself an own row), no all_logits with a prefix (as fo1_llm_generate), no open slot pool
+ * (the call writes the K/V cache, as fo1_llm_generate does).
+ *
+ * ABI: fo1_llm_loglik and fo1_loglik_desc are additions; no existing declaration changed, so FO1_ABI_VERSION stays 4.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct {
+  int32_t n_seqs;
+  const int32_t* seq_lens;         /* HOST [n_seqs]: L_b after the splice */
+  const void* inputs_embeds;       /* DEVICE bf16 [rows][llm_hidden]: every row, or with `prefix` only each sequence's own rows */
+  const int32_t* position_ids;     /* DEVICE int32 [3][rows], rows as inputs_embeds */
+  const fo1_prefix_desc* prefix;   /* optional shared prefix (fo1_prefix_desc, checked as fo1_llm_generate checks it) */
+  const int32_t* targets;          /* HOST int32 [sum L_b]: HOST because the host checks them and sizes the head from them */
+  float* logprobs;                 /* DEVICE fp32 [sum L_b] */
+  int32_t* greedy;                 /* optional DEVICE int32 [sum L_b] (0 where not scored) */
+  double* seq_logprob;             /* DEVICE fp64 [n_seqs] */
+  int32_t* seq_count;              /* DEVICE int32 [n_seqs] */
+  float* all_logits;               /* optional DEVICE fp32 [sum L_b][vocab], as fo1_llm_generate's (refused with prefix) */
+  float* lse;                      /* optional DEVICE fp32 [n_scored]: lse of the scored rows, in row order */
+  float* target_logits;            /* optional DEVICE fp32 [n_scored]: their target logits, in row order */
+} fo1_loglik_desc;
+int fo1_llm_loglik(fo1_model* m, const fo1_loglik_desc* d, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Beam search (HF generate with num_beams > 1 and do_sample=False: transformers' GenerationMixin._beam_search and its helpers).
  * Each of the n_seqs prompts runs as if it were alone in the call, with num_beams = N decode rows and cache slots.  Per step,
  * over log_softmax(logits) of the running beams: accumulated = log-prob + running score (initially [0, -1e9, ...]); the best

@@ -93,6 +93,15 @@ class PrefixAttnDesc(C.Structure):
                 ("kv_heads", C.c_int32), ("head_dim", C.c_int32), ("scale", C.c_float), ("out", C.c_void_p), ("ldo", C.c_int64)]
 
 
+class LoglikDesc(C.Structure):
+    """fo1_loglik_desc: HOST seq_lens [n] and targets [sum L]; DEVICE embeddings, positions [3][rows], outputs logprobs / greedy
+    [sum L], seq_logprob fp64 / seq_count [n], all_logits [sum L][V], lse / target_logits [n_scored]."""
+    _fields_ = [("n_seqs", C.c_int32), ("seq_lens", C.POINTER(C.c_int32)), ("inputs_embeds", C.c_void_p), ("position_ids", C.c_void_p),
+                ("prefix", C.POINTER(PrefixDesc)), ("targets", C.POINTER(C.c_int32)), ("logprobs", C.c_void_p), ("greedy", C.c_void_p),
+                ("seq_logprob", C.c_void_p), ("seq_count", C.c_void_p), ("all_logits", C.c_void_p), ("lse", C.c_void_p),
+                ("target_logits", C.c_void_p)]
+
+
 class BeamDesc(C.Structure):
     """fo1_beam_desc: HOST parameters; DEVICE outputs sequence_scores [n * num_return], beam_indices [n * num_return][max_new],
     steps_run [n], optional scores / logits [max_new][n * num_beams][V] and logprobs [n * num_return][max_new]."""
@@ -172,6 +181,8 @@ def lib() -> C.CDLL:
                                     C.c_void_p, C.c_size_t, C.c_void_p]
     L.fo1_llm_generate.restype = C.c_int
     L.fo1_llm_generate.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    L.fo1_llm_loglik.restype = C.c_int
+    L.fo1_llm_loglik.argtypes = [C.c_void_p, C.POINTER(LoglikDesc), C.c_void_p]
     L.fo1_logits_process.restype = C.c_int
     L.fo1_logits_process.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.POINTER(ProcessorDesc), C.c_void_p, C.c_int64,
                                      C.POINTER(C.c_int32), C.c_void_p]

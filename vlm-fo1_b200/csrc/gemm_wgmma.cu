@@ -48,6 +48,11 @@ struct GemmArgs {
   // implicit 3x3 / pad 1 / stride 1 convolution over an NHWC map (conv_cpb = C / 64 k-blocks per tap; 0: ordinary GEMM): the A tile of
   // k-block kb is the [Ht][Wt][64] patch of tap kb / conv_cpb, fetched by a 4-D TMA whose out-of-range coordinates read as zero
   int conv_cpb, conv_H, conv_W, conv_Wt;
+  // log-likelihood epilogue (LL instantiation, loglik_head): per row and 128-column tile, (max, lowest index of the max, sum of
+  // exp(x - max)) into ll_part[row][tile] (ll_nparts tiles per row), and the logit of column ll_target[row] into ll_xtgt[row]
+  float4* ll_part; int ll_nparts;
+  const int* ll_target;
+  float* ll_xtgt;
 };
 
 constexpr int kMaxStages = 24;
@@ -349,6 +354,48 @@ __device__ __forceinline__ void epilogue_frag(const GemmArgs& g, float (&acc)[BN
   }
 }
 
+// log-likelihood epilogue: a warp's 16 x BN share of a logits tile -> per row the tile's partial (max, lowest column of the max, sum of
+// exp(x - max) over the columns < N) into ll_part[row][n0 / BN], and the raw fp32 logit of the row's target when it lies in the tile.
+// Every reduction runs in an order fixed by the fragment layout (each thread's columns, then the quad's butterfly, whose lanes all end
+// with the same bits), so a row's partials depend on the row alone.
+template <int BN>
+__device__ __forceinline__ void loglik_frag(const GemmArgs& g, const float (&acc)[BN / 2], int lane, int m_base, int n0) {
+  const int fc = n0 + (lane & 3) * 2;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int m = m_base + (lane >> 2) + h * 8;
+    const int tgt = m < g.M ? __ldg(g.ll_target + m) : -1;
+    float mx = -INFINITY;
+    int ix = 0x7fffffff;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+      for (int c = 0; c < 2; ++c) {
+        const int col = fc + j * 8 + c;
+        const float x = acc[4 * j + 2 * h + c];
+        if (col < g.N && x > mx) { mx = x; ix = col; }   // ascending columns: the first maximum is kept
+        if (col == tgt) g.ll_xtgt[m] = x;
+      }
+    }
+#pragma unroll
+    for (int o = 1; o <= 2; o <<= 1) {
+      const float om = __shfl_xor_sync(0xffffffffu, mx, o);
+      const int oi = __shfl_xor_sync(0xffffffffu, ix, o);
+      if (om > mx || (om == mx && oi < ix)) { mx = om; ix = oi; }
+    }
+    float s = 0.f;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+      for (int c = 0; c < 2; ++c)
+        if (fc + j * 8 + c < g.N) s += expf(acc[4 * j + 2 * h + c] - mx);
+    }
+    s += __shfl_xor_sync(0xffffffffu, s, 1);
+    s += __shfl_xor_sync(0xffffffffu, s, 2);
+    if (m < g.M && (lane & 3) == 0) g.ll_part[(long long)m * g.ll_nparts + n0 / BN] = make_float4(mx, s, __int_as_float(ix), 0.f);
+  }
+}
+
 // one A tile into a ring stage: rows m0 .. m0+127 of the [M][K] matrix, or (implicit conv) the shifted pixel patch of the k-block's tap
 __device__ __forceinline__ void load_a_tile(const GemmArgs& g, const CUtensorMap* tmA, uint32_t dst, uint32_t bar, int kb, int m0) {
   if (g.conv_cpb == 0) {
@@ -410,7 +457,8 @@ __device__ __forceinline__ void release_stage(uint32_t empty_bar, uint32_t rank)
 }
 
 // CL = 1: one CTA per work item.  CL = 2: clusters of two CTAs along M sharing (multicasting) the W tile; split-K is never paired.
-template <int BN, int CL>
+// LL: the log-likelihood epilogue (loglik_frag) in place of the stores; one CTA per tile, no split-K.
+template <int BN, int CL, bool LL = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW, const __grid_constant__ GemmArgs g) {
   static_assert(CL == 1 || CL == 2, "CTA pairs only");
@@ -520,7 +568,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       ptx::wgmma_wait<0>();
       ptx::wgmma_fence_regs(acc);
       if (lane == 0) release_stage<CL>(ptx::smem_u32(empty_bar + prev_s), rank);
-      if (CL == 1 && g.ksplit > 1) {
+      if (!LL && CL == 1 && g.ksplit > 1) {
         // ---- split-K: park the fp32 partial, the last split to arrive reduces + finishes the tile ----
         float* part = g.ws + (long long)(tile * g.ksplit + split) * BM * BN;
         if (live) {
@@ -545,7 +593,11 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
         asm volatile("bar.sync 1, 256;" ::: "memory");   // last_flag is reused by the next work item
         continue;
       }
-      if (live) epilogue_frag<BN>(g, acc, stg, lane, m0 + wrow, n0);
+      if constexpr (LL) {
+        if (live) loglik_frag<BN>(g, acc, lane, m0 + wrow, n0);
+      } else {
+        if (live) epilogue_frag<BN>(g, acc, stg, lane, m0 + wrow, n0);
+      }
     }
   }
   // paired: no CTA leaves while its peer may still multicast into its shared memory or arrive on its barriers
@@ -698,14 +750,24 @@ static int pair_clusters() {
   return n;
 }
 
+// the outputs of the log-likelihood epilogue (see GemmArgs)
+struct LoglikOut { float4* part; const int* target; float* x_tgt; };
+
 template <int BN>
-static int launch_gemm(const fo1_gemm_desc* d, cudaStream_t stream, int ksplit = 1, const ConvInfo* conv = nullptr) {
+static int launch_gemm(const fo1_gemm_desc* d, cudaStream_t stream, int ksplit = 1, const ConvInfo* conv = nullptr, const LoglikOut* ll = nullptr) {
   using Cfg = GemmCfg<BN>;
   static bool attr_set = false;
   if (!attr_set) {
     FO1_CUDA(cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<BN, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
     FO1_CUDA(cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<BN, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
     attr_set = true;
+  }
+  static bool ll_attr_set = false;
+  if constexpr (BN == kLoglikTile) {   // the log-likelihood epilogue is instantiated for its one tile width
+    if (ll != nullptr && !ll_attr_set) {
+      FO1_CUDA(cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<BN, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+      ll_attr_set = true;
+    }
   }
   // CTA pairs: each CTA of a pair loads its own A tile and half of the W tile, multicast into both, which halves the W bytes a CTA pulls
   // per k-block.  Measured on H100, that pays on the large weights (LLM down 2.85 -> 2.55 ms, ViT gated fc1 7.09 -> 6.79 ms with pairs
@@ -715,7 +777,7 @@ static int launch_gemm(const fo1_gemm_desc* d, cudaStream_t stream, int ksplit =
   const int tiles_m = ceil_div(d->M, BM);
   const int num_kb = ceil_div(d->K, BK);
   const int kb_per_split = ceil_div(num_kb, ksplit);
-  const bool paired = tiles_m >= 2 && ceil_div(num_kb, kb_per_split) == 1 && conv == nullptr &&
+  const bool paired = tiles_m >= 2 && ceil_div(num_kb, kb_per_split) == 1 && conv == nullptr && ll == nullptr &&
                       (d->tile_n != 0 || 2LL * d->N * d->K >= kPairMinWeightBytes);
   CUtensorMap tmA, tmW;
   // one m-tile only (decode: M = batch): fetch just the live rows of A, rounded to the 8-row swizzle atom; a live
@@ -764,6 +826,7 @@ static int launch_gemm(const fo1_gemm_desc* d, cudaStream_t stream, int ksplit =
   g.kb_per_split = kb_per_split;
   g.ksplit = ceil_div(num_kb, g.kb_per_split);   // every split owns at least one k-block
   g.ws = nullptr; g.counters = nullptr;
+  g.ll_part = ll ? ll->part : nullptr; g.ll_nparts = g.tiles_n; g.ll_target = ll ? ll->target : nullptr; g.ll_xtgt = ll ? ll->x_tgt : nullptr;
   if (g.ksplit > 1) {
     SplitKScratch* sc = nullptr;
     FO1_TRY(splitk_scratch(stream, (size_t)g.tiles_m * g.tiles_n * g.ksplit * BM * BN * sizeof(float), g.tiles_m * g.tiles_n, &sc));
@@ -779,11 +842,17 @@ static int launch_gemm(const fo1_gemm_desc* d, cudaStream_t stream, int ksplit =
     grid = tiles < device_sm_count() ? tiles : device_sm_count();
   }
   char tag[96] = "gemm";
-  if (g_prof_on) snprintf(tag, sizeof(tag), "%s:%dx%dx%d%s%s", d->M <= 128 ? "gemm_skinny" : "gemm", d->M, d->N, d->K, d->gated ? ":gated" : "", conv ? ":conv3x3" : "");
+  if (g_prof_on) snprintf(tag, sizeof(tag), "%s:%dx%dx%d%s%s", ll ? "gemm_loglik" : d->M <= 128 ? "gemm_skinny" : "gemm", d->M, d->N, d->K,
+                          d->gated ? ":gated" : "", conv ? ":conv3x3" : "");
   ProfScope prof(tag, 2.0 * d->M * (double)d->N * d->K,
                  2.0 * ((double)d->M * d->K + (double)d->N * d->K + (double)d->M * (d->gated ? d->N / 2 : d->N)), stream);
   if (paired) launch_k_cluster(2, gemm_bf16_wgmma_kernel<BN, 2>, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, tmA, tmW, g);
-  else launch_k(gemm_bf16_wgmma_kernel<BN, 1>, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, tmA, tmW, g);
+  else if constexpr (BN == kLoglikTile) {
+    if (ll) launch_k(gemm_bf16_wgmma_kernel<BN, 1, true>, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, tmA, tmW, g);
+    else launch_k(gemm_bf16_wgmma_kernel<BN, 1>, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, tmA, tmW, g);
+  } else {
+    launch_k(gemm_bf16_wgmma_kernel<BN, 1>, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, tmA, tmW, g);
+  }
   FO1_LAUNCH_CHECK();
   return FO1_OK;
 }
@@ -866,6 +935,20 @@ extern "C" int fo1_gemm_bf16(const fo1_gemm_desc* d, void* stream) {
 }
 
 namespace fo1 {
+// X [M][K] . W [N][K]^T reduced by the log-likelihood epilogue in kLoglikTile-column tiles, whatever M: the partial granule, and so
+// every row's bits, never depend on the number of rows.  No split-K: each logit is the fp32 accumulator the FO1_F32 store of the
+// same GEMM would write.  part: [M][ceil(N / kLoglikTile)].
+int loglik_head(const bf16* X, const bf16* W, int M, int N, int K, const int* target, float4* part, float* x_tgt, cudaStream_t stream) {
+  static_assert(kLoglikTile == 128, "loglik_head launches the 128-column instantiation");
+  if (M == 0) return FO1_OK;
+  fo1_gemm_desc d;
+  memset(&d, 0, sizeof(d));
+  d.M = M; d.N = N; d.K = K;
+  d.A = X; d.lda = K; d.W = W; d.ldw = K; d.D = part; d.ldd = N; d.d_dtype = FO1_F32;
+  const LoglikOut ll{part, target, x_tgt};
+  return launch_gemm<kLoglikTile>(&d, stream, 1, nullptr, &ll);
+}
+
 int linear(const bf16* A, long long lda, const bf16* W, long long ldw, void* D, long long ldd, int d_dtype, int M, int N,
            int K, const void* bias, int bias_dtype, int act, const bf16* residual, long long ldr, int gated,
            cudaStream_t stream) {

@@ -18,6 +18,15 @@ int conv3x3_gemm(const bf16* x, int B, int H, int W, int C, const bf16* Wm, bf16
 int linear(const bf16* A, long long lda, const bf16* W, long long ldw, void* D, long long ldd, int d_dtype, int M, int N,
            int K, const void* bias, int bias_dtype, int act, const bf16* residual, long long ldr, int gated,
            cudaStream_t stream);
+// log-likelihood head: the LM-head GEMM with the log-likelihood epilogue (gemm_wgmma.cu), and the merge of its partials (loglik.cu)
+constexpr int kLoglikTile = 128;
+int loglik_head(const bf16* X, const bf16* W, int M, int N, int K, const int* target, float4* part, float* x_tgt, cudaStream_t stream);
+// per scored row i: lse = M* + log sum_t s_t exp(m_t - M*) over its partials in ascending column order; logprobs[out_row[i]] = x_tgt - lse,
+// greedy[out_row[i]] = (lowest index of the maximum == target); lse / x_out (optional) take lse and x_tgt at row i
+int loglik_merge(const float4* part, int n_parts, int M, const int* target, const float* x_tgt, const int* out_row, float* logprobs,
+                 int* greedy, float* lse, float* x_out, cudaStream_t s);
+// seq_logprob[b] = sum of logprobs[off[b] .. off[b + 1]) in ascending row order, in fp64
+int loglik_seq_sum(const float* logprobs, const int* off, int n_seqs, double* seq_logprob, cudaStream_t s);
 
 // ---- norm.cu ----
 // The two row-norm kernels sum a row in different orders, so the CALL SITE names one and keeps it whatever the number of rows: a

@@ -781,6 +781,46 @@ static int prefill_plan(Model* m, const GenerateCall& q, const LayerBuf& b, int 
   return FO1_OK;
 }
 
+// the prefill's layer stack over T packed rows (with a shared prefix: the n_pre prefix rows, then the own rows), from the caller's
+// embeddings and positions through every layer; *x_out: the last layer's output (g.xa or g.xb).  d_lens: the sequences' lengths on
+// the device; pos_all: [3][T] scratch of a prefix call.
+static int prefill_layers(Model* m, const GenerateCall& q, const PrefillAttn& pa, DecodeBufs& g, long long T, int n_pre, float* cs_pre,
+                          int* pos_all, const int* d_lens, cudaStream_t s, bool dry, const bf16** x_out) {
+  const fo1_model_config& c = m->cfg;
+  const fo1_generate_desc* d = q.d;
+  const fo1_prefix_desc* px = q.px;
+  const int B = d->n_seqs, H = c.llm_hidden, hd = c.llm_head_dim, KD = c.llm_kv_heads * hd;
+  LayerBuf& buf = g.layer;
+  const bf16* x = static_cast<const bf16*>(d->inputs_embeds);
+  const int* pos = d->position_ids;
+  FO1_RUN(attention_rowseg(pa.causal.cu_seqlens, pa.causal.n_seqs, pa.causal.total_rows, buf.rowseg, s));
+  if (px) {   // one packed matrix (prefix rows, then own rows) and one position table
+    const size_t no = (size_t)T - n_pre;
+    if (!dry) {
+      FO1_CUDA(cudaMemcpyAsync(g.xb, px->prefix_embeds, (size_t)n_pre * H * sizeof(bf16), cudaMemcpyDeviceToDevice, s));
+      FO1_CUDA(cudaMemcpyAsync(g.xb + (size_t)n_pre * H, d->inputs_embeds, no * H * sizeof(bf16), cudaMemcpyDeviceToDevice, s));
+      FO1_CUDA(cudaMemcpy2DAsync(pos_all, (size_t)T * sizeof(int), px->prefix_position_ids, (size_t)n_pre * sizeof(int), (size_t)n_pre * sizeof(int),
+                                 3, cudaMemcpyDeviceToDevice, s));
+      FO1_CUDA(cudaMemcpy2DAsync(pos_all + n_pre, (size_t)T * sizeof(int), d->position_ids, no * sizeof(int), no * sizeof(int), 3,
+                                 cudaMemcpyDeviceToDevice, s));
+      const size_t layer_stride = (size_t)m->kv_batch * m->kv_cap * KD;
+      kv_zero_tail_kernel<<<dim3(B, c.llm_layers), 128, 0, s>>>(static_cast<bf16*>(m->kv_cache) + (size_t)c.llm_layers * layer_stride,
+                                                                 (long long)layer_stride, d_lens, m->kv_cap, KD);
+      FO1_LAUNCH_CHECK();
+    }
+    x = g.xb;
+    pos = pos_all;
+  }
+  FO1_RUN(mrope_table(pos, cs_pre, (int)T, hd, c.mrope_section[0], c.mrope_section[1], c.mrope_section[2], c.rope_theta, s));
+  for (int li = 0; li < c.llm_layers; ++li) {
+    bf16* xo = (li & 1) ? g.xb : g.xa;
+    FO1_TRY(llm_layer(m, li, x, xo, buf, (int)T, cs_pre, pa, s, dry));
+    x = xo;
+  }
+  *x_out = x;
+  return FO1_OK;
+}
+
 // buffer plan, integer tables and the prefill; then (unless `dry`, the pass that sizes the arena) the decode state and column 0
 static int llm_prefill(Model* m, GenerateCall& q, cudaStream_t s, bool dry, DecodeBufs& g) {
   const fo1_model_config& c = m->cfg;
@@ -789,7 +829,6 @@ static int llm_prefill(Model* m, GenerateCall& q, cudaStream_t s, bool dry, Deco
   const fo1_prefix_desc* px = q.px;
   const bool beam = q.bmd != nullptr, lookup = q.lkd != nullptr;
   const int B = d->n_seqs, H = c.llm_hidden, hd = c.llm_head_dim, V = c.llm_vocab;
-  const int KD = c.llm_kv_heads * hd;
   long long T = 0;      // packed rows through the layers: every sequence's rows, or (px) the prefix rows then the own rows
   int n_pre = 0;
   for (int b = 0; b < B; ++b) T += d->seq_lens[b] - prefix_of(px, b);
@@ -848,32 +887,8 @@ static int llm_prefill(Model* m, GenerateCall& q, cudaStream_t s, bool dry, Deco
   }
 
   // ---- prefill ----
-  const bf16* x = static_cast<const bf16*>(d->inputs_embeds);
-  const int* pos = d->position_ids;
-  FO1_RUN(attention_rowseg(pa.causal.cu_seqlens, pa.causal.n_seqs, pa.causal.total_rows, buf.rowseg, s));
-  if (px) {   // one packed matrix (prefix rows, then own rows) and one position table
-    const size_t no = (size_t)T - n_pre;
-    if (!dry) {
-      FO1_CUDA(cudaMemcpyAsync(g.xb, px->prefix_embeds, (size_t)n_pre * H * sizeof(bf16), cudaMemcpyDeviceToDevice, s));
-      FO1_CUDA(cudaMemcpyAsync(g.xb + (size_t)n_pre * H, d->inputs_embeds, no * H * sizeof(bf16), cudaMemcpyDeviceToDevice, s));
-      FO1_CUDA(cudaMemcpy2DAsync(pos_all, (size_t)T * sizeof(int), px->prefix_position_ids, (size_t)n_pre * sizeof(int), (size_t)n_pre * sizeof(int),
-                                 3, cudaMemcpyDeviceToDevice, s));
-      FO1_CUDA(cudaMemcpy2DAsync(pos_all + n_pre, (size_t)T * sizeof(int), d->position_ids, no * sizeof(int), no * sizeof(int), 3,
-                                 cudaMemcpyDeviceToDevice, s));
-      const size_t layer_stride = (size_t)m->kv_batch * m->kv_cap * KD;
-      kv_zero_tail_kernel<<<dim3(B, c.llm_layers), 128, 0, s>>>(static_cast<bf16*>(m->kv_cache) + (size_t)c.llm_layers * layer_stride,
-                                                                 (long long)layer_stride, d_lens, m->kv_cap, KD);
-      FO1_LAUNCH_CHECK();
-    }
-    x = g.xb;
-    pos = pos_all;
-  }
-  FO1_RUN(mrope_table(pos, cs_pre, (int)T, hd, c.mrope_section[0], c.mrope_section[1], c.mrope_section[2], c.rope_theta, s));
-  for (int li = 0; li < c.llm_layers; ++li) {
-    bf16* xo = (li & 1) ? g.xb : g.xa;
-    FO1_TRY(llm_layer(m, li, x, xo, buf, (int)T, cs_pre, pa, s, dry));
-    x = xo;
-  }
+  const bf16* x = nullptr;
+  FO1_TRY(prefill_layers(m, q, pa, g, T, n_pre, cs_pre, pos_all, d_lens, s, dry, &x));
   if (d->all_logits) {
     FO1_RUN(rmsnorm(x, H, m->llm.norm, alln, H, (int)T, H, c.rms_eps, NORM_WARP, s));
     FO1_RUN(linear(alln, H, m->llm.lm_head, H, d->all_logits, V, FO1_F32, (int)T, V, H, nullptr, 0, FO1_EPI_NONE, nullptr, 0, 0, s));
@@ -1071,23 +1086,23 @@ static int stream_resolve(const fo1_stream_desc* h, StreamArgs* sa) {
   return FO1_OK;
 }
 
-// host checks of a shared-prefix call: before the model or the device is touched
-static int prefix_check(const fo1_generate_desc* d, const fo1_prefix_desc* px) {
+// host checks of a shared-prefix call: before the model or the device is touched.  who: the entry point named in the messages
+static int prefix_check(const fo1_generate_desc* d, const fo1_prefix_desc* px, const char* who = "fo1_llm_generate") {
   FO1_CHECK_ARG(px->n_groups > 0 && px->prefix_lens && px->prefix_embeds && px->prefix_position_ids && px->seq_group,
-                "fo1_llm_generate: prefix: null prefix argument");
-  FO1_CHECK_ARG(d->n_seqs > 0 && d->seq_lens, "fo1_llm_generate: prefix: null argument");
-  FO1_CHECK_ARG(d->all_logits == nullptr, "fo1_llm_generate: prefix: all_logits is not available with a shared prefix");
+                "%s: prefix: null prefix argument", who);
+  FO1_CHECK_ARG(d->n_seqs > 0 && d->seq_lens, "%s: prefix: null argument", who);
+  FO1_CHECK_ARG(d->all_logits == nullptr, "%s: prefix: all_logits is not available with a shared prefix", who);
   std::vector<int> members(px->n_groups, 0);
   for (int b = 0; b < d->n_seqs; ++b) {
     const int g = px->seq_group[b];
-    FO1_CHECK_ARG(g >= -1 && g < px->n_groups, "fo1_llm_generate: prefix: sequence %d: group %d out of range [-1, %d)", b, g, px->n_groups);
+    FO1_CHECK_ARG(g >= -1 && g < px->n_groups, "%s: prefix: sequence %d: group %d out of range [-1, %d)", who, b, g, px->n_groups);
     if (g < 0) continue;
     ++members[g];
     FO1_CHECK_ARG(px->prefix_lens[g] >= 1 && px->prefix_lens[g] < d->seq_lens[b],
-                  "fo1_llm_generate: prefix: sequence %d: prefix %d rows, length %d (1 <= P < L)", b, px->prefix_lens[g], d->seq_lens[b]);
+                  "%s: prefix: sequence %d: prefix %d rows, length %d (1 <= P < L)", who, b, px->prefix_lens[g], d->seq_lens[b]);
   }
   for (int g = 0; g < px->n_groups; ++g)
-    FO1_CHECK_ARG(members[g] >= 2, "fo1_llm_generate: prefix: group %d has %d member(s) (at least 2)", g, members[g]);
+    FO1_CHECK_ARG(members[g] >= 2, "%s: prefix: group %d has %d member(s) (at least 2)", who, g, members[g]);
   return FO1_OK;
 }
 
@@ -1218,6 +1233,131 @@ static int llm_generate(Model* m, fo1_generate_desc* d, cudaStream_t s) {
   if (g.mega_grid > 0 && d->max_new_tokens > 1) return decode_persistent(m, q, g, s);
   FO1_TRY(decode_per_kernel(m, q, g, s));
   return bmd ? beam_finalize(q.beam, s) : FO1_OK;
+}
+
+// -------------------------------------------------------------------------------- teacher-forced scoring
+// the generate descriptor of a scoring call's prefill (no decoding), and every host check of include/fo1.h, before anything is enqueued
+static int loglik_check(Model* m, const fo1_loglik_desc* d, fo1_generate_desc* gd, const fo1_prefix_desc** px_out) {
+  FO1_CHECK_ARG(d->n_seqs > 0 && d->seq_lens && d->inputs_embeds && d->position_ids && d->targets, "fo1_llm_loglik: null argument");
+  FO1_CHECK_ARG(d->logprobs && d->seq_logprob && d->seq_count, "fo1_llm_loglik: null output (logprobs, seq_logprob and seq_count are required)");
+  *gd = fo1_generate_desc{};
+  gd->n_seqs = d->n_seqs; gd->seq_lens = d->seq_lens; gd->inputs_embeds = d->inputs_embeds; gd->position_ids = d->position_ids;
+  gd->all_logits = d->all_logits;
+  const fo1_prefix_desc* px = d->prefix != nullptr && d->prefix->n_groups > 0 ? d->prefix : nullptr;
+  for (int b = 0; b < d->n_seqs; ++b) FO1_CHECK_ARG(d->seq_lens[b] > 0, "fo1_llm_loglik: sequence %d is empty", b);
+  if (px) FO1_TRY(prefix_check(gd, px, "fo1_llm_loglik"));
+  const int V = m->cfg.llm_vocab;
+  long long r = 0;
+  for (int b = 0; b < d->n_seqs; ++b) {
+    const int L = d->seq_lens[b], P = prefix_of(px, b);
+    for (int t = 0; t < L; ++t, ++r) {
+      const int tg = d->targets[r];
+      if (tg == -100) continue;
+      FO1_CHECK_ARG(tg >= 0 && tg < V, "fo1_llm_loglik: sequence %d row %d: target %d is outside [0, %d) and not -100", b, t, tg, V);
+      FO1_CHECK_ARG(t < L - 1, "fo1_llm_loglik: sequence %d: its last row (%d) is scored; it has no next token", b, t);
+      FO1_CHECK_ARG(t >= P, "fo1_llm_loglik: sequence %d row %d is scored inside its shared prefix of %d rows", b, t, P);
+    }
+  }
+  FO1_CHECK_ARG(m->slot_pool == nullptr, "fo1_llm_loglik: a slot pool is open on this model (it owns the K/V cache); fo1_slots_close first");
+  *px_out = px;
+  return FO1_OK;
+}
+
+// the prefill of fo1_llm_generate (prefill_plan, prefill_layers), then the scored rows only: gathered, normed with the all_logits
+// path's kernel, the log-likelihood head and the merge; `dry` sizes the arena
+static int llm_loglik_run(Model* m, const fo1_loglik_desc* ld, GenerateCall& q, const std::vector<int>& ints, int n_scored, cudaStream_t s,
+                          bool dry) {
+  const fo1_model_config& c = m->cfg;
+  Arena& A = m->arena;
+  const fo1_generate_desc* d = q.d;
+  const fo1_prefix_desc* px = q.px;
+  const int B = d->n_seqs, H = c.llm_hidden, hd = c.llm_head_dim, V = c.llm_vocab, Ms = n_scored;
+  const int n_parts = ceil_div(V, kLoglikTile);
+  long long T = 0, rows = 0;
+  int n_pre = 0;
+  for (int b = 0; b < B; ++b) { T += d->seq_lens[b] - prefix_of(px, b); rows += d->seq_lens[b]; }
+  for (int gi = 0; px && gi < px->n_groups; ++gi) n_pre += px->prefix_lens[gi];
+  T += n_pre;
+  DecodeBufs g{};
+  decode_bufs_alloc(m, g, (int)T, 1, B);
+  float* cs_pre = A.alloc<float>((size_t)T * hd);
+  g.layer.rowseg = A.alloc<int>((size_t)T * 2);
+  int* d_lens = A.alloc<int>(B);
+  int* pos_all = px ? A.alloc<int>((size_t)3 * T) : nullptr;
+  bf16* alln = d->all_logits ? A.alloc<bf16>((size_t)T * H) : nullptr;
+  bf16* xs = A.alloc<bf16>((size_t)std::max(Ms, 1) * H);
+  bf16* xn = A.alloc<bf16>((size_t)std::max(Ms, 1) * H);
+  float4* part = A.alloc<float4>((size_t)std::max(Ms, 1) * n_parts);
+  float* xt = A.alloc<float>(std::max(Ms, 1));
+  int* di = A.alloc<int>(ints.size());     // packed rows [Ms], full rows [Ms], targets [Ms], sequence offsets [B + 1], counts [B]
+  const int *d_pack = di, *d_full = di + Ms, *d_tgt = di + 2 * Ms, *d_off = di + 3 * Ms, *d_cnt = di + 3 * Ms + B + 1;
+  PrefillAttn pa = {};
+  const int* d_last = nullptr;
+  if (!dry) {
+    FO1_TRY(prefill_plan(m, q, g.layer, (int)T, pa, &d_last, s));
+    FO1_CUDA(cudaMemcpyAsync(d_lens, d->seq_lens, B * sizeof(int), cudaMemcpyHostToDevice, s));
+    FO1_CUDA(cudaMemcpyAsync(di, ints.data(), ints.size() * sizeof(int), cudaMemcpyHostToDevice, s));   // (pageable: returns once staged)
+  }
+  const bf16* x = nullptr;
+  FO1_TRY(prefill_layers(m, q, pa, g, T, n_pre, cs_pre, pos_all, d_lens, s, dry, &x));
+  if (d->all_logits) {
+    FO1_RUN(rmsnorm(x, H, m->llm.norm, alln, H, (int)T, H, c.rms_eps, NORM_WARP, s));
+    FO1_RUN(linear(alln, H, m->llm.lm_head, H, d->all_logits, V, FO1_F32, (int)T, V, H, nullptr, 0, FO1_EPI_NONE, nullptr, 0, 0, s));
+  }
+  if (dry) return FO1_OK;
+  FO1_CUDA(cudaMemsetAsync(ld->logprobs, 0, (size_t)rows * sizeof(float), s));
+  if (ld->greedy) FO1_CUDA(cudaMemsetAsync(ld->greedy, 0, (size_t)rows * sizeof(int), s));
+  if (Ms > 0) {
+    FO1_TRY(gather_rows_bf16(x, H, d_pack, xs, H, Ms, H, s));
+    FO1_TRY(rmsnorm(xs, H, m->llm.norm, xn, H, Ms, H, c.rms_eps, NORM_WARP, s));   // the all_logits rows' kernel: the same bits
+    FO1_TRY(loglik_head(xn, m->llm.lm_head, Ms, V, H, d_tgt, part, xt, s));
+    FO1_TRY(loglik_merge(part, n_parts, Ms, d_tgt, xt, d_full, ld->logprobs, ld->greedy, ld->lse, ld->target_logits, s));
+  }
+  FO1_TRY(loglik_seq_sum(ld->logprobs, d_off, B, ld->seq_logprob, s));
+  FO1_CUDA(cudaMemcpyAsync(ld->seq_count, d_cnt, B * sizeof(int), cudaMemcpyDeviceToDevice, s));
+  return FO1_OK;
+}
+
+static int llm_loglik(Model* m, const fo1_loglik_desc* ld, cudaStream_t s) {
+  fo1_generate_desc gd;
+  GenerateCall q{};
+  FO1_TRY(loglik_check(m, ld, &gd, &q.px));
+  q.d = &gd;
+  FO1_CHECK_ARG(m->llm.ok, "fo1_llm_loglik: model not finalized (LLM weights unresolved)");
+  const fo1_model_config& c = m->cfg;
+  FO1_CHECK_ARG(c.llm_head_dim == 128, "fo1_llm_loglik: head_dim %d unsupported (128)", c.llm_head_dim);
+  const int B = gd.n_seqs;
+  // scored rows in row order: their packed row (prefix rows first with a shared prefix), their row over the full sequences, target
+  std::vector<int> pack, full, tgt, off(1, 0), cnt(B, 0);
+  int n_pre = 0, max_len = 0;
+  for (int gi = 0; q.px && gi < q.px->n_groups; ++gi) n_pre += q.px->prefix_lens[gi];
+  int own0 = n_pre;
+  for (int b = 0; b < B; ++b) {
+    const int L = gd.seq_lens[b], P = prefix_of(q.px, b);
+    max_len = std::max(max_len, L);
+    for (int t = 0; t < L; ++t) {
+      const int r = off.back() + t;
+      if (ld->targets[r] == -100) continue;
+      pack.push_back(q.px ? own0 + t - P : r); full.push_back(r); tgt.push_back(ld->targets[r]);
+      ++cnt[b];
+    }
+    own0 += L - P;
+    off.push_back(off.back() + L);
+  }
+  const int Ms = (int)pack.size();
+  std::vector<int> ints(pack);
+  ints.insert(ints.end(), full.begin(), full.end());
+  ints.insert(ints.end(), tgt.begin(), tgt.end());
+  ints.insert(ints.end(), off.begin(), off.end());
+  ints.insert(ints.end(), cnt.begin(), cnt.end());
+  // the cache the prefill of fo1_llm_generate with max_new_tokens 0 uses (a shared prefix rounds the slot up to 64 rows)
+  FO1_TRY(ensure_kv(m, B, q.px ? (max_len + 1 + 63) / 64 * 64 : max_len + 1));
+  FO1_TRY(int_cache_trim(m));
+  m->arena.reset(true);
+  FO1_TRY(llm_loglik_run(m, ld, q, ints, Ms, s, true));
+  FO1_TRY(arena_ensure(m, m->arena.peak));
+  m->arena.reset(false);
+  return llm_loglik_run(m, ld, q, ints, Ms, s, false);
 }
 
 // -------------------------------------------------------------------------------- slot pool
@@ -1581,6 +1721,11 @@ extern "C" int fo1_llm_build_embeds(fo1_model* m, const int32_t* src_kind, const
 extern "C" int fo1_llm_generate(fo1_model* m, fo1_generate_desc* d, void* stream) {
   FO1_CHECK_ARG(m && d, "fo1_llm_generate: null argument");
   return llm_generate(m, d, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int fo1_llm_loglik(fo1_model* m, const fo1_loglik_desc* d, void* stream) {
+  FO1_CHECK_ARG(m && d, "fo1_llm_loglik: null argument");
+  return llm_loglik(m, d, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int fo1_slots_open(fo1_model* m, const fo1_slots_desc* o, void* stream) {

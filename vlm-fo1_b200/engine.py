@@ -546,6 +546,65 @@ def _engine_generate(self, inputs_embeds: torch.Tensor, position_ids: torch.Tens
     return out
 
 
+IGNORE_INDEX = -100
+
+
+def _engine_loglik(self, inputs_embeds: torch.Tensor, position_ids: torch.Tensor, seq_lens: Sequence[int], targets,
+                   prefix: Optional[Prefix] = None, want_greedy: bool = False, want_all_logits: bool = False, want_lse: bool = False):
+    """Teacher-forced scoring of a packed batch (fo1_llm_loglik): the prefill of generate, then the log-likelihood of each scored
+    row's target from the LM head, without a vocabulary-wide matrix.  ``targets``: int [sum L] over the rows of the full sequences
+    (HF labels already shifted by one within each sequence), -100 = not scored; a host sequence or a tensor (copied to the host).
+    ``prefix``: as generate's (``inputs_embeds`` / ``position_ids`` then hold each sequence's own rows only).  Returns a dict of device
+    tensors: ``logprobs`` fp32 [sum L] (0 where not scored), ``seq_logprob`` fp64 [B], ``seq_count`` int32 [B]; with ``want_greedy``
+    ``greedy`` int32 [sum L] (1: the target is the row's lowest-index maximum); with ``want_all_logits`` ``all_logits`` fp32 [sum L, V]
+    (refused with a prefix); with ``want_lse`` ``lse`` / ``target_logits`` fp32 [n_scored] of the scored rows in row order."""
+    import numpy as np
+    B = len(seq_lens)
+    pre = [0] * B
+    if prefix is not None:
+        assert len(prefix.seq_group) == B, "one group index per sequence"
+        pre = [int(prefix.lens[g]) if g >= 0 else 0 for g in prefix.seq_group]
+    rows = int(sum(int(x) for x in seq_lens))
+    T = rows - sum(pre)
+    assert inputs_embeds.shape == (T, self.cfg.llm["hidden_size"]) and inputs_embeds.dtype == torch.bfloat16
+    inputs_embeds = inputs_embeds.contiguous()
+    position_ids = position_ids.to(self.device, torch.int32).contiguous()
+    assert position_ids.shape == (3, T)
+    tg = np.ascontiguousarray(targets.cpu().numpy() if isinstance(targets, torch.Tensor) else np.asarray(targets), dtype=np.int32)
+    assert tg.shape == (rows,), "one target per row of the full sequences"
+    n_scored = int((tg != IGNORE_INDEX).sum())
+    V = self.cfg.llm["vocab_size"]
+    dev = self.device
+    out = dict(logprobs=torch.empty(rows, dtype=torch.float32, device=dev), seq_logprob=torch.empty(B, dtype=torch.float64, device=dev),
+               seq_count=torch.empty(B, dtype=torch.int32, device=dev))
+    if want_greedy:
+        out["greedy"] = torch.empty(rows, dtype=torch.int32, device=dev)
+    if want_all_logits:
+        out["all_logits"] = torch.empty((rows, V), dtype=torch.float32, device=dev)
+    if want_lse:
+        out["lse"] = torch.empty(max(n_scored, 1), dtype=torch.float32, device=dev)[:n_scored]
+        out["target_logits"] = torch.empty(max(n_scored, 1), dtype=torch.float32, device=dev)[:n_scored]
+    ptr = lambda k: out[k].data_ptr() if k in out else None
+    d = _lib.LoglikDesc()
+    d.n_seqs = B
+    d.seq_lens = (C.c_int32 * B)(*[int(x) for x in seq_lens])
+    d.inputs_embeds, d.position_ids = inputs_embeds.data_ptr(), position_ids.data_ptr()
+    d.targets = tg.ctypes.data_as(C.POINTER(C.c_int32))
+    d.logprobs, d.greedy, d.seq_logprob, d.seq_count = ptr("logprobs"), ptr("greedy"), ptr("seq_logprob"), ptr("seq_count")
+    d.all_logits, d.lse, d.target_logits = ptr("all_logits"), ptr("lse"), ptr("target_logits")
+    if prefix is not None:
+        G = len(prefix.lens)
+        pe = prefix.embeds.contiguous()
+        pp = prefix.position_ids.to(dev, torch.int32).contiguous()
+        assert pe.dtype == torch.bfloat16 and pe.shape == (sum(int(x) for x in prefix.lens), self.cfg.llm["hidden_size"])
+        assert pp.shape == (3, pe.shape[0])
+        px = _lib.PrefixDesc(G, (C.c_int32 * max(G, 1))(*[int(x) for x in prefix.lens]), pe.data_ptr(), pp.data_ptr(),
+                             (C.c_int32 * B)(*[int(g) for g in prefix.seq_group]))
+        d.prefix = C.pointer(px)
+    check(lib().fo1_llm_loglik(self._h, C.byref(d), _stream()), "fo1_llm_loglik")
+    return out
+
+
 class SlotPool:
     """In-flight batching over the engine (include/fo1.h, fo1_slots_*): ``n_slots`` K/V cache slots of ``cap`` rows and their decode
     state live across calls.  ``admit`` prefills requests into free slots, ``decode(exit_at)`` decodes every slot until at most
@@ -732,6 +791,7 @@ def _engine_run_streamed(self, launch, B: int, T: int, on_tokens) -> None:
 
 Engine.build_embeds = _engine_build_embeds
 Engine.generate = _engine_generate
+Engine.loglik = _engine_loglik
 Engine._stream_buffers = _engine_stream_buffers
 Engine._run_streamed = _engine_run_streamed
 Engine.sample_tokens = staticmethod(sample_tokens)

@@ -4,6 +4,7 @@
     encode_regions  (omchat_qwen2_5_vl.py:75-128)  -> Engine.davit_forward + fpn_forward + hfre_forward + region_project
     splice + M-RoPE (omchat_qwen2_5_vl.py:291-463) -> splice_plan (host ints) + Engine.build_embeds
     generate        (HF greedy loop)               -> Engine.generate (prefill + device-resident decode)
+    score           (forward(labels=...))          -> Engine.loglik  (prefill + log-likelihood head)
 
 One image per sample (what every caller in the reference does).  torch is the memory / stream plumbing."""
 from __future__ import annotations
@@ -93,6 +94,38 @@ def shared_prefix_groups(prompts: Sequence[Sequence[int]], rep: Sequence[int], i
         if P >= 1:
             out.append((mem, P))
     return out
+
+
+IGNORE_INDEX = -100
+
+
+def splice_labels(input_ids: Sequence[int], labels: Sequence[int], image_rows: int, image_placeholder: int = -200,
+                  region_placeholder: int = -300) -> List[int]:
+    """The labels of a sample's spliced rows, by the reference's rule (omchat_qwen2_5_vl.py:318-368): a text position keeps its label,
+    an image placeholder becomes ``image_rows`` rows labelled -100, a region placeholder one row labelled -100."""
+    assert len(labels) == len(input_ids), "one label per input id"
+    out: List[int] = []
+    for t, lab in zip(input_ids, labels):
+        if t == image_placeholder:
+            out += [IGNORE_INDEX] * image_rows
+        elif t == region_placeholder:
+            out.append(IGNORE_INDEX)
+        else:
+            out.append(int(lab))
+    return out
+
+
+def shift_targets(spliced_labels: Sequence[int]) -> List[int]:
+    """HF's ForCausalLMLoss shift within one sequence: row t predicts label t + 1; the last row predicts nothing (-100)."""
+    return [int(x) for x in spliced_labels[1:]] + [IGNORE_INDEX]
+
+
+def causal_lm_loss(seq_logprob: Sequence[float], seq_count: Sequence[int]) -> float:
+    """ForCausalLMLoss (reduction 'mean' over every non-ignored shifted label of the batch) from per-sequence sums of the targets'
+    log-probabilities and their counts: -sum / count, NaN when nothing is scored (torch's 0 / 0)."""
+    n = int(sum(int(c) for c in seq_count))
+    tot = float(sum(float(x) for x in seq_logprob))
+    return -tot / n if n > 0 else float("nan")
 
 
 def refill_need(n_slots: int, n_waiting: int) -> int:
@@ -356,24 +389,7 @@ class Fo1Pipeline:
         regions = torch.cat(region_tokens, 0)
         # beam search prefills each prompt once in full (its K/V goes to its N slots); only the towers are shared
         groups = shared_prefix_groups(prompts, rep, [gh * gw // (merge * merge) for gh, gw in grids], lens) if beams is None else []
-        prefix = None
-        if not groups:
-            embeds, pos = eng.build_embeds(plan["kind"], plan["index"], feats, regions), plan["position_ids"]
-        else:
-            start = np.cumsum([0] + list(lens))
-            seq_group, pre = [-1] * B, [0] * B
-            sel = []
-            for g, (mem, P) in enumerate(groups):
-                sel.append(np.arange(start[mem[0]], start[mem[0]] + P))
-                for b in mem:
-                    seq_group[b], pre[b] = g, P
-            sel += [np.arange(start[b] + pre[b], start[b + 1]) for b in range(B)]
-            idx = torch.from_numpy(np.concatenate(sel).astype(np.int64)).to(dev, non_blocking=True)
-            n_pre = sum(P for _, P in groups)
-            emb = eng.build_embeds(plan["kind"][idx].contiguous(), plan["index"][idx].contiguous(), feats, regions)
-            pos_all = plan["position_ids"][:, idx]
-            prefix = Prefix([P for _, P in groups], emb[:n_pre], pos_all[:, :n_pre], seq_group)
-            embeds, pos = emb[n_pre:], pos_all[:, n_pre:]
+        embeds, pos, prefix = self._prefix_inputs(plan, lens, groups, feats, regions)
         self._mark("splice")
         out = eng.generate(embeds, pos, lens, plan["rope_delta"], max_new_tokens, stop_ids, pad_id, want_prefill_logits=want_prefill_logits,
                            early_exit_interval=early_exit_interval, sampling=sampling, want_logprobs=want_logprobs, want_scores=want_scores,
@@ -382,6 +398,74 @@ class Fo1Pipeline:
         self._mark("llm_prefill_decode")
         out["prompt_lens"] = lens
         return out
+
+    # ---- teacher-forced scoring -----------------------------------------------------------------------------
+    def score(self, samples: Sequence[SampleInputs], labels: Sequence[Sequence[int]], want_greedy: bool = False,
+              want_all_logits: bool = False, want_lse: bool = False) -> dict:
+        """The log-likelihood of each sample's labels (HF layout over its ``input_ids``, -100 ignored) under the model, teacher
+        forced, without decoding (Engine.loglik).  Labels are spliced as the reference splices them (splice_labels) and shifted within
+        each sample (shift_targets).  Samples with equal encoder inputs share the towers, and their common prompt prefix is prefilled
+        once, capped before the first scored row of every member: ranking K answers about one image is a score() of K samples that
+        differ only in the answer.  Every output is bit-identical to scoring each sample alone.  Returns Engine.loglik's dict plus
+        ``prompt_lens`` (spliced lengths) and ``targets`` (int32 numpy [sum L])."""
+        eng, dev = self.eng, self.eng.device
+        B = len(samples)
+        assert len(labels) == B, "one label list per sample"
+        rep = encoder_groups(samples) if self._share_inputs and B > 1 else list(range(B))
+        own = [b for b in range(B) if rep[b] == b]
+        slot = {b: i for i, b in enumerate(own)}
+        uniq = self.preprocess([samples[b] for b in own])
+        feats, _, region_tokens, _ = self.encode(uniq)
+        merge = eng.cfg.vit["spatial_merge_size"]
+        grids = [uniq[slot[rep[b]]].grid_hw for b in range(B)]
+        prompts = [list(samples[b].input_ids) for b in range(B)]
+        plan = splice_plan_batch(prompts, [[g] for g in grids], [region_tokens[slot[rep[b]]].shape[0] for b in range(B)], dev, merge=merge,
+                                 row_src=rep, **self.ids)
+        lens = plan["lens"]
+        st = plan["status"].cpu().tolist()
+        if any(st):
+            raise ValueError(f"fo1_splice_plan_batch: per-sample status {st} (placeholders and features disagree)")
+        image_rows = [gh * gw // (merge * merge) for gh, gw in grids]
+        targets = []
+        for b in range(B):
+            sl = splice_labels(prompts[b], labels[b], image_rows[b])
+            assert len(sl) == lens[b], f"sample {b}: {len(sl)} spliced labels for {lens[b]} rows"
+            targets.append(shift_targets(sl))
+        regions = torch.cat(region_tokens, 0)
+        groups = shared_prefix_groups(prompts, rep, image_rows, lens) if self._share_inputs and not want_all_logits else []
+        first = [next((t for t, x in enumerate(tg) if x != IGNORE_INDEX), len(tg)) for tg in targets]
+        groups = [(mem, min(P, min(first[b] for b in mem))) for mem, P in groups]     # no scored row inside a prefix
+        groups = [(mem, P) for mem, P in groups if P >= 1]
+        embeds, pos, prefix = self._prefix_inputs(plan, lens, groups, feats, regions)
+        self._mark("splice")
+        tg = np.asarray([x for t in targets for x in t], dtype=np.int32)
+        out = eng.loglik(embeds, pos, lens, tg, prefix=prefix, want_greedy=want_greedy, want_all_logits=want_all_logits, want_lse=want_lse)
+        self._mark("llm_loglik")
+        out["prompt_lens"] = lens
+        out["targets"] = tg
+        out["rope_delta"] = plan["rope_delta"]
+        return out
+
+    def _prefix_inputs(self, plan, lens, groups, feats, regions):
+        """-> (embeds, position_ids, Prefix or None) of a spliced batch with the shared-prefix ``groups`` [(members, P)]: the groups'
+        prefix rows once, then every sequence's own rows."""
+        eng, dev = self.eng, self.eng.device
+        if not groups:
+            return eng.build_embeds(plan["kind"], plan["index"], feats, regions), plan["position_ids"], None
+        B = len(lens)
+        start = np.cumsum([0] + list(lens))
+        seq_group, pre = [-1] * B, [0] * B
+        sel = []
+        for g, (mem, P) in enumerate(groups):
+            sel.append(np.arange(start[mem[0]], start[mem[0]] + P))
+            for b in mem:
+                seq_group[b], pre[b] = g, P
+        sel += [np.arange(start[b] + pre[b], start[b + 1]) for b in range(B)]
+        idx = torch.from_numpy(np.concatenate(sel).astype(np.int64)).to(dev, non_blocking=True)
+        n_pre = sum(P for _, P in groups)
+        emb = eng.build_embeds(plan["kind"][idx].contiguous(), plan["index"][idx].contiguous(), feats, regions)
+        pos_all = plan["position_ids"][:, idx]
+        return emb[n_pre:], pos_all[:, n_pre:], Prefix([P for _, P in groups], emb[:n_pre], pos_all[:, :n_pre], seq_group)
 
     # ---- in-flight batching ---------------------------------------------------------------------------------
     def prompt_rows(self, s: SampleInputs, image_placeholder: int = -200) -> int:

@@ -453,6 +453,76 @@ class Fo1ForCausalLM:
             inputs = batch[i]["inputs"]
             yield i, torch.cat([inputs[0].to(tokens.device), tokens.to(torch.long)]).unsqueeze(0)
 
+    # ---- teacher-forced scoring (the reference's forward(labels=...), omchat_qwen2_5_vl.py:466-532) ----
+    def _score_sample(self, input_ids, images, images_aux, image_grid_thws, bbox_list, labels):
+        """(SampleInputs, label list) of one forward-style call; labels None: nothing scored."""
+        sample, _, _ = self._sample(input_ids, images, images_aux, image_grid_thws, bbox_list)
+        if labels is None:
+            lab = [-100] * len(sample.input_ids)
+        else:
+            labels = torch.as_tensor(labels)
+            if labels.dim() == 2:
+                if labels.shape[0] != 1:
+                    raise ValueError("labels must be [1, P] like input_ids (the reference runs one sample per call)")
+                labels = labels[0]
+            lab = [int(x) for x in labels.tolist()]
+            if len(lab) != len(sample.input_ids):
+                raise ValueError(f"labels has {len(lab)} positions, input_ids {len(sample.input_ids)}")
+        return sample, lab
+
+    @torch.no_grad()
+    def forward(self, input_ids=None, images=None, images_aux=None, image_grid_thws=None, bbox_list=None, labels=None, attention_mask=None,
+                position_ids=None, past_key_values=None, inputs_embeds=None, use_cache=None, output_attentions=None,
+                output_hidden_states=None, return_dict=None, **kwargs):
+        """The reference's forward for one sample: -> transformers' Qwen2_5_VLCausalLMOutputWithPast with ``logits`` fp32 [1, L, V] at
+        every spliced position (the engine's all_logits), ``loss`` HF's ForCausalLMLoss over ``labels`` (the mean over every
+        non-ignored shifted label, NaN when none is; None without labels) from the device's per-token log-likelihoods,
+        ``rope_deltas`` [1, 1] and ``past_key_values`` None.  No K/V cache in or out, attentions, hidden states or tuple returns."""
+        if past_key_values is not None:
+            raise NotImplementedError("forward with past_key_values is not supported by the fo1-b200 engine (its K/V cache stays inside it)")
+        if inputs_embeds is not None:
+            raise NotImplementedError("forward with inputs_embeds is not supported by the fo1-b200 engine (it splices input_ids itself)")
+        for name, v in (("output_attentions", output_attentions), ("output_hidden_states", output_hidden_states)):
+            if v:
+                raise NotImplementedError(f"{name}=True is not supported by the fo1-b200 engine's forward (it returns loss and logits)")
+        if return_dict is False:
+            raise NotImplementedError("return_dict=False is not supported by the fo1-b200 engine's forward (it returns the output dataclass)")
+        if attention_mask is not None and not bool(torch.as_tensor(attention_mask).bool().all()):
+            raise NotImplementedError("a padded attention_mask is not supported by the fo1-b200 engine's forward (one unpadded sample)")
+        sample, lab = self._score_sample(input_ids, images, images_aux, image_grid_thws, bbox_list, labels)
+        out = self.pipeline.score([sample], [lab], want_all_logits=True)
+        from transformers.models.qwen2_5_vl.modeling_qwen2_5_vl import Qwen2_5_VLCausalLMOutputWithPast
+        loss = None
+        if labels is not None:
+            loss = (-out["seq_logprob"].sum() / out["seq_count"].sum().to(torch.float64)).to(torch.float32)
+        return Qwen2_5_VLCausalLMOutputWithPast(loss=loss, logits=out["all_logits"].unsqueeze(0), past_key_values=None,
+                                                rope_deltas=out["rope_delta"].to(torch.long).view(1, 1))
+
+    __call__ = forward
+
+    @torch.no_grad()
+    def score_batch(self, batch, labels):
+        """Scoring of many samples in ONE engine call without any logits matrix (what ``generate_batch`` is for ``generate``).
+        ``batch``: the dicts ``prepare_inputs`` returns; ``labels[b]``: [1, P_b] or a list over sample b's input_ids (-100 ignored).
+        Samples about the same image share the towers and their common prompt prefix.  -> per sample a dict: ``loss`` (fp32 scalar,
+        forward's loss), ``logprobs`` fp32 [n_b] (the log-probability of each non-ignored shifted label, in order) and ``greedy``
+        int32 [n_b] (1 where that label is the arg-max)."""
+        if len(labels) != len(batch):
+            raise ValueError("one label sequence per sample")
+        keys = ("inputs", "images", "images_aux", "image_grid_thws", "bbox_list")
+        pairs = [self._score_sample(*(kw.get(k) for k in keys), lab) for kw, lab in zip(batch, labels)]
+        out = self.pipeline.score([p[0] for p in pairs], [p[1] for p in pairs], want_greedy=True)
+        scored = torch.from_numpy(out["targets"] != -100)
+        off = [0]
+        for n in out["prompt_lens"]:
+            off.append(off[-1] + n)
+        res = []
+        for b in range(len(batch)):
+            sel = torch.nonzero(scored[off[b]:off[b + 1]]).view(-1).to(out["logprobs"].device) + off[b]
+            loss = (-out["seq_logprob"][b] / out["seq_count"][b].to(torch.float64)).to(torch.float32)
+            res.append(dict(loss=loss, logprobs=out["logprobs"][sel], greedy=out["greedy"][sel]))
+        return res
+
     def _generate_batch_beams(self, batch, beams, wants, max_new_tokens, output_logprobs):
         """generate_batch of beam-search samples: one packed engine call when every sample asks for the same beam setting.  With
         ``output_logprobs`` each element carries fp32 [num_return, T], the returned tokens' log-probabilities gathered along their
